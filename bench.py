@@ -13,19 +13,19 @@ tower (dim 768, 12 layers, 12 heads, 224 px / patch 16, reference-default visual
 + 12-layer text tower (dim 512, 77 tokens), dim_latent 512, plain InfoNCE, 4096 pairs per GPU
 (global batch 4096*N: 32768 at N = 8, weak scaling, negatives all-gathered across ranks), encoder
 micro-batch 768 (GradCache-style step, engine.ChunkedClipLossFn: 4096 pairs of ViT-B/16 activations are
-~260 GB; the chunks that fit the 180 GB of HBM keep their activations, the rest is re-encoded in backward;
+~260 GB; the chunks that fit the 80 GB of HBM keep their activations, the rest is re-encoded in backward;
 the reference's own answer is activation checkpointing).
 
 One JSON line on rank 0:
   value        pairs/s with the batch already on the device
   e2e          the same step through the public CLIP.forward with the batch copied from pinned
                host memory inside the timed region (double buffered, side stream) + loss read-back
-  roofline     the dominant kernel family (tcgen05 GEMM) measured live with CUDA events around every
+  roofline     the dominant kernel family (wgmma GEMM) measured live with CUDA events around every
                C-ABI call in one instrumented step, plus `attention` and `logits` sub-objects (the
                kernels the north star names): tensor-pipe fraction AND achieved HBM GB/s
   cpu_baseline the UNMODIFIED reference (oracle/_ref, pip-installed from /root/reference) on the
                host cores, bounded sample of the same model; `gpu_eager_baseline`: the unmodified
-               reference module on this B200 in eager PyTorch (fp32 and bf16 autocast)
+               reference module on this GPU in eager PyTorch (fp32 and bf16 autocast)
   other_workloads  short measurements of cfg2 (README model, 1024/GPU), cfg4 (FILIP, 256/GPU) and
                cfg5 (DCL + extra projections, 8192/GPU) on the same N GPUs
   multirank_parity (N > 1) per-rank loss / grad-norm / d temperature of a tiny sharded step against
@@ -93,6 +93,8 @@ def parse():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip the cfg2 / cfg4 / cfg5 side measurements")
     ap.add_argument("--no-parity", action="store_true", help="skip the N>1 per-rank parity check")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write what the last timed step computed (loss, sampled gradients) as DIR/<name>.npy")
     a = ap.parse_args()
     a.retain = a.retain if a.retain == "auto" else int(a.retain)
     d = DEFAULTS[a.workload]
@@ -397,7 +399,7 @@ def gpu_eager_baseline(model_cfg, loss_kw, patch_dropout, dev, batch=256):
     g = torch.Generator(device=dev).manual_seed(3)
     text = torch.randint(0, model_cfg["num_text_tokens"], (batch, model_cfg["text_seq_len"]), generator=g, device=dev)
     image = torch.randn(batch, 3, model_cfg["visual_image_size"], model_cfg["visual_image_size"], generator=g, device=dev)
-    out = {"batch": batch, "what": "unmodified reference x_clip.CLIP (oracle/_ref), eager PyTorch on this B200, "
+    out = {"batch": batch, "what": "unmodified reference x_clip.CLIP (oracle/_ref), eager PyTorch on this GPU, "
                                    "fwd+bwd, same model / patch dropout as the headline"}
 
     def run(autocast):
@@ -431,6 +433,26 @@ def gpu_eager_baseline(model_cfg, loss_kw, patch_dropout, dev, batch=256):
 
 
 # --------------------------------------------------------------------------- GPU arm
+
+def dump_outputs(out_dir, run, loss):
+    """What the last timed step handed its caller: loss.npy (float64) and, per parameter, the gradient
+    as grad.<name>.npy (float32), sampled at 4096 fixed, seeded positions when it is larger (a few MB
+    in all), so that two builds can be compared output for output."""
+    import numpy as np
+    import torch
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    np.save(d / "loss.npy", np.asarray([loss.item()], dtype=np.float64))
+    g = torch.Generator().manual_seed(0)
+    for name, p in run.clip.named_parameters():
+        if p.grad is None:
+            continue
+        flat = p.grad.detach().reshape(-1)
+        if flat.numel() > 4096:
+            idx = torch.randint(0, flat.numel(), (4096,), generator=g)
+            flat = flat[idx.to(flat.device)]
+        np.save(d / f"grad.{name}.npy", flat.float().cpu().numpy())
+
 
 def main():
     args = parse()
@@ -503,6 +525,8 @@ def main():
     peak_mem = torch.cuda.max_memory_allocated(dev)
     clocks = sampler.stop() if rank == 0 else None
     note(f"device-resident timing done: {ms_dev / args.steps:.1f} ms/step")
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, run, loss)
 
     # ---- (2) end-to-end: pinned host -> device copy of every step's batch (side stream, double
     #          buffered) + loss read-back, all inside the timed region
@@ -610,11 +634,11 @@ def main():
     pk = ROOT / "MEASURED_PEAKS.json"
     if pk.exists():
         peaks = json.loads(pk.read_text())
-    peak_tf = peaks.get("bf16_tflops_sustained") or 1400.0
-    peak_burst = peaks.get("bf16_tflops") or 1640.0
-    peak_hbm = peaks.get("hbm_gbs") or 6500.0
+    peak_tf = peaks.get("bf16_tflops_sustained") or 989.0
+    peak_burst = peaks.get("bf16_tflops") or 989.0
+    peak_hbm = peaks.get("hbm_gbs") or 3350.0
     peak_src = ("MEASURED_PEAKS.json (bf16_tflops_sustained for kernels inside the step, hbm_gbs)" if peaks
-                else "fallback 1.4 PF sustained / 6.5 TB/s (B200_PROFILING.md)")
+                else "H100 SXM data sheet: 989 TFLOP/s dense bf16, 3.35 TB/s HBM3 (700 W); not reached")
 
     roofline, families = None, None
     if prof:
@@ -628,18 +652,11 @@ def main():
         g_fl = sum(d["flops"] for d in gem)
         g_calls = sum(d["calls"] for d in gem)
         achieved = g_fl / g_ms / 1e9
-        traffic = None
-        tf = ROOT / "profiles" / "gemm_traffic.json"
-        if tf.exists():
-            ratio = json.loads(tf.read_text()).get("traffic_over_algorithmic")
-            if ratio:
-                traffic = round(ratio * sum(d["bytes"] for d in gem) / g_calls)
-        roofline = {"kernel": "gemm_pair_kernel / gemm_bf16_kernel (tcgen05, plain-epilogue fwd+dgrad+wgrad launches; "
+        roofline = {"kernel": "gemm_bf16_kernel (wgmma, plain-epilogue fwd+dgrad+wgrad launches; "
                               "the fused feed-forward GEMMs are listed under feed_forward_fused)",
                     "bound": "tensor", "achieved": round(achieved, 1), "peak": peak_tf,
                     "unit": "TFLOP/s", "frac": round(achieved / peak_tf, 4),
-                    "frac_of_burst_peak": round(achieved / peak_burst, 4), "traffic": traffic,
-                    "traffic_note": "ncu dram bytes / algorithmic bytes ratio (profiles/gemm_traffic.json) x live algorithmic bytes per launch",
+                    "frac_of_burst_peak": round(achieved / peak_burst, 4),
                     "peak_source": peak_src, "launches_per_step": g_calls,
                     "avg_launch_ms": round(g_ms / g_calls, 4),
                     "flops_per_launch": g_fl / g_calls,
@@ -660,19 +677,19 @@ def main():
                     "hbm_frac_of_peak": round(fh, 4), "bound": "hbm" if fh > ft else "tensor",
                     "frac": round(max(ft, fh), 4), "note": note_txt}
         roofline["feed_forward_fused"] = {
-            "up": sub(["ff_up"], "gemm_pair_kernel<PEPI_FF_UP> (up-projection GEMM + GEGLU epilogue)",
+            "up": sub(["ff_up"], "gemm_bf16_kernel<EPI_FF_UP> (up-projection GEMM + GEGLU epilogue)",
                       "flops = the GEMM only (2*M*8d*d); the epilogue also evaluates 4d GELUs per token and writes "
                       "u (8d, skipped in forward-only sweeps) + hp (4d)"),
-            "down": sub(["ff_down"], "gemm_pair_kernel<PEPI_FF_DOWN> (down-projection GEMM + LayerNorm fold + residual)",
+            "down": sub(["ff_down"], "gemm_bf16_kernel<EPI_FF_DOWN> (down-projection GEMM + LayerNorm fold + residual)",
                         "flops = the GEMM only (2*M*4d*d)"),
-            "bwd": sub(["ff_bwd"], "gemm_pair_kernel<PEPI_FF_BWD2> (dgrad GEMM + LayerNorm/GEGLU backward epilogue, u by TMA one and a half steps ahead)",
+            "bwd": sub(["ff_bwd"], "gemm_bf16_kernel<EPI_FF_BWD> (dgrad GEMM + LayerNorm/GEGLU backward epilogue)",
                        "flops = the GEMM only (2*M*4d*d); reads u 8d, writes du 8d: HBM-bound by design")}
         roofline["attention"] = {
-            "fwd": sub(["attn_fwd"], "attn_fwd_small_kernel / attn_fwd_wg_kernel",
+            "fwd": sub(["attn_fwd"], "attn_fwd_kernel",
                        "algorithmic: 4 n^2 64 flops and q,k,v read + o write per (batch, head); at n = 98 / 78 "
-                       "(cfg3) the arithmetic intensity is n/2 ~ 40-50 flop/B, below the B200 ridge (~250): "
-                       "short-sequence attention is HBM-bound, 40 % of the tensor peak is not reachable"),
-            "bwd": sub(["attn_bwd"], "attn_delta_kernel + attn_bwd_small_kernel / attn_bwd_kernel",
+                       "(cfg3) the arithmetic intensity is n/2 ~ 40-50 flop/B, below the H100 ridge (~300): "
+                       "short-sequence attention is HBM-bound"),
+            "bwd": sub(["attn_bwd"], "attn_delta_kernel + attn_bwd_dkdv_kernel + attn_bwd_dq_kernel",
                        "algorithmic: 10 n^2 64 flops; q,k,v,o,dO read + dq,dk,dv write")}
         roofline["logits"] = {
             "fwd": sub(["nce_fwd"], "gemm_bf16_kernel<EPI_NCE_FWD> + nce_finalize_kernel",
@@ -702,7 +719,7 @@ def main():
                    "global_batch_at_8_gpus": B * 8,
                    "step_plan": plan, "peak_hbm_bytes_allocated": int(peak_mem),
                    "parallelism": f"dp{world}" + ("+grad-allreduce" if args.grad_sync and world > 1 else ""),
-                   "l2": "per-step working set (tens of GB of activations) >> 126 MB L2; no flush needed",
+                   "l2": "per-step working set (tens of GB of activations) >> 50 MB L2; no flush needed",
                    "timing": "CUDA events on the launching stream, barrier+synchronize both sides, max over ranks",
                    "loss": round(last_loss, 5)},
         "clocks": clocks,

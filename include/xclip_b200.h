@@ -1,5 +1,5 @@
 /*
- * xclip_b200.h - C-ABI of the B200-native CLIP training hot path.
+ * xclip_b200.h - C-ABI of the H100-native (sm_90a) CLIP training hot path.
  *
  * This is the drop-in boundary (SURVEY.md 8b): plain `extern "C"` entry points,
  * raw device pointers + explicit shapes, a cudaStream_t, int return codes.  The
@@ -29,7 +29,7 @@ extern "C" {
 #define XCLIP_OK 0
 #define XCLIP_ERR_INVALID 1      /* bad argument / unsupported shape */
 #define XCLIP_ERR_CUDA 2         /* CUDA runtime / driver error */
-#define XCLIP_ERR_UNSUPPORTED 3  /* device is not sm_100 */
+#define XCLIP_ERR_UNSUPPORTED 3  /* device is not sm_90 */
 
 #define XCLIP_MAJOR_K 0  /* operand stored with the contraction index contiguous */
 #define XCLIP_MAJOR_MN 1 /* operand stored transposed (its M / N index contiguous) */
@@ -39,26 +39,19 @@ typedef void* xclip_stream_t; /* cudaStream_t */
 /* ---- library ---------------------------------------------------------- */
 int xclip_abi_version(void);
 const char* xclip_last_error(void);
-/* Binds to the current CUDA device, checks it is sm_100, resolves the driver
+/* Binds to the current CUDA device, checks it is sm_90, resolves the driver
  * entry point used for TMA descriptors.  Idempotent. */
 int xclip_init(void);
 /* number of kernels this library has launched since the last reset (host counter) */
 long long xclip_launch_count(void);
 void xclip_launch_count_reset(void);
 /* Explicit, process-wide tuning switches for A/B measurements (never read from the environment;
- * results are identical either way).  Returns the previous value, -1 for an unknown knob.
- *   XCLIP_TUNE_FF_BWD_VARIANT (0): xclip_ff_bwd epilogue: 0 = u by ld.global -> st.shared per step,
- *                                  1 (default) = u by TMA one and a half steps ahead into one of three
- *                                  rotating box sets (0.346 -> 0.297 ms at [50176 x 768], bit-identical)
- *   XCLIP_TUNE_ATTN_SMALL_CTAS (1): resident CTAs per SM of the n <= 128 attention forward, 0 = built-in */
-#define XCLIP_TUNE_FF_BWD_VARIANT 0
-#define XCLIP_TUNE_ATTN_SMALL_CTAS 1
-#define XCLIP_TUNE_ATTN_SMALL_PREFETCH 2 /* n <= 128 attention: next item towards L2 by TMA prefetch (default 0) */
+ * results are identical either way).  Returns the previous value, -1 for an unknown knob. */
 #define XCLIP_TUNE_LN_FWD_BLOCKS 3 /* LayerNorm forward: cap on resident blocks per SM (0 = built-in 8) */
 #define XCLIP_TUNE_LN_BWD_BLOCKS 4 /* LayerNorm backward: blocks per SM (0 = built-in 2) */
 int xclip_tune_set(int knob, int value);
 
-/* ---- dense contraction (tcgen05) --------------------------------------
+/* ---- dense contraction (wgmma) ------------------------------------------
  * C[M,N] (+)= alpha * A * B^T (+ bias[N]) (+ residual[res_row_idx[row] | row % res_row_mod | row, N])
  * Replaces nn.Linear fwd + its autograd dgrad/wgrad:
  *   x_clip/x_clip.py:191,195 (FeedForward), :209,:210 (Attention to_qkv/to_out),
@@ -71,10 +64,6 @@ int xclip_tune_set(int knob, int value);
  * Requirements: N % 8 == 0, lda/ldb/ldr % 8 == 0, ldc % 8 == 0 (bf16) or % 4 (f32),
  * 16-byte aligned base pointers.  bias is f32, residual is bf16.
  */
-/* 256-wide problems run on CTA pairs (tcgen05 cta_group::2, 256 x 256 tiles) by default;
- * xclip_gemm_set_pair_mode(0) selects the single-CTA 128 x 256 kernel instead (returns the
- * previous setting).  Same results either way - a tuning / A-B switch, process-wide. */
-int xclip_gemm_set_pair_mode(int enabled);
 int xclip_gemm_bf16(const void* a, int64_t lda, int a_major, const void* b, int64_t ldb,
                     int b_major, void* c, int64_t ldc, int c_dtype, int M, int N, int K,
                     float alpha, const float* bias, const void* residual, int64_t ldr,
@@ -116,25 +105,23 @@ int xclip_l2norm_bwd(const float* dz, const float* z, const float* inv, void* dp
                      xclip_stream_t stream);
 int xclip_cast_f32_bf16(const float* src, void* dst, int64_t n, xclip_stream_t stream);
 
-/* ---- fused attention (tcgen05) -------------------------------------------
+/* ---- fused attention ------------------------------------------------------
  * Attention core of x_clip/x_clip.py:217-244 (dim_head = 64, n <= 320).  causal != 0 adds the
- * reference's causal mask (keys j > i get -FLT_MAX, :233-236); implemented for n <= 128.
+ * reference's causal mask (keys j > i get -FLT_MAX, :233-236).
  * qkv bf16 [B*n, ld_qkv] holds q | k | v, each heads*64 wide, head-major inside.
  * key_mask uint8 [B, n] (1 = attend; may be NULL).  o bf16 [B*n, ldo] (heads merged).
  * lse f32 [B, heads, n]: base-2 log-sum-exp of scale*log2(e)*scores (saved for backward). */
 int xclip_attn_fwd(const void* qkv, int64_t ld_qkv, const uint8_t* key_mask, void* o, int64_t ldo,
                    float* lse, int B, int n, int heads, float scale, int causal,
                    xclip_stream_t stream);
-/* delta f32 [B, heads, n] is scratch (rowsum(dO*O), written here).  dq_workspace f32
- * [B*n, heads*64] is required when n > 128 (partial dQ across key tiles), else may be NULL;
- * its contents are scratch too (with XCLIP_ATTN_TAIL=1 and n = 128k+1 the first three floats of a
- * token's 64-float slot also carry the tail-token scalars between the two backward kernels). */
+/* delta f32 [B, heads, n] is scratch (rowsum(dO*O), written here).  dq_workspace is not used
+ * (dQ is accumulated on chip) and may be NULL. */
 int xclip_attn_bwd(const void* qkv, int64_t ld_qkv, const uint8_t* key_mask, const void* o,
                    int64_t ldo, const void* d_o, int64_t lddo, const float* lse, float* delta,
                    void* dqkv, int64_t ld_dqkv, float* dq_workspace, int B, int n, int heads,
                    float scale, int causal, xclip_stream_t stream);
 
-/* ---- similarity + InfoNCE / DCL (tcgen05, logits never materialised in forward) ----------
+/* ---- similarity + InfoNCE / DCL (wgmma, logits never materialised in forward) ------------
  * Replaces x_clip/x_clip.py:813-847 for one direction of the loss:
  *   s[r,c] = *temp_exp * <a_r, b_c> (temp_exp: DEVICE scalar exp(temperature), so the host
  *   never synchronises on the parameter),  a bf16 [R,D] = LOCAL unit-norm latents of one modality,
@@ -199,10 +186,10 @@ int xclip_text_embed_fwd(const int64_t* ids, const float* tok, const float* pos,
 int xclip_text_embed_bwd(const int64_t* ids, const void* dx, float* dtok, float* dpos, float* dcls,
                          int B, int n, int d, int vocab, xclip_stream_t stream);
 
-/* ---- fused feed-forward block (x_clip/x_clip.py:180-199) on the CTA-pair GEMM ------------------
+/* ---- fused feed-forward block (x_clip/x_clip.py:180-199) on the wgmma GEMM ----------------------
  * FeedForward = Linear(d, 8d) -> GEGLU -> LayerNorm(4d) -> Linear(4d, d), + residual (:289).
- *   ff_permute_cast : bf16 copy of net.0.weight [8d, d] with rows reordered so that a 256-row tile
- *                     holds 128 value rows and the 128 MATCHING gate rows.
+ *   ff_permute_cast : bf16 copy of net.0.weight [8d, d] with rows reordered so that a 128-row tile
+ *                     holds 64 value rows and the 64 MATCHING gate rows.
  *   ff_scale_cast   : w2g = bf16(net.4.weight [d, 4d] * net.2.g [4d]) and colvec[j] = sum_k w2g[j,k].
  *   ff_up           : u = [value | gate] bf16 [M, 8d] (reference layout, kept for the backward),
  *                     hp = value * gelu_erf(gate) bf16 [M, 4d], rowsum[r, box] = (sum hp, sum hp^2) of

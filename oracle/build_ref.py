@@ -8,13 +8,14 @@ like the built libxclip_b200.so.  Users of the result:
 
   * bench.py `cpu_baseline` / `--impl reference`  - the reference's own CLIP.forward + backward on
     the host cores (kind "reference"), and `gpu_eager_baseline` - the same unmodified module on
-    the B200 in eager PyTorch (the only GPU path the reference has, SURVEY.md 8d);
+    the H100 in eager PyTorch (the only GPU path the reference has, SURVEY.md 8d);
   * tests/golden/make_golden.py imports the reference straight from /root/reference instead.
 
     python oracle/build_ref.py            # no-op when /root/reference is absent (GPU box)
 """
 from __future__ import annotations
 
+import os
 import shutil
 import subprocess
 import sys
@@ -30,11 +31,20 @@ def available() -> bool:
     return (DEST / "x_clip" / "x_clip.py").exists()
 
 
+def _source_readable() -> bool:
+    """The reference checkout exists and this user may read it (an unprivileged user may not even
+    see whether it exists)."""
+    try:
+        return (REF_SRC / "setup.py").is_file() and os.access(REF_SRC / "setup.py", os.R_OK)
+    except OSError:
+        return False
+
+
 def build(force: bool = False) -> bool:
     """Returns True when oracle/_ref holds the reference afterwards."""
     if available() and not force:
         return True
-    if not (REF_SRC / "setup.py").exists():
+    if not _source_readable():
         return available()
     with tempfile.TemporaryDirectory(prefix="xclip_ref_src_") as tmp:
         src = Path(tmp) / "src"

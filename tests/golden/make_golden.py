@@ -14,6 +14,7 @@ from __future__ import annotations
 
 import json
 import os
+import random
 import sys
 from pathlib import Path
 
@@ -100,7 +101,19 @@ def build_reference(x_clip, cfg_kwargs, patch_dropout, state):
     return clip
 
 
-def run_case(x_clip, name, cfg_kwargs, batch, pad_fraction, patch_dropout):
+def sample_positions(numel: int, n: int, seed: int) -> list:
+    """n fixed flat positions of a tensor with numel entries (a stride through it that depends on seed)."""
+    return [(seed * 7919 + j * 1000003) % numel for j in range(min(n, numel))]
+
+
+def sample(t: torch.Tensor, n: int, seed: int) -> list:
+    d = t.detach().flatten()
+    return d[sample_positions(d.numel(), n, seed)].tolist()
+
+
+def run_case(x_clip, name, cfg_kwargs, batch, pad_fraction, patch_dropout, samples=0):
+    """samples > 0 also records that many entries of every gradient (sample seed 0) and of both
+    encodings (seeds 1, 2) at the positions of sample_positions()."""
     cfg = O.ClipConfig(**cfg_kwargs)
     state = O.protocol_state_dict(cfg, WEIGHT_SEED)
     text, image = O.protocol_inputs(cfg, batch, INPUT_SEED, pad_fraction)
@@ -152,7 +165,68 @@ def run_case(x_clip, name, cfg_kwargs, batch, pad_fraction, patch_dropout):
     if not cfg.use_all_token_embeds:
         out["text_latents"] = lat[0].tolist()
         out["image_latents"] = lat[1].tolist()
+    if samples:
+        out["grad_samples"] = {k: sample(g, samples, 0) for k, g in grads.items()}
+        out["enc_text_sample"] = sample(enc_t, 2 * samples, 1)
+        out["enc_image_sample"] = sample(enc_i, 2 * samples, 2)
     return out
+
+
+RANDOM_SEEDS = range(16)
+
+
+def draw_random_case(seed: int):
+    """(cfg kwargs, batch, pad fraction, patch dropout) of random configuration `seed`: widths, head
+    counts, depths, sequence lengths, batch sizes, pad fractions, patch dropout and the loss flags."""
+    rng = random.Random(1000 + seed)
+    heads_t, heads_i = rng.choice([1, 2, 4]), rng.choice([1, 2, 4])
+    patch = rng.choice([8, 16])
+    side = patch * rng.choice([2, 3, 4])
+    cfg = dict(dim_text=64 * rng.choice([1, 2, 4]), dim_image=64 * rng.choice([1, 2, 4]),
+               dim_latent=64 * rng.choice([1, 2, 4]), num_text_tokens=rng.choice([32, 97, 300]),
+               text_enc_depth=rng.choice([1, 2, 3]), text_seq_len=rng.choice([5, 16, 33]), text_heads=heads_t,
+               visual_enc_depth=rng.choice([1, 2]), visual_heads=heads_i, visual_image_size=side,
+               visual_patch_size=patch)
+    flags = dict(decoupled_contrastive_learning=rng.random() < 0.4, extra_latent_projection=rng.random() < 0.4,
+                 use_all_token_embeds=rng.random() < 0.3)
+    # (FILIP with a causal text tower does not run in the reference itself: 15 text tokens after the CLS
+    #  strip against a 16-wide mask, x_clip.py:705 / :806)
+    text_kind = rng.choice(["plain", "plain", "rotary"] + ([] if flags["use_all_token_embeds"] else ["causal"]))
+    if text_kind == "rotary":
+        flags["text_rotary_pos_emb"] = True
+    elif text_kind == "causal":
+        flags.update(text_causal_mask=True, text_eos_id=cfg["num_text_tokens"] - 1)
+    cfg.update({k: v for k, v in flags.items() if v})
+    batch = rng.choice([2, 3, 5, 8])
+    pad = rng.choice([0.0, 0.2, 0.5])
+    n_patches = (side // patch) ** 2
+    drop = rng.choice([0.0, 0.0, 0.5]) if n_patches >= 4 else 0.0
+    return cfg, batch, pad, drop
+
+
+RANDOM_SAMPLES = 32
+
+
+def random_cases(x_clip):
+    """The reference on every random configuration -> (cases, samples).  cases (JSON: loss, d temperature,
+    gradient norms, encoding and latent summaries) go to tests/golden/random_configs.json; samples is one
+    float32 vector for tests/golden/random_configs_samples.npy: per case, from its "sample_offset" on,
+    RANDOM_SAMPLES entries (fewer for smaller tensors) of every gradient in "grad_norms" order, then twice
+    that of enc_text and of enc_image (sample_positions() with seeds 0, 1, 2).
+    Checked by tests/test_oracle_vs_reference_live.py."""
+    import numpy as np
+    cases, samples = [], []
+    for seed in RANDOM_SEEDS:
+        cfg, batch, pad, drop = draw_random_case(seed)
+        out = run_case(x_clip, f"random_{seed}", cfg, batch, pad, drop, samples=RANDOM_SAMPLES)
+        offset = sum(len(v) for v in samples)
+        gs = out.pop("grad_samples")
+        samples += [gs[k] for k in out["grad_norms"]]
+        samples += [out.pop("enc_text_sample"), out.pop("enc_image_sample")]
+        for k in ("text_latents", "image_latents", "torch_version"):
+            out.pop(k, None)
+        cases.append(dict(out, seed=seed, sample_offset=offset))
+    return cases, np.asarray([x for v in samples for x in v], dtype=np.float32)
 
 
 def multiview_case(x_clip, name, cfg_kwargs, batch, n_aug_text, n_aug_image):
@@ -264,6 +338,10 @@ def sharded_case(name, cfg_kwargs, world=2, per_rank=3):
 def main():
     torch.set_num_threads(max(1, os.cpu_count() or 1))
     x_clip = import_reference()
+    cases, samples = random_cases(x_clip)
+    (HERE / "random_configs.json").write_text(json.dumps(cases, separators=(",", ":")) + "\n")
+    import numpy as np
+    np.save(HERE / "random_configs_samples.npy", samples)
     for name, (cfgk, batch, padf, drop) in CASES.items():
         out = run_case(x_clip, name, cfgk, batch, padf, drop)
         (HERE / f"{name}.json").write_text(json.dumps(out))

@@ -20,13 +20,15 @@ def _ref_attention(qkv, mask, B, n, H, scale, causal=False):
 
 CASES = [(2, 33, 4, False), (3, 65, 8, False), (2, 128, 2, True), (2, 17, 4, True),
          (2, 197, 12, False), (2, 257, 8, True), (1, 320, 2, True), (5, 78, 8, True),
-         # n = 128k+1 takes the tail-token path; 24*8 (b,h) items > 148 CTAs: several items per CTA
+         # n = 64k+1: a last 64-row block with one row; 24*8 (b,h) items: many CTAs per SM
          (2, 129, 4, True), (3, 129, 2, False), (24, 257, 8, True), (20, 257, 8, False),
          # short sequences (attention_small.cu): ViT-B/16 with patch dropout (98), CLIP text (78),
          # README image tower (32); several items per CTA; every 16-key tail width
          (130, 98, 12, False), (90, 78, 8, True), (300, 32, 8, False), (3, 64, 4, True), (2, 112, 3, True),
          (2, 1, 2, False), (3, 16, 2, True), (2, 100, 4, True), (4, 128, 12, False), (2, 48, 2, False),
-         (2, 81, 5, True)]
+         (2, 81, 5, True),
+         # batch x heads beyond 65535 CTAs in one grid dimension
+         (16640, 16, 4, True)]
 CAUSAL_CASES = [(3, 78, 8, True), (2, 33, 4, False), (2, 128, 2, True), (40, 64, 8, False)]
 
 

@@ -46,7 +46,7 @@ def test_mlm_loss_matches_fp32_restatement(cuda_device):
     from oracle import clip_oracle as O
     import x_clip_b200
     kw = dict(TINY, num_text_tokens=120)             # + [MASK] -> 121 rows in the embedding table; the
-    # 120-way vocabulary projection of the masked rows runs on the tcgen05 GEMM (N % 8 == 0)
+    # 120-way vocabulary projection of the masked rows runs on the wgmma GEMM (N % 8 == 0)
     clip = x_clip_b200.CLIP(**kw, use_mlm=True, mlm_mask_token_id=2, visual_patch_dropout=0.).to(cuda_device)
     clip.train()
     cfg = O.ClipConfig(**dict(kw, num_text_tokens=121))

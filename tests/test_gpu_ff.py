@@ -13,7 +13,7 @@ def _ln(x, g, eps=1e-5):
 
 
 @pytest.mark.parametrize("M,d", [(300, 256), (1000, 512), (2 * 98 * 3, 768), (130, 1024), (77, 512),
-                                 (148 * 128 * 3 + 40, 512)])   # > 1 tile per CTA pair: the steady-state pipeline
+                                 (148 * 128 * 3 + 40, 512)])   # several tiles per CTA: the steady-state pipeline
 def test_ff_forward_and_w2_gradient(cuda_device, M, d):
     from x_clip_b200 import kernels as K
     dev = cuda_device
@@ -53,18 +53,11 @@ def test_ff_forward_and_w2_gradient(cuda_device, M, d):
     (_ln(hp_a, g4_leaf) @ w2_leaf.t()).backward(dx.float())
 
     dxs, vsum, ab = K.ff_bwd_prep(dx, stats, acc, colvec)
-    # both epilogue variants of the fused backward (explicit A/B switch, include/xclip_b200.h): same numbers
-    from x_clip_b200 import _lib
-    lib = _lib.load()
-    prev = lib.xclip_tune_set(0, 0)
-    try:
-        du0 = K.ff_bwd(dx, w2g, u, stats, ab)
-        lib.xclip_tune_set(0, 1)
-        du = K.ff_bwd(dx, w2g, u, stats, ab)
-    finally:
-        lib.xclip_tune_set(0, prev)
+    # the fused backward is deterministic: two runs give the same bits
+    du0 = K.ff_bwd(dx, w2g, u, stats, ab)
+    du = K.ff_bwd(dx, w2g, u, stats, ab)
     torch.cuda.synchronize()
-    assert torch.equal(du0, du), "ff_bwd: the TMA-pipelined epilogue must reproduce the ld.global one bit for bit"
+    assert torch.equal(du0, du), "ff_bwd: two runs on the same inputs must agree bit for bit"
     raw = torch.zeros(d, 4 * d, device=dev)
     K.gemm(dxs, hp, a_major=1, b_major=1, out=raw, accumulate=True)
     dg4 = torch.zeros(4 * d, device=dev)

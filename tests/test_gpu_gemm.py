@@ -1,4 +1,4 @@
-"""tcgen05 GEMM vs a plain fp32 torch matmul of the same bf16-rounded operands."""
+"""wgmma GEMM vs a plain fp32 torch matmul of the same bf16-rounded operands."""
 import pytest
 import torch
 
@@ -92,28 +92,6 @@ def test_gemm_wgrad_splitk_accumulate(cuda_device, M, N, K):
     ref = _ref(a, b, 1, 1) + 1.0
     err = (out - ref).abs().max().item()
     assert err <= 2e-3 * ref.abs().max().item() + 1e-2
-
-
-@pytest.mark.parametrize("a_major,b_major", [(0, 0), (0, 1), (1, 1)])
-def test_gemm_cta_pair_equals_single_cta(cuda_device, a_major, b_major):
-    """The cta_group::2 kernel (256 x 256 tiles on CTA pairs) and the single-CTA kernel accumulate
-    every output element over the same k order: identical results, also with an odd number of
-    128-row blocks (M = 896 + 40) and a ragged N."""
-    from x_clip_b200 import kernels, _lib
-    lib = _lib.load()
-    M, N, K = 936, 1288, 704
-    a, b = _mk(M, N, K, a_major, b_major, cuda_device, seed=5)
-    outs = []
-    try:
-        for mode in (1, 0):
-            lib.xclip_gemm_set_pair_mode(mode)
-            outs.append(kernels.gemm(a, b, a_major=a_major, b_major=b_major))
-    finally:
-        lib.xclip_gemm_set_pair_mode(1)
-    torch.cuda.synchronize()
-    ref = _ref(a, b, a_major, b_major)
-    assert (outs[0].float() - ref).abs().max().item() <= 1e-2 * ref.abs().max().item()
-    assert torch.equal(outs[0], outs[1])
 
 
 def test_gemm_rejects_bad_args(cuda_device):

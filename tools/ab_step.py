@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Interleaved A/B timing of whole benchmark steps in ONE process on ONE model (cfg3 by default).
 
-    python tools/ab_step.py "mb=512,retain=auto" "mb=768,retain=auto" "mb=512,retain=auto,tune=0:0" ...
+    python tools/ab_step.py "mb=512,retain=auto" "mb=768,retain=auto" "mb=512,retain=auto,tune=3:4" ...
 
 Boxes differ by several percent in sustained clocks under the power cap, and one box drifts while it
 warms up, so configurations are compared round-robin (A B C A B C ...) inside one process: `rounds`

@@ -1,4 +1,4 @@
-"""Time the tcgen05 GEMM at the shapes of the bench workloads, CTA-pair kernel vs single-CTA kernel.
+"""Time the wgmma GEMM at the shapes of the bench workloads.
 
     python tools/gemm_bench.py            (cfg3 micro-batch 512 and cfg2 shapes)"""
 import os
@@ -40,12 +40,6 @@ for (label, M, N, Kd, am, bm, acc) in SHAPES:
     a = torch.randn((M, Kd) if am == 0 else (Kd, M), generator=g).to(dev).bfloat16()
     b = torch.randn((N, Kd) if bm == 0 else (Kd, N), generator=g).to(dev).bfloat16()
     out = torch.zeros(M, N, device=dev, dtype=torch.float32 if acc else torch.bfloat16)
-    res = {}
-    for mode in (1, 0):
-        lib.xclip_gemm_set_pair_mode(mode)
-        ms = timeit(lambda: K.gemm(a, b, a_major=am, b_major=bm, out=out, accumulate=acc))
-        res[mode] = ms
-    lib.xclip_gemm_set_pair_mode(1)
+    ms = timeit(lambda: K.gemm(a, b, a_major=am, b_major=bm, out=out, accumulate=acc))
     fl = 2.0 * M * N * Kd
-    print(f"{label:22s} M={M} N={N} K={Kd}: pair {res[1]:.3f} ms {fl / res[1] / 1e9:7.1f} TF/s | "
-          f"single {res[0]:.3f} ms {fl / res[0] / 1e9:7.1f} TF/s", flush=True)
+    print(f"{label:22s} M={M} N={N} K={Kd}: {ms:.3f} ms {fl / ms / 1e9:7.1f} TF/s", flush=True)

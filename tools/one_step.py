@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""One benchmark step between cudaProfilerStart/Stop, for
+"""One benchmark step between cudaProfilerStart/Stop, for a profiler that honours them, e.g.
     ncu --profile-from-start off --metrics gpu__time_duration.sum --clock-control none --csv --log-file X python tools/one_step.py
 (the launch list the roofline shares are checked against).  Reduced batch (same model, same chunk size,
 one resident + one re-encoded chunk) so that the serialised capture stays within a minute or two."""

@@ -1,4 +1,5 @@
-"""Stand-alone launches of the hot kernels at benchmark shapes, for `ncu --set full`.
+"""Stand-alone launches of the hot kernels at benchmark shapes, for a kernel profiler (torch.profiler, or
+`ncu --set full` where Nsight Compute is available).
 
     python tools/profile_kernels.py gemm|attn|nce|rowwise [reps]
 

@@ -1,4 +1,4 @@
-"""x_clip_b200: B200-native (sm_100a) CLIP contrastive-training hot path behind the
+"""x_clip_b200: H100-native (sm_90a) CLIP contrastive-training hot path behind the
 lucidrains/x-clip `CLIP(...)` surface.  `import x_clip_b200 as x_clip` is the drop-in."""
 from .clip import CLIP, TextTransformer, VisionTransformer, Unsupported  # noqa: F401
 

@@ -28,7 +28,6 @@ SIGNATURES = {
     "xclip_init": (c_int, []),
     "xclip_launch_count": (c_longlong, []),
     "xclip_launch_count_reset": (None, []),
-    "xclip_gemm_set_pair_mode": (c_int, [c_int]),
     "xclip_tune_set": (c_int, [c_int, c_int]),
     "xclip_gemm_bf16": (c_int, [c_void_p, c_int64, c_int, c_void_p, c_int64, c_int, c_void_p,
                                 c_int64, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p,
@@ -102,7 +101,7 @@ def load() -> ctypes.CDLL:
     if not LIB_PATH.exists():
         raise XClipB200Error(
             f"{LIB_PATH} is missing. Build it with `python -m x_clip_b200.build` "
-            "(nvcc, sm_100a). x_clip_b200 has no CPU or eager-PyTorch fallback.")
+            "(nvcc, sm_90a). x_clip_b200 has no CPU or eager-PyTorch fallback.")
     lib = ctypes.CDLL(str(LIB_PATH))
     for name, (res, args) in SIGNATURES.items():
         fn = getattr(lib, name)

@@ -4,8 +4,8 @@ The reference wraps its encoders in generic torch modules: `MLM` (x_clip/mlm.py:
 language modelling on the text transformer), `SimSiam` / `SimCLR` (x_clip/visual_ssl.py, a
 BYOL-style wrapper around the vision transformer) and mixes their losses into the contrastive
 loss (x_clip/x_clip.py:611-621, :851-868).  Here the same objectives are written against the
-B200 encoders of this package: the expensive part - every encoder pass - runs on the CUDA kernels
-(engine.TransformerFn), the vocabulary projection of the MLM head runs on the tcgen05 GEMM over the
+H100 encoders of this package: the expensive part - every encoder pass - runs on the CUDA kernels
+(engine.TransformerFn), the vocabulary projection of the MLM head runs on the wgmma GEMM over the
 MASKED positions only (engine.LinearFn), and the small heads (cross entropy over the selected
 rows, BatchNorm MLPs, cosine / NT-Xent losses, torchvision augmentations) stay ordinary torch
 modules, exactly as in the reference - they are not on the north-star path.

@@ -1,4 +1,4 @@
-"""In-tree build of libxclip_b200.so (the C-ABI library) with nvcc for sm_100a.
+"""In-tree build of libxclip_b200.so (the C-ABI library) with nvcc for sm_90a.
 
 `python -m x_clip_b200.build` or `__graft_entry__.build()`.  nvcc cross-compiles
 without a GPU; the resulting .so is git-ignored but travels with the source tree.
@@ -21,7 +21,7 @@ LIB = PKG / "libxclip_b200.so"
 NVCC_FLAGS = [
     "-O3",
     "-std=c++17",
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo",
     "--expt-relaxed-constexpr",
     "-Xcompiler", "-fPIC",
@@ -94,7 +94,7 @@ def build(verbose: bool = False, force: bool = False) -> Path:
     if LIB.exists() and stamp.exists() and stamp.read_text().strip() == link_key:
         return LIB
     cmd = [_nvcc(), "-shared", "-o", str(LIB), *map(str, objs),
-           "-gencode", "arch=compute_100a,code=sm_100a", "-Xcompiler", "-fPIC"]
+           "-gencode", "arch=compute_90a,code=sm_90a", "-Xcompiler", "-fPIC"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

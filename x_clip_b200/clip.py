@@ -1,4 +1,4 @@
-"""Drop-in `CLIP` / `TextTransformer` / `VisionTransformer` for lucidrains/x-clip, B200 path.
+"""Drop-in `CLIP` / `TextTransformer` / `VisionTransformer` for lucidrains/x-clip, H100 path.
 
 The constructor keywords, forward signature, early returns, assertions and - crucially -
 the parameter tree (`state_dict` keys and shapes, SURVEY.md 8b) mirror the reference
@@ -119,7 +119,7 @@ class Transformer(nn.Module):
     def forward(self, x, rotary_pos_emb=None, mask=None):
         """rotary_pos_emb: the reference's angle table [n, 32] (RotaryEmbedding.forward, :161-166);
         its two halves are equal, the kernel takes cos / sin of the first 16 columns."""
-        _require(x.is_cuda, "inputs must live on a CUDA (sm_100) device")
+        _require(x.is_cuda, "inputs must live on a CUDA (sm_90) device")
         n = x.shape[1]
         _require(not self.causal or n <= 128, "the causal mask is implemented for sequences <= 128 tokens")
         cos = sin = None
@@ -192,7 +192,7 @@ class TextTransformer(nn.Module):
 
     def forward(self, x, mask=None):
         b, n = x.shape
-        _require(x.is_cuda, "inputs must live on a CUDA (sm_100) device")
+        _require(x.is_cuda, "inputs must live on a CUDA (sm_90) device")
         _require(n <= self.max_seq_len, "text longer than text_seq_len")
         rotary = None
         if self.abs_pos_emb is not None and self.cls_token is not None:
@@ -234,7 +234,7 @@ class VisionTransformer(nn.Module):
         bf16 cast are ONE pass that reads only the kept patches (xclip_patchify_gather); the
         patch-embedding GEMM adds bias and the gathered position rows in its epilogue."""
         b = x.shape[0]
-        _require(x.is_cuda, "inputs must live on a CUDA (sm_100) device")
+        _require(x.is_cuda, "inputs must live on a CUDA (sm_90) device")
         p = self.patch_size
         _require(x.shape[2] % p == 0 and x.shape[3] % p == 0, "image size must be a multiple of the patch size")
         n = (x.shape[2] // p) * (x.shape[3] // p)
@@ -449,7 +449,7 @@ class CLIP(nn.Module):
         aug_text=None,
         aug_image=None,
     ):
-        _require(text.is_cuda and image.is_cuda, "inputs must live on a CUDA (sm_100) device")
+        _require(text.is_cuda and image.is_cuda, "inputs must live on a CUDA (sm_90) device")
 
         text_mask = text != self.text_pad_id
 

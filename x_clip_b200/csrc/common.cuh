@@ -1,12 +1,11 @@
-// Device-side primitives for the sm_100a kernels of x_clip_b200: mbarrier, TMA
-// (cp.async.bulk.tensor), tcgen05 (UMMA + TMEM) and descriptor builders.
+// Device-side primitives for the sm_90a kernels of x_clip_b200: mbarrier, TMA
+// (cp.async.bulk.tensor), wgmma (warpgroup MMA from shared-memory descriptors) and the descriptor
+// builder.
 //
-// Everything here is inline PTX; nothing depends on CUTLASS/CuTe.  Bit layouts of
-// the shared-memory matrix descriptor and the instruction descriptor follow the
-// PTX ISA "tcgen05" chapter (the same fields CuTe names in
-// cute/arch/mma_sm100_desc.hpp: start_address[0,14) LBO[16,30) SBO[32,46)
-// version[46,48) layout_type[61,64); idesc: c_format[4,6) a_format[7,10)
-// b_format[10,13) a_major[15] b_major[16] n>>3[17,23) m>>4[24,29)).
+// Everything here is inline PTX; nothing depends on CUTLASS/CuTe.  The shared-memory matrix
+// descriptor follows the PTX ISA "wgmma" chapter (the fields CuTe names in
+// cute/arch/mma_sm90_desc.hpp: start_address[0,14) LBO[16,30) SBO[32,46) base_offset[49,52)
+// layout_type[62,64), 1 = SWIZZLE_128B).
 #pragma once
 
 #include <cuda.h>
@@ -32,10 +31,8 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
 
 __device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31; }
 
-// Single-thread regions that issue tcgen05.mma / TMA instructions are entered through
-// elect.sync: with `lane == 0` ptxas cannot prove that one thread is active, so every UTCHMMA /
-// UTMALDG got a waterfall loop (ELECT + BRA.U.ANY + R2UR, ~17 SASS instructions per MMA instead
-// of ~8).  Validated on a B200 in round 2 (full GPU suite; attention backward 1.91 -> 1.80 ms).
+// Single-thread regions that issue TMA instructions are entered through elect.sync: with
+// `lane == 0` ptxas cannot prove that one thread is active and wraps every issue in a loop.
 #define XCLIP_ONE_LANE(lane) (::xclip::elect_one())
 
 __device__ __forceinline__ bool elect_one() {
@@ -84,7 +81,7 @@ __device__ __forceinline__ void fence_barrier_init() {
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
 
-// make generic-proxy writes to shared memory visible to the async proxy (TMA, UMMA)
+// make generic-proxy writes to shared memory visible to the async proxy (TMA, wgmma)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
@@ -127,6 +124,16 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   }
 }
 
+// The same bound without the diagnostic printf, for kernels that issue wgmma: a function call
+// (printf) anywhere in such a kernel makes ptxas serialise the wgmma pipeline.
+__device__ __forceinline__ void mbar_wait_nocall(uint64_t* bar, uint32_t parity) {
+  if (mbar_try_wait(bar, parity)) return;
+  const long long t0 = clock64();
+  while (!mbar_try_wait(bar, parity)) {
+    if (clock64() - t0 > 8000000000ll) __trap();
+  }
+}
+
 // ---------------------------------------------------------------------------
 // TMA
 // ---------------------------------------------------------------------------
@@ -162,149 +169,9 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
 }
 
 // ---------------------------------------------------------------------------
-// CTA pair (cta_group::2) primitives: two CTAs of a 2-cluster issue ONE tcgen05.mma of M = 256;
-// each CTA stages its own 128 rows of A and its own half of B's N columns, so the operand bytes
-// every SM pulls from L2 per flop drop by a third against two independent 128 x 256 tiles.
-// PTX forms as in CUTLASS (cute/arch/copy_sm100_tma.hpp, mma_sm100_umma.hpp, cutlass/arch/barrier.h).
-// ---------------------------------------------------------------------------
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;   // clears the CTA-rank bit of a shared::cluster address
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// TMA load whose completion bytes are credited to the mbarrier of the pair's LEADER (even) CTA
-__device__ __forceinline__ void tma_load_2d_pair(void* smem_dst, const CUtensorMap* m, uint64_t* bar,
-                                                 int32_t c0, int32_t c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_pair_512(uint32_t* smem_result) {  // whole warp, BOTH CTAs
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_result)),
-               "r"(512)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair_512(uint32_t taddr) {  // whole warp, BOTH CTAs
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(512) : "memory");
-}
-// D[tmem of both CTAs, M = 256] (+)= A * B; issued by ONE thread of the leader CTA
-__device__ __forceinline__ void umma_bf16_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                               uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on the mbarrier at the same smem offset in BOTH CTAs once all prior MMAs retired
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(static_cast<uint16_t>(3))
-      : "memory");
-}
-// plain arrive on the LEADER CTA's copy of a barrier (from either CTA of the pair)
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & kPeerBitMask)
-               : "memory");
-}
-
-// ---------------------------------------------------------------------------
-// tcgen05: TMEM allocation, MMA, commit, loads, fences
-// ---------------------------------------------------------------------------
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result) {  // whole warp
-  static_assert(kCols == 32 || kCols == 64 || kCols == 128 || kCols == 256 || kCols == 512, "");
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_result)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols)
-               : "memory");
-}
-
-__device__ __forceinline__ void tcgen05_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tcgen05_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-
-// D[tmem] (+)= A[smem] * B[smem]; issued by ONE thread.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                          uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// mbarrier arrive when all previously issued tcgen05.mma of this thread completed.
-// (implies tcgen05.fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-
-// 32 lanes x 32 consecutive fp32 columns: thread t of the warp receives lane
-// (lane_base + t), columns [col, col+32).  A warp may only touch the lane quarter
-// 32*(warp_id%4)..+31.
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]),
-        "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]),
-        "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// ---------------------------------------------------------------------------
 // descriptors
 // ---------------------------------------------------------------------------
-// Shared-memory matrix descriptor for a SWIZZLE_128B tile whose base is 1024 B aligned.
+// Shared-memory matrix descriptor (wgmma) for a SWIZZLE_128B tile whose base is 1024 B aligned.
 //   K-major  : rows (M/N index) of 128 B (64 bf16 along K); 8-row groups SBO apart
 //              (1024 B when the tile is dense); LBO unused.
 //   MN-major : rows (K index) of 128 B (64 bf16 along M/N); 8-row K-groups SBO apart
@@ -315,8 +182,7 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t 
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= static_cast<uint64_t>(1) << 46;  // descriptor version (Blackwell)
-  d |= static_cast<uint64_t>(2) << 61;  // SWIZZLE_128B
+  d |= static_cast<uint64_t>(1) << 62;  // SWIZZLE_128B
   return d;
 }
 
@@ -325,11 +191,39 @@ __device__ __forceinline__ uint64_t desc_advance(uint64_t desc, uint32_t bytes) 
   return desc + static_cast<uint64_t>(bytes >> 4);
 }
 
-// kind::f16 instruction descriptor: bf16 x bf16 -> fp32
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N, int a_major, int b_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(a_major) << 15) |
-         (static_cast<uint32_t>(b_major) << 16) | (static_cast<uint32_t>(N >> 3) << 17) |
-         (static_cast<uint32_t>(M >> 4) << 24);
+// ---------------------------------------------------------------------------
+// wgmma: D[64 x N] (fp32, registers of one warpgroup) += A[smem] * B[smem], bf16 inputs.
+// kTransA / kTransB = 1 when the operand is MN-major.  Fragment layout of D (thread t of the
+// warpgroup, w = t / 32, l = t % 32): d[j] sits at row 16 w + l / 4 + 8 ((j / 2) % 2),
+// column 8 (j / 4) + 2 (l % 4) + (j % 2).
+// ---------------------------------------------------------------------------
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+template <int kTransA, int kTransB>
+__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t da, uint64_t db) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %34, %35;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "n"(kTransA), "n"(kTransB));
+}
+
+template <int kTransA, int kTransB>
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t da, uint64_t db) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %66, %67;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "n"(kTransA), "n"(kTransB));
+}
+
+__device__ __forceinline__ void named_bar_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 
 // byte offset of 16 B chunk `c16` of 128 B row `row` inside a SWIZZLE_128B tile
@@ -371,45 +265,25 @@ __device__ __forceinline__ GeluParts gelu_parts(float x) {
 __device__ __forceinline__ float gelu_erf(float x) { return x * gelu_parts(x).cdf; }
 
 // ---------------------------------------------------------------------------
-// Packed fp32x2 arithmetic (sm_100: FFMA2 - one instruction, one issue slot, two IEEE fp32 FMAs on
-// an aligned register pair).  The GELU epilogues of the fused feed-forward are bound by the FMA pipe
-// (~28 FMA-class instructions per element in scalar form against 2 MUFU); in packed form the
-// polynomial and the affine chains cost half the instructions and the two MUFU become the floor.
+// fp32 pairs: the GELU epilogues of the fused feed-forward handle two adjacent columns at a time
+// (two independent dependency chains per thread).
 // ---------------------------------------------------------------------------
-typedef unsigned long long f32x2;
-__device__ __forceinline__ f32x2 f2_pack(float lo, float hi) {
-  f32x2 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ f32x2 f2_splat(float v) { return f2_pack(v, v); }
-__device__ __forceinline__ void f2_unpack(f32x2 v, float& lo, float& hi) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-}
+struct f32x2 {
+  float x, y;
+};
+__device__ __forceinline__ f32x2 f2_pack(float lo, float hi) { return f32x2{lo, hi}; }
+__device__ __forceinline__ f32x2 f2_splat(float v) { return f32x2{v, v}; }
+__device__ __forceinline__ void f2_unpack(f32x2 v, float& lo, float& hi) { lo = v.x; hi = v.y; }
 __device__ __forceinline__ f32x2 f2_fma(f32x2 a, f32x2 b, f32x2 c) {
-  f32x2 r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-  return r;
+  return f32x2{fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)};
 }
-__device__ __forceinline__ f32x2 f2_mul(f32x2 a, f32x2 b) {
-  f32x2 r;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-__device__ __forceinline__ f32x2 f2_add(f32x2 a, f32x2 b) {
-  f32x2 r;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-// two consecutive bf16 of one 32-bit word -> packed fp32 pair (element 0 in the low half)
+__device__ __forceinline__ f32x2 f2_mul(f32x2 a, f32x2 b) { return f32x2{__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)}; }
+__device__ __forceinline__ f32x2 f2_add(f32x2 a, f32x2 b) { return f32x2{__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)}; }
+// two consecutive bf16 of one 32-bit word -> fp32 pair (element 0 in the low half)
 __device__ __forceinline__ f32x2 f2_from_bf16x2(uint32_t w) {
   return f2_pack(__uint_as_float(w << 16), __uint_as_float(w & 0xffff0000u));
 }
-__device__ __forceinline__ uint32_t f2_to_bf16x2(f32x2 v) {
-  float lo, hi;
-  f2_unpack(v, lo, hi);
-  return pack_bf16x2(lo, hi);
-}
+__device__ __forceinline__ uint32_t f2_to_bf16x2(f32x2 v) { return pack_bf16x2(v.x, v.y); }
 
 // gelu_parts for two elements at once: cdf = Phi(x), pdf = phi(x) (same A&S 7.1.26 polynomial).
 struct GeluParts2 {

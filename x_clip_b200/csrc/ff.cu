@@ -1,4 +1,4 @@
-// Fused feed-forward block (reference x_clip/x_clip.py:180-199) on the CTA-pair GEMM:
+// Fused feed-forward block (reference x_clip/x_clip.py:180-199) on the wgmma GEMM (gemm.cuh):
 //   u = xn W1^T, hp = value * gelu(gate)          one GEMM, GEGLU in its epilogue   (xclip_ff_up)
 //   x2 = LN_4d(hp) g W2^T + x1                     one GEMM, LayerNorm folded into
 //                                                  weight + epilogue                (xclip_ff_down)
@@ -10,12 +10,12 @@
 // Backward pieces that replace the LayerNorm output h (never materialised now):
 //   dW2_jk = g_k (sum_r dxs_rj hp_rk - v_j),  dxs = dx * rstd_r,  v_j = sum_r dxs_rj mean_r
 // (xclip_ff_bwd_prep, xclip_ff_w2_grad_post); everything else of the backward is unchanged.
-#include "gemm_pair.cuh"
+#include "gemm.cuh"
 #include "host.h"
 
 namespace xclip {
 
-// out[256 t + i] = w1[128 t + i] (i < 128: value rows) | w1[4d + 128 t + i - 128] (gate rows)
+// out[128 t + i] = w1[64 t + i] (i < 64: value rows) | w1[4d + 64 t + i - 64] (gate rows)
 __global__ void __launch_bounds__(256)
 ff_permute_cast_kernel(const float* __restrict__ w1, bf16* __restrict__ out, int d) {
   const long long vec_per_row = d / 8;
@@ -24,9 +24,9 @@ ff_permute_cast_kernel(const float* __restrict__ w1, bf16* __restrict__ out, int
        idx += (long long)gridDim.x * blockDim.x) {
     const long long orow = idx / vec_per_row;
     const int c = (int)(idx - orow * vec_per_row) * 8;
-    const long long t = orow >> 8;
-    const int i = (int)(orow & 255);
-    const long long srow = i < 128 ? 128 * t + i : 4ll * d + 128 * t + (i - 128);
+    const long long t = orow >> 7;
+    const int i = (int)(orow & 127);
+    const long long srow = i < 64 ? 64 * t + i : 4ll * d + 64 * t + (i - 64);
     const float4 a = *reinterpret_cast<const float4*>(w1 + srow * d + c);
     const float4 b = *reinterpret_cast<const float4*>(w1 + srow * d + c + 4);
     uint4 o;
@@ -69,17 +69,15 @@ ff_scale_cast_kernel(const float* __restrict__ w2, const float* __restrict__ g, 
 }
 
 template <int EPI, int B_MAJOR = kMajorK>
-static int launch_pair_ff(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC,
-                          const CUtensorMap& tmC2, const GemmParams& p, cudaStream_t stream) {
-  using S = PairCfg<EPI>;
-  auto kern = gemm_pair_kernel<kMajorK, B_MAJOR, EPI>;
+static int launch_ff(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, cudaStream_t stream) {
+  using S = GemmSmem<128>;
+  auto kern = gemm_bf16_kernel<128, kMajorK, B_MAJOR, EPI>;
   const int rc = ensure_dynamic_smem(reinterpret_cast<const void*>(kern), S::kTotal);
   if (rc) return rc;
-  const long long tiles = (long long)((p.M + 255) / 256) * ((p.N + 255) / 256);
-  const int units = num_sms() / 2;
-  const int pairs = (int)(tiles < units ? tiles : units);
-  kern<<<2 * pairs, S::kThreads, S::kTotal, stream>>>(tmA, tmB, tmC, tmC2, p);
-  XCLIP_LAUNCH_CHECK("gemm_pair_kernel<ff>");
+  const long long tiles = (long long)((p.M + kGemmBlockM - 1) / kGemmBlockM) * ((p.N + 127) / 128);
+  const int grid = (int)(tiles < num_sms() ? tiles : num_sms());
+  kern<<<grid, kGemmThreads, S::kTotal, stream>>>(tmA, tmB, p);
+  XCLIP_LAUNCH_CHECK("gemm_bf16_kernel<ff>");
   return XCLIP_OK;
 }
 
@@ -118,22 +116,20 @@ extern "C" int xclip_ff_up(const void* x, int64_t ldx, const void* w1p, void* u,
   if (rc) return rc;
   XCLIP_REQUIRE(x && w1p && hp && rowsum, "ff_up: null pointer");
   const bool skip_u = (u == nullptr);      // forward-only sweeps: hp is all the down-projection needs
-  if (skip_u) { u = hp; ldu = ldhp >= 8 * (int64_t)d ? ldhp : 8 * (int64_t)d; }   // (placeholder map, never stored to)
+  if (skip_u) { u = hp; ldu = 8 * (int64_t)d; }   // (placeholder, never stored to)
   XCLIP_REQUIRE(M > 0 && d > 0 && d % 256 == 0, "ff_up: M=%d d=%d (d %% 256)", M, d);
   XCLIP_REQUIRE(ldx % 8 == 0 && ldx >= d && ldu % 8 == 0 && ldu >= 8 * d && ldhp % 8 == 0 && ldhp >= 4 * d,
                 "ff_up: bad leading dimensions");
   XCLIP_REQUIRE(FF_ALIGNED(x) && FF_ALIGNED(w1p) && FF_ALIGNED(u) && FF_ALIGNED(hp), "ff_up: misaligned pointer");
-  CUtensorMap tmA, tmB, tmC, tmC2;
+  CUtensorMap tmA, tmB;
   if ((rc = encode_2d_bf16(&tmA, x, (uint64_t)d, (uint64_t)M, (uint64_t)ldx, 64, kGemmBlockM))) return rc;
   if ((rc = encode_2d_bf16(&tmB, w1p, (uint64_t)d, (uint64_t)(8 * d), (uint64_t)d, 64, 128))) return rc;
-  if (skip_u) {
-    if ((rc = encode_2d_bf16(&tmC, hp, (uint64_t)(4 * d), (uint64_t)M, (uint64_t)ldhp, 64, kGemmBlockM))) return rc;
-  } else if ((rc = encode_2d_bf16(&tmC, u, (uint64_t)(8 * d), (uint64_t)M, (uint64_t)ldu, 64, kGemmBlockM))) return rc;
-  if ((rc = encode_2d_bf16(&tmC2, hp, (uint64_t)(4 * d), (uint64_t)M, (uint64_t)ldhp, 64, kGemmBlockM))) return rc;
   GemmParams p = {};
   p.M = M; p.N = 8 * d; p.K = d; p.split_k = 1; p.alpha = 1.f;
   p.ff_rowsum = rowsum; p.ff_hidden = 4 * d; p.ff_skip_u = skip_u ? 1 : 0;
-  return launch_pair_ff<PEPI_FF_UP>(tmA, tmB, tmC, tmC2, p, reinterpret_cast<cudaStream_t>(stream));
+  p.ff_u = reinterpret_cast<bf16*>(u); p.ff_ldu = ldu;
+  p.ff_out2 = reinterpret_cast<bf16*>(hp); p.ff_ld2 = ldhp;
+  return launch_ff<EPI_FF_UP>(tmA, tmB, p, reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int xclip_ff_down(const void* hp, int64_t ldhp, const void* w2g, const float* colvec,
@@ -150,17 +146,17 @@ extern "C" int xclip_ff_down(const void* hp, int64_t ldhp, const void* w2g, cons
   XCLIP_REQUIRE(FF_ALIGNED(hp) && FF_ALIGNED(w2g) && FF_ALIGNED(out) && FF_ALIGNED(acc_out) &&
                     FF_ALIGNED(colvec) && (!residual || FF_ALIGNED(residual)),
                 "ff_down: misaligned pointer");
-  CUtensorMap tmA, tmB, tmC, tmC2;
+  CUtensorMap tmA, tmB;
   if ((rc = encode_2d_bf16(&tmA, hp, (uint64_t)(4 * d), (uint64_t)M, (uint64_t)ldhp, 64, kGemmBlockM))) return rc;
   if ((rc = encode_2d_bf16(&tmB, w2g, (uint64_t)(4 * d), (uint64_t)d, (uint64_t)(4 * d), 64, 128))) return rc;
-  if ((rc = encode_2d_bf16(&tmC, out, (uint64_t)d, (uint64_t)M, (uint64_t)ldo, 64, kGemmBlockM))) return rc;
-  if ((rc = encode_2d_bf16(&tmC2, acc_out, (uint64_t)d, (uint64_t)M, (uint64_t)ldacc, 64, kGemmBlockM))) return rc;
   GemmParams p = {};
   p.M = M; p.N = d; p.K = 4 * d; p.split_k = 1; p.alpha = 1.f;
+  p.c = out; p.ldc = ldo;
   p.residual = reinterpret_cast<const bf16*>(residual); p.ldr = ldr;
   p.ff_rowsum = const_cast<float*>(rowsum); p.ff_colvec = colvec; p.ff_stats = stats;
   p.ff_eps = eps; p.ff_hidden = 4 * d;
-  return launch_pair_ff<PEPI_FF_DOWN>(tmA, tmB, tmC, tmC2, p, reinterpret_cast<cudaStream_t>(stream));
+  p.ff_out2 = reinterpret_cast<bf16*>(acc_out); p.ff_ld2 = ldacc;
+  return launch_ff<EPI_FF_DOWN>(tmA, tmB, p, reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int xclip_ff_bwd(const void* dx, int64_t lddx, const void* w2g, const void* u, int64_t ldu,
@@ -173,18 +169,14 @@ extern "C" int xclip_ff_bwd(const void* dx, int64_t lddx, const void* w2g, const
   XCLIP_REQUIRE(lddx % 8 == 0 && lddx >= d && ldu % 8 == 0 && ldu >= 8 * d && lddu % 8 == 0 && lddu >= 8 * d,
                 "ff_bwd: bad leading dimensions");
   XCLIP_REQUIRE(FF_ALIGNED(dx) && FF_ALIGNED(w2g) && FF_ALIGNED(u) && FF_ALIGNED(du), "ff_bwd: misaligned pointer");
-  CUtensorMap tmA, tmB, tmC;
+  CUtensorMap tmA, tmB;
   if ((rc = encode_2d_bf16(&tmA, dx, (uint64_t)d, (uint64_t)M, (uint64_t)lddx, 64, kGemmBlockM))) return rc;
   // B = w2g [d, 4d] consumed MN-major: contraction index d on rows, 64 x 64 boxes
   if ((rc = encode_2d_bf16(&tmB, w2g, (uint64_t)(4 * d), (uint64_t)d, (uint64_t)(4 * d), 64, kGemmBlockK))) return rc;
-  if ((rc = encode_2d_bf16(&tmC, du, (uint64_t)(8 * d), (uint64_t)M, (uint64_t)lddu, 64, kGemmBlockM))) return rc;
   GemmParams p = {};
   p.M = M; p.N = 4 * d; p.K = d; p.split_k = 1; p.alpha = 1.f;
+  p.c = du; p.ldc = lddu;
   p.ff_stats = const_cast<float*>(stats); p.ff_ab = ab; p.ff_hidden = 4 * d;
-  p.ff_u = reinterpret_cast<const bf16*>(u); p.ff_ldu = ldu;
-  if (tune(XCLIP_TUNE_FF_BWD_VARIANT) == 0)      // older epilogue: u by ld.global -> st.shared (kept for A/B)
-    return launch_pair_ff<PEPI_FF_BWD, kMajorMN>(tmA, tmB, tmC, tmC, p, reinterpret_cast<cudaStream_t>(stream));
-  CUtensorMap tmU;                               // u = [value | gate], loaded box-wise ahead of its step
-  if ((rc = encode_2d_bf16(&tmU, u, (uint64_t)(8 * d), (uint64_t)M, (uint64_t)ldu, 64, kGemmBlockM))) return rc;
-  return launch_pair_ff<PEPI_FF_BWD2, kMajorMN>(tmA, tmB, tmC, tmU, p, reinterpret_cast<cudaStream_t>(stream));
+  p.ff_u = const_cast<bf16*>(reinterpret_cast<const bf16*>(u)); p.ff_ldu = ldu;
+  return launch_ff<EPI_FF_BWD, kMajorMN>(tmA, tmB, p, reinterpret_cast<cudaStream_t>(stream));
 }

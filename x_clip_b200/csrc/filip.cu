@@ -6,12 +6,12 @@
 //              [text,image] orientation for i2t as well)
 //
 // The 6-D similarity tensor (68.7 G elements at cfg4) is never materialised:
-//   xclip_filip_segmax : the tcgen05 GEMM with the EPI_SEGMAX epilogue produces, per token row and
+//   xclip_filip_segmax : the wgmma GEMM with the EPI_SEGMAX epilogue produces, per token row and
 //                        per sample of the other modality, max + argmax over that sample's tokens
 //   xclip_filip_reduce : [tokens, B] maxima -> [B, B] similarity (masked mean / mean)
 //   xclip_filip_nce_*  : row-wise InfoNCE / DCL on a [B,B] fp32 matrix (warp-shuffle reductions)
 //   xclip_filip_expand : backward: one-hot (at the argmax) weighted bf16 operand G[rows, cols]
-//                        for a chunk of rows, which then feeds two plain tcgen05 GEMMs
+//                        for a chunk of rows, which then feeds two plain wgmma GEMMs
 //                        (d rows = G @ Zcols, d cols += G^T @ Zrows).
 #include "gemm.cuh"
 #include "host.h"
@@ -154,7 +154,7 @@ extern "C" int xclip_filip_segmax(const void* a, const void* b, int R, int C, in
     const int rc_attr = ensure_dynamic_smem(reinterpret_cast<const void*>(kern), S::kTotal);
     if (rc_attr) return rc_attr;
   }
-  kern<<<grid, kGemmThreads, S::kTotal, reinterpret_cast<cudaStream_t>(stream)>>>(tmA, tmB, tmA, p);
+  kern<<<grid, kGemmThreads, S::kTotal, reinterpret_cast<cudaStream_t>(stream)>>>(tmA, tmB, p);
   XCLIP_LAUNCH_CHECK("gemm_bf16_kernel<segmax>");
   return XCLIP_OK;
 }

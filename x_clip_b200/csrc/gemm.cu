@@ -1,68 +1,34 @@
-// C-ABI launcher for the tcgen05 GEMM (see gemm.cuh and include/xclip_b200.h).
-#include "gemm_pair.cuh"
+// C-ABI launcher for the wgmma GEMM (see gemm.cuh and include/xclip_b200.h).
+#include "gemm.cuh"
 #include "host.h"
 
 namespace xclip {
 
 template <int BLOCK_N, int A_MAJOR, int B_MAJOR>
-static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC,
-                       const GemmParams& p, int grid, cudaStream_t stream) {
+static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, int grid,
+                       cudaStream_t stream) {
   using S = GemmSmem<BLOCK_N>;
   auto kern = gemm_bf16_kernel<BLOCK_N, A_MAJOR, B_MAJOR>;
-  {
-    const int rc_attr = ensure_dynamic_smem(reinterpret_cast<const void*>(kern), S::kTotal);
-    if (rc_attr) return rc_attr;
-  }
-  kern<<<grid, kGemmThreads, S::kTotal, stream>>>(tmA, tmB, tmC, p);
+  const int rc_attr = ensure_dynamic_smem(reinterpret_cast<const void*>(kern), S::kTotal);
+  if (rc_attr) return rc_attr;
+  kern<<<grid, kGemmThreads, S::kTotal, stream>>>(tmA, tmB, p);
   XCLIP_LAUNCH_CHECK("gemm_bf16_kernel");
   return XCLIP_OK;
 }
 
 template <int BLOCK_N>
 static int dispatch_major(int a_major, int b_major, const CUtensorMap& tmA, const CUtensorMap& tmB,
-                          const CUtensorMap& tmC, const GemmParams& p, int grid,
-                          cudaStream_t stream) {
+                          const GemmParams& p, int grid, cudaStream_t stream) {
   if (a_major == kMajorK && b_major == kMajorK)
-    return launch_gemm<BLOCK_N, kMajorK, kMajorK>(tmA, tmB, tmC, p, grid, stream);
+    return launch_gemm<BLOCK_N, kMajorK, kMajorK>(tmA, tmB, p, grid, stream);
   if (a_major == kMajorK && b_major == kMajorMN)
-    return launch_gemm<BLOCK_N, kMajorK, kMajorMN>(tmA, tmB, tmC, p, grid, stream);
+    return launch_gemm<BLOCK_N, kMajorK, kMajorMN>(tmA, tmB, p, grid, stream);
   if (a_major == kMajorMN && b_major == kMajorK)
-    return launch_gemm<BLOCK_N, kMajorMN, kMajorK>(tmA, tmB, tmC, p, grid, stream);
-  return launch_gemm<BLOCK_N, kMajorMN, kMajorMN>(tmA, tmB, tmC, p, grid, stream);
+    return launch_gemm<BLOCK_N, kMajorMN, kMajorK>(tmA, tmB, p, grid, stream);
+  return launch_gemm<BLOCK_N, kMajorMN, kMajorMN>(tmA, tmB, p, grid, stream);
 }
-
-template <int A_MAJOR, int B_MAJOR>
-static int launch_gemm_pair(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC,
-                            const GemmParams& p, int pairs, cudaStream_t stream) {
-  using S = PairCfg<PEPI_STORE>;
-  auto kern = gemm_pair_kernel<A_MAJOR, B_MAJOR, PEPI_STORE>;
-  const int rc_attr = ensure_dynamic_smem(reinterpret_cast<const void*>(kern), S::kTotal);
-  if (rc_attr) return rc_attr;
-  kern<<<2 * pairs, S::kThreads, S::kTotal, stream>>>(tmA, tmB, tmC, tmC, p);   // __cluster_dims__(2,1,1)
-  XCLIP_LAUNCH_CHECK("gemm_pair_kernel");
-  return XCLIP_OK;
-}
-
-static int dispatch_pair(int a_major, int b_major, const CUtensorMap& tmA, const CUtensorMap& tmB,
-                         const CUtensorMap& tmC, const GemmParams& p, int pairs, cudaStream_t stream) {
-  if (a_major == kMajorK && b_major == kMajorK)
-    return launch_gemm_pair<kMajorK, kMajorK>(tmA, tmB, tmC, p, pairs, stream);
-  if (a_major == kMajorK && b_major == kMajorMN)
-    return launch_gemm_pair<kMajorK, kMajorMN>(tmA, tmB, tmC, p, pairs, stream);
-  if (a_major == kMajorMN && b_major == kMajorK)
-    return launch_gemm_pair<kMajorMN, kMajorK>(tmA, tmB, tmC, p, pairs, stream);
-  return launch_gemm_pair<kMajorMN, kMajorMN>(tmA, tmB, tmC, p, pairs, stream);
-}
-
-static int g_pair_mode = 1;
 
 }  // namespace xclip
-
-extern "C" int xclip_gemm_set_pair_mode(int enabled) {
-  const int prev = xclip::g_pair_mode;
-  xclip::g_pair_mode = enabled ? 1 : 0;
-  return prev;
-}
 
 extern "C" int xclip_gemm_bf16(const void* a, int64_t lda, int a_major, const void* b, int64_t ldb,
                                int b_major, void* c, int64_t ldc, int c_dtype, int M, int N, int K,
@@ -96,9 +62,6 @@ extern "C" int xclip_gemm_bf16(const void* a, int64_t lda, int a_major, const vo
   if (bias) XCLIP_REQUIRE((reinterpret_cast<uintptr_t>(bias) & 15) == 0, "gemm: bias misaligned");
 
   const int block_n = (N % 256 == 0 || N > 1024) ? 256 : 128;
-  // CTA-pair kernel (256 x 256 tiles, see gemm.cuh): whenever the single-CTA kernel would use 256-wide
-  // tiles and there are at least two 128-row blocks to pair up
-  const bool use_pair = g_pair_mode && block_n == 256 && M > kGemmBlockM;
 
   CUtensorMap tmA, tmB;
   if (a_major == 0) {
@@ -108,16 +71,14 @@ extern "C" int xclip_gemm_bf16(const void* a, int64_t lda, int a_major, const vo
   }
   if (rc) return rc;
   if (b_major == 0) {
-    rc = encode_2d_bf16(&tmB, b, (uint64_t)K, (uint64_t)N, (uint64_t)ldb, 64,
-                        use_pair ? 128u : (uint32_t)block_n);
+    rc = encode_2d_bf16(&tmB, b, (uint64_t)K, (uint64_t)N, (uint64_t)ldb, 64, (uint32_t)block_n);
   } else {
     rc = encode_2d_bf16(&tmB, b, (uint64_t)N, (uint64_t)K, (uint64_t)ldb, 64, kGemmBlockK);
   }
   if (rc) return rc;
 
-  const int tile_m = use_pair ? 2 * kGemmBlockM : kGemmBlockM;
-  const int units = use_pair ? num_sms() / 2 : num_sms();      // CTAs or CTA pairs that run concurrently
-  const int num_m = (M + tile_m - 1) / tile_m;
+  const int units = num_sms();      // CTAs that run concurrently (one per SM)
+  const int num_m = (M + kGemmBlockM - 1) / kGemmBlockM;
   const int num_n = (N + block_n - 1) / block_n;
   const int num_kb = (K + kGemmBlockK - 1) / kGemmBlockK;
   const long long tiles_mn = (long long)num_m * num_n;
@@ -154,14 +115,7 @@ extern "C" int xclip_gemm_bf16(const void* a, int64_t lda, int a_major, const vo
   p.residual = reinterpret_cast<const bf16*>(residual); p.ldr = ldr; p.res_row_mod = res_row_mod;
   p.res_row_idx = res_row_idx;
 
-  CUtensorMap tmC = tmA;   // placeholder unless the TMA-store epilogue is used
-  if (c_dtype == 0) {
-    rc = encode_2d_bf16(&tmC, c, (uint64_t)N, (uint64_t)M, (uint64_t)ldc, 64, kGemmBlockM);
-    if (rc) return rc;
-    p.use_tma_store = 1;
-  }
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  if (use_pair) return dispatch_pair(a_major, b_major, tmA, tmB, tmC, p, grid, s);
-  if (block_n == 256) return dispatch_major<256>(a_major, b_major, tmA, tmB, tmC, p, grid, s);
-  return dispatch_major<128>(a_major, b_major, tmA, tmB, tmC, p, grid, s);
+  if (block_n == 256) return dispatch_major<256>(a_major, b_major, tmA, tmB, p, grid, s);
+  return dispatch_major<128>(a_major, b_major, tmA, tmB, p, grid, s);
 }

@@ -51,9 +51,9 @@ static int do_init() {
   e = cudaGetDeviceProperties(&prop, dev);
   if (e != cudaSuccess)
     return fail(XCLIP_ERR_CUDA, "cudaGetDeviceProperties failed: %s", cudaGetErrorString(e));
-  if (prop.major != 10)
+  if (prop.major != 9 || prop.minor != 0)
     return fail(XCLIP_ERR_UNSUPPORTED,
-                "x_clip_b200 needs an sm_100 (B200) device; device %d is sm_%d%d - there is no "
+                "x_clip_b200 needs an sm_90 (H100) device; device %d is sm_%d%d - there is no "
                 "fallback path",
                 dev, prop.major, prop.minor);
   g_sms = prop.multiProcessorCount;
@@ -136,14 +136,14 @@ int encode_3d_bf16(CUtensorMap* out, const void* ptr, uint64_t inner, uint64_t m
 }  // namespace xclip
 
 namespace xclip {
-static int g_tune[8] = {1, 0, 0, 0, 0, 0, 0, 0};   // XCLIP_TUNE_FF_BWD_VARIANT = 1 (TMA-pipelined)
+static int g_tune[8] = {0, 0, 0, 0, 0, 0, 0, 0};
 int tune(int knob) { return (knob >= 0 && knob < 8) ? g_tune[knob] : 0; }
 }  // namespace xclip
 
 extern "C" {
 
 int xclip_tune_set(int knob, int value) {
-  if (knob < 0 || knob >= 8) return -1;
+  if (knob != XCLIP_TUNE_LN_FWD_BLOCKS && knob != XCLIP_TUNE_LN_BWD_BLOCKS) return -1;
   const int prev = xclip::g_tune[knob];
   xclip::g_tune[knob] = value;
   return prev;

@@ -1,7 +1,7 @@
 // All-pairs similarity + InfoNCE / DCL loss (reference x_clip/x_clip.py:813-847) on top of the
-// tcgen05 GEMM mainloop (gemm.cuh) with loss-specific epilogues:
+// wgmma GEMM mainloop (gemm.cuh) with loss-specific epilogues:
 //
-//   forward  : s = exp(temperature) * A B^T is produced tile by tile in TMEM and immediately
+//   forward  : s = exp(temperature) * A B^T is produced tile by tile in registers and immediately
 //              reduced to per-row, per-column-block (running max, sum of exp(s - max)) pairs;
 //              the B_l x B_g logits matrix is never written.  A finalize kernel turns the partials into log-denominators
 //              and the loss contribution  scale * sum_r (lse_r - s_rr).
@@ -48,15 +48,15 @@ nce_finalize_kernel(const float* __restrict__ part, int nblk, const float* __res
 }
 
 template <int BLOCK_N, int EPI>
-static int launch_nce(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC,
-                      const GemmParams& p, int grid, cudaStream_t stream) {
+static int launch_nce(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, int grid,
+                      cudaStream_t stream) {
   using S = GemmSmem<BLOCK_N>;
   auto kern = gemm_bf16_kernel<BLOCK_N, kMajorK, kMajorK, EPI>;
   {
     const int rc_attr = ensure_dynamic_smem(reinterpret_cast<const void*>(kern), S::kTotal);
     if (rc_attr) return rc_attr;
   }
-  kern<<<grid, kGemmThreads, S::kTotal, stream>>>(tmA, tmB, tmC, p);
+  kern<<<grid, kGemmThreads, S::kTotal, stream>>>(tmA, tmB, p);
   XCLIP_LAUNCH_CHECK("gemm_bf16_kernel<nce>");
   return XCLIP_OK;
 }
@@ -104,8 +104,8 @@ extern "C" int xclip_nce_fwd(const void* a, const void* b, int R, int C, int D,
   p.alpha_dev = temp_exp; p.diag_offset = diag_offset; p.dcl = dcl;
   p.nce_part = part_ws; p.nce_pos = pos;
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  rc = block_n == 256 ? launch_nce<256, EPI_NCE_FWD>(tmA, tmB, tmA, p, grid, s)
-                      : launch_nce<128, EPI_NCE_FWD>(tmA, tmB, tmA, p, grid, s);
+  rc = block_n == 256 ? launch_nce<256, EPI_NCE_FWD>(tmA, tmB, p, grid, s)
+                      : launch_nce<128, EPI_NCE_FWD>(tmA, tmB, p, grid, s);
   if (rc) return rc;
   const int nblk = xclip_nce_num_col_blocks(C);
   int fgrid = (R + 1023) / 1024;
@@ -134,10 +134,7 @@ extern "C" int xclip_nce_bwd(const void* a, const void* b, int R, int C, int D,
   p.lse_row = lse_row; p.lse_col = lse_col;
   p.w_row = w_row; p.w_col = w_col; p.w_diag = w_diag;
   p.c = g; p.ldc = ldg; p.dtemp = dtemp;
-  CUtensorMap tmC;   // g [R, ldg] written in [128 rows x 64 columns] boxes; pad columns [C, ldg) get zeros
-  rc = encode_2d_bf16(&tmC, g, (uint64_t)ldg, (uint64_t)R, (uint64_t)ldg, 64, kGemmBlockM);
-  if (rc) return rc;
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  return block_n == 256 ? launch_nce<256, EPI_NCE_BWD>(tmA, tmB, tmC, p, grid, s)
-                        : launch_nce<128, EPI_NCE_BWD>(tmA, tmB, tmC, p, grid, s);
+  return block_n == 256 ? launch_nce<256, EPI_NCE_BWD>(tmA, tmB, p, grid, s)
+                        : launch_nce<128, EPI_NCE_BWD>(tmA, tmB, p, grid, s);
 }

@@ -540,8 +540,8 @@ class ChunkedClipLossFn(torch.autograd.Function):
       2. one contrastive loss over ALL latents (with the usual cross-rank all-gather)
       3. in backward: d loss / d latents, then back-propagate the matching slice of the latent
          gradient through every chunk's encoders.
-    B200-first memory plan: a chunk's saved activations are KEPT from step 1 for as many chunks as
-    the 180 GB of HBM hold (`retain`: "auto" measures the first chunk's footprint and plans against
+    Memory plan: a chunk's saved activations are KEPT from step 1 for as many chunks as
+    the GPU's HBM holds (80 GB on an H100) (`retain`: "auto" measures the first chunk's footprint and plans against
     the free memory; an int fixes the count; 0 = none); only the remaining chunks are encoded
     without saving anything and re-encoded in step 3 (RNG replayed for PatchDropout).  Retained
     chunks cost no extra flops; each re-encoded chunk costs one extra encoder forward."""

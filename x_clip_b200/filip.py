@@ -3,7 +3,7 @@
 Schedule (see csrc/filip.cu): two segment-max GEMM passes (text tokens x image tokens and the
 transposed orientation, fp32-accurate through the split-bf16 operands), two tiny reductions to the
 [B,B] similarity matrices, row-wise InfoNCE/DCL; backward re-expands the saved argmax into a
-one-hot weighted bf16 operand chunk by chunk and runs two plain tcgen05 GEMMs per chunk.
+one-hot weighted bf16 operand chunk by chunk and runs two plain wgmma GEMMs per chunk.
 The 6-D similarity tensor of the reference is never materialised.  Under data parallelism the
 image-token operands are all-gathered and each rank owns the rows of its local texts (the
 reference itself cannot all-gather FILIP latents, SURVEY.md 8c - what W ranks must reproduce is

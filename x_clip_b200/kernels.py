@@ -243,10 +243,9 @@ def attn_bwd(qkv, key_mask, o, d_o, lse, B, n, heads, scale, causal=False):
     _need(d_o, BF16, "d_o"); _rows2d(d_o, "d_o")
     dqkv = torch.empty_like(qkv)
     delta = torch.empty((B, heads, n), device=qkv.device, dtype=F32)
-    ws = torch.empty((B * n, heads * 64), device=qkv.device, dtype=F32) if n > 128 else None
     _call(qkv, "attn_bwd", 10.0 * B * heads * n * n * 64, 2.0 * B * n * heads * 64 * 8, "xclip_attn_bwd", qkv.data_ptr(), qkv.stride(0), _ptr(key_mask), o.data_ptr(),
               o.stride(0), d_o.data_ptr(), d_o.stride(0), lse.data_ptr(), delta.data_ptr(),
-              dqkv.data_ptr(), dqkv.stride(0), _ptr(ws), B, n, heads, float(scale),
+              dqkv.data_ptr(), dqkv.stride(0), None, B, n, heads, float(scale),
               1 if causal else 0)
     return dqkv
 
