@@ -49,6 +49,7 @@ void xclip_launch_count_reset(void);
  * results are identical either way).  Returns the previous value, -1 for an unknown knob. */
 #define XCLIP_TUNE_LN_FWD_BLOCKS 3 /* LayerNorm forward: cap on resident blocks per SM (0 = built-in 8) */
 #define XCLIP_TUNE_LN_BWD_BLOCKS 4 /* LayerNorm backward: blocks per SM (0 = built-in 2) */
+#define XCLIP_TUNE_ATTN_STREAM 5   /* attention: != 0 runs the streaming kernels at every n (0 = only n > 320) */
 int xclip_tune_set(int knob, int value);
 
 /* ---- dense contraction (wgmma) ------------------------------------------
@@ -106,8 +107,11 @@ int xclip_l2norm_bwd(const float* dz, const float* z, const float* inv, void* dp
 int xclip_cast_f32_bf16(const float* src, void* dst, int64_t n, xclip_stream_t stream);
 
 /* ---- fused attention ------------------------------------------------------
- * Attention core of x_clip/x_clip.py:217-244 (dim_head = 64, n <= 320).  causal != 0 adds the
+ * Attention core of x_clip/x_clip.py:217-244 (dim_head = 64, any n).  causal != 0 adds the
  * reference's causal mask (keys j > i get -FLT_MAX, :233-236).
+ * n <= 320 runs kernels that hold a head's whole K and V (Q and dO in the backward) in shared
+ * memory; n > 320 runs kernels that stream them through shared memory in 64-row blocks (~40-50 KB
+ * per CTA for any n).  Both compute the same blocks in the same order: bit-identical results.
  * qkv bf16 [B*n, ld_qkv] holds q | k | v, each heads*64 wide, head-major inside.
  * key_mask uint8 [B, n] (1 = attend; may be NULL).  o bf16 [B*n, ldo] (heads merged).
  * lse f32 [B, heads, n]: base-2 log-sum-exp of scale*log2(e)*scores (saved for backward). */

@@ -6,8 +6,10 @@ the parameter tree (`state_dict` keys and shapes, SURVEY.md 8b) mirror the refer
 working.  The modules here are parameter CONTAINERS: all arithmetic on the hot path is
 done by the CUDA kernels behind include/xclip_b200.h, scheduled by x_clip_b200.engine.
 
-Feature combinations the kernels do not cover raise at construction (never a silent CPU or
-eager fallback): dim_head != 64, model dims not multiples of 256, a causal text tower longer than
+Sequence length is not limited by the non-causal attention: image towers such as ViT-B/16 at 384 px
+(576 patches) and long text towers run on the same kernels (streamed through shared memory above
+320 tokens).  Feature combinations the kernels do not cover raise at construction (never a silent
+CPU or eager fallback): dim_head != 64, model dims not multiples of 256, a causal text tower longer than
 128 tokens, rotary + causal together (broken in the reference itself: n+1 angles for n tokens,
 x_clip.py:328), dropout > 0, the similarity-regularisation term and conv-downsampled image
 latents.  MLM, SimSiam / SimCLR and the multiview term run through the fast encoders (aux.py).
@@ -181,7 +183,6 @@ class TextTransformer(nn.Module):
         _require(not (rotary_pos_emb and causal),
                  "text_rotary_pos_emb with text_causal_mask is broken in the reference itself "
                  "(n+1 rotary positions for n tokens, x_clip.py:328) and not offered here")
-        _require(max_seq_len + 1 <= 320, "text_seq_len + CLS must be <= 320 tokens")
         _require(not causal or max_seq_len <= 128, "text_causal_mask needs text_seq_len <= 128")
         self.token_emb = nn.Embedding(num_tokens, dim)
         self.abs_pos_emb = nn.Embedding(max_seq_len, dim) if not rotary_pos_emb else None
@@ -222,7 +223,6 @@ class VisionTransformer(nn.Module):
         num_patches = (image_size // patch_size) ** 2
         patch_dim = channels * patch_size ** 2
         _require(patch_dim % 8 == 0, "channels * patch_size^2 must be a multiple of 8")
-        _require(num_patches <= 320, "at most 320 image patches are supported")
         self.to_tokens = nn.Sequential(_Slot(), nn.Linear(patch_dim, dim))
         self.pos_emb = nn.Embedding(num_patches, dim)
         self.patch_dropout = PatchDropout(patch_dropout)

@@ -1,16 +1,23 @@
-// Fused attention core of x_clip/x_clip.py:217-244 for dim_head = 64 and n <= 320 (sm_90a).
+// Fused attention core of x_clip/x_clip.py:217-244 for dim_head = 64 and any sequence length (sm_90a).
 //
 // One CTA = 4 warps = 64 rows of one (batch, head) (1-D grid: row block fastest, then head, then
 // batch); every warp owns 16 rows and runs bf16
 // m16n8k16 tensor-core MMAs on fragments loaded from XOR-swizzled shared memory with ldmatrix.
-// A whole head's keys and values (<= 320 x 64 bf16 each) fit in shared memory, so each CTA loads
-// its operands once and loops over 64-wide blocks in shared memory.
 //   forward : O = softmax(scale q k^T) v with an online softmax; lse = base-2 log-sum-exp.
 //   backward: delta = rowsum(dO * O); one kernel per 64-key block accumulates dK, dV over all
 //             queries, one per 64-query block accumulates dQ over all keys (P and dP recomputed),
 //             so every gradient is written exactly once, without atomics.
+// Two schedules run the same per-block bodies (attn_*_block) in the same block order, so they give
+// bit-identical results:
+//   resident  (n <= 320): a whole head's other operand (<= 320 x 64 bf16 per tensor) is loaded into
+//             shared memory once and the CTA loops over its 64-row blocks there (up to ~100 KB).
+//   streaming (n > 320) : only the CTA's own 64-row block stays on chip; the other operand passes
+//             through a 2-stage cp.async ring of 64-row blocks (with their key flags or lse / delta
+//             values), ~40-50 KB per CTA whatever n is.  XCLIP_TUNE_ATTN_STREAM forces it for any n.
 // Masking follows the reference: a masked key (key_mask = 0, or j > i under the causal mask of
-// :233-236) gets the score -FLT_MAX after scaling; keys beyond n do not exist (-inf).
+// :233-236) gets the score -FLT_MAX after scaling; keys beyond n do not exist (-inf).  Causal blocks
+// wholly above the diagonal are not skipped: a row whose visible keys are all key-masked gets the
+// reference's uniform softmax over all n keys.
 #include "common.cuh"
 #include "host.h"
 
@@ -19,6 +26,8 @@ namespace xclip {
 constexpr int kAttnDh = 64;
 constexpr int kAttnRows = 64;       // rows (queries or keys) per CTA
 constexpr int kAttnThreads = 128;
+constexpr int kAttnTile = kAttnRows * 128;  // bytes of one swizzled 64 x 64 bf16 tile
+constexpr int kAttnResidentMaxN = 320;      // longest sequence the resident kernels take
 constexpr float kLog2e = 1.4426950408889634f;
 
 // byte offset of 16-byte chunk `chunk` of row `row` in a [rows x 64] bf16 tile (128 B rows)
@@ -119,11 +128,11 @@ __device__ __forceinline__ void zero_acc(float (&a)[8][4]) {
 }
 
 // key flags: 0 = attend, 1 = masked (score -FLT_MAX), 2 = no such key (j >= n)
+__device__ __forceinline__ uint8_t key_flag(const uint8_t* mask, int b, int n, int gj) {
+  return gj >= n ? 2 : ((mask != nullptr && !mask[(long long)b * n + gj]) ? 1 : 0);
+}
 __device__ __forceinline__ void load_key_flags(uint8_t* flags, const uint8_t* mask, int b, int n, int j0, int cnt) {
-  for (int j = threadIdx.x; j < cnt; j += kAttnThreads) {
-    const int gj = j0 + j;
-    flags[j] = gj >= n ? 2 : ((mask != nullptr && !mask[(long long)b * n + gj]) ? 1 : 0);
-  }
+  for (int j = threadIdx.x; j < cnt; j += kAttnThreads) flags[j] = key_flag(mask, b, n, j0 + j);
 }
 
 // scaled, masked score in the base-2 domain
@@ -149,6 +158,142 @@ __device__ __forceinline__ void store_rows(bf16* dst, long long ld, int r0, int 
   }
 }
 
+// ---- per-block bodies, shared by the resident and the streaming kernels ---------------------------
+// Each processes one 64-row block of the streamed operand for the warp's 16 rows.  The block's tiles
+// sit at rows [c0, c0 + 64) of tK / tV (tQ / tdO); kb (qb) is the block's first global row and
+// flags[j] (lse_b[j], delta_b[j]) belong to global row kb + j (qb + j).
+
+// forward: s = q k^T, online-softmax update of (m, l, oacc), oacc += p v
+template <bool kCausal>
+__device__ __forceinline__ void attn_fwd_block(const uint32_t (&qf)[4][4], const uint8_t* tK, const uint8_t* tV,
+                                               int c0, const uint8_t* flags, int kb, const int (&row)[2],
+                                               float scale_log2, float (&m)[2], float (&l)[2],
+                                               float (&oacc)[8][4]) {
+  const int lane = threadIdx.x & 31;
+  float s[8][4];
+  zero_acc(s);
+  mma_abt(s, qf, tK, c0);
+  float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+  for (int nt = 0; nt < 8; ++nt)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int j = nt * 8 + 2 * (lane & 3) + (e & 1);
+      const float t = attn_t(s[nt][e], scale_log2, flags[j], kCausal && kb + j > row[e >> 1]);
+      s[nt][e] = t;
+      mx[e >> 1] = fmaxf(mx[e >> 1], t);
+    }
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
+    mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 2));
+    const float mn = fmaxf(m[hh], mx[hh]);
+    const float corr = exp2f(m[hh] - mn);
+    m[hh] = mn;
+    l[hh] *= corr;
+#pragma unroll
+    for (int nt = 0; nt < 8; ++nt) {
+      oacc[nt][2 * hh] *= corr;
+      oacc[nt][2 * hh + 1] *= corr;
+    }
+  }
+#pragma unroll
+  for (int nt = 0; nt < 8; ++nt)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const float pv = exp2f(s[nt][e] - m[e >> 1]);
+      s[nt][e] = pv;
+      l[e >> 1] += pv;
+    }
+  uint32_t pf[4][4];
+  acc_to_a(s, pf);
+  mma_ab(oacc, pf, tV, c0);
+}
+
+// forward epilogue: o = oacc / l for rows [rr0, rr0 + 16) (o and lse_bh point at this (batch, head))
+__device__ __forceinline__ void attn_fwd_finish(float (&oacc)[8][4], const float (&m)[2], float (&l)[2],
+                                                const int (&row)[2], bf16* o, long long ldo, int rr0,
+                                                float* lse_bh, int n) {
+  const int lane = threadIdx.x & 31;
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 1);
+    l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 2);
+  }
+  const float inv[2] = {1.f / l[0], 1.f / l[1]};
+#pragma unroll
+  for (int nt = 0; nt < 8; ++nt)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) oacc[nt][e] *= inv[e >> 1];
+  store_rows(o, ldo, rr0, n, oacc, 1.f);
+  if ((lane & 3) == 0) {
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh)
+      if (row[hh] < n) lse_bh[row[hh]] = m[hh] + log2f(l[hh]);
+  }
+}
+
+// dK / dV: the warp's accumulators are S^T / dP^T (keys x queries), so P^T and dS^T feed the next
+// MMAs straight from registers.  key[] are the thread's two global key rows, flag[] their flags.
+template <bool kCausal>
+__device__ __forceinline__ void attn_dkdv_block(const uint32_t (&kf)[4][4], const uint32_t (&vf)[4][4],
+                                                const uint8_t* tQ, const uint8_t* tdO, int c0,
+                                                const float* lse_b, const float* delta_b, int qb,
+                                                const int (&key)[2], const int (&flag)[2], int n,
+                                                float scale_log2, float (&dk)[8][4], float (&dv)[8][4]) {
+  const int lane = threadIdx.x & 31;
+  float st[8][4], dpt[8][4];
+  zero_acc(st);
+  zero_acc(dpt);
+  mma_abt(st, kf, tQ, c0);
+  mma_abt(dpt, vf, tdO, c0);
+#pragma unroll
+  for (int nt = 0; nt < 8; ++nt)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int j = nt * 8 + 2 * (lane & 3) + (e & 1);
+      const int q = qb + j;
+      const float t = q < n ? attn_t(st[nt][e], scale_log2, flag[e >> 1], kCausal && key[e >> 1] > q) : -INFINITY;
+      const float pv = exp2f(t - lse_b[j]);
+      st[nt][e] = pv;
+      dpt[nt][e] = pv * (dpt[nt][e] - delta_b[j]);
+    }
+  uint32_t pf[4][4], df[4][4];
+  acc_to_a(st, pf);
+  acc_to_a(dpt, df);
+  mma_ab(dv, pf, tdO, c0);
+  mma_ab(dk, df, tQ, c0);
+}
+
+// dQ: ds = p (dp - delta) over one block of keys, dq += ds k
+template <bool kCausal>
+__device__ __forceinline__ void attn_dq_block(const uint32_t (&qf)[4][4], const uint32_t (&of)[4][4],
+                                              const uint8_t* tK, const uint8_t* tV, int c0,
+                                              const uint8_t* flags, int kb, const int (&row)[2], int n,
+                                              const float (&lr)[2], const float (&dr)[2], float scale_log2,
+                                              float (&dq)[8][4]) {
+  const int lane = threadIdx.x & 31;
+  float s[8][4], dp[8][4];
+  zero_acc(s);
+  zero_acc(dp);
+  mma_abt(s, qf, tK, c0);
+  mma_abt(dp, of, tV, c0);
+#pragma unroll
+  for (int nt = 0; nt < 8; ++nt)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int j = nt * 8 + 2 * (lane & 3) + (e & 1);
+      const float t = attn_t(s[nt][e], scale_log2, flags[j], kCausal && kb + j > row[e >> 1]);
+      const float pv = row[e >> 1] < n ? exp2f(t - lr[e >> 1]) : 0.f;
+      s[nt][e] = pv * (dp[nt][e] - dr[e >> 1]);
+    }
+  uint32_t df[4][4];
+  acc_to_a(s, df);
+  mma_ab(dq, df, tK, c0);
+}
+
+// ---- forward ------------------------------------------------------------------------------------
+// resident: the head's whole K, V and key flags in shared memory
 template <bool kCausal>
 __global__ void __launch_bounds__(kAttnThreads)
 attn_fwd_kernel(const bf16* __restrict__ qkv, long long ld, const uint8_t* __restrict__ mask,
@@ -156,7 +301,7 @@ attn_fwd_kernel(const bf16* __restrict__ qkv, long long ld, const uint8_t* __res
   extern __shared__ __align__(128) uint8_t sm[];
   const int NP = (n + 63) & ~63;
   uint8_t* sQ = sm;
-  uint8_t* sK = sQ + kAttnRows * 128;
+  uint8_t* sK = sQ + kAttnTile;
   uint8_t* sV = sK + NP * 128;
   uint8_t* sFlag = sV + NP * 128;
   const int nblk = NP / kAttnRows, bh_ = blockIdx.x / nblk;
@@ -178,63 +323,62 @@ attn_fwd_kernel(const bf16* __restrict__ qkv, long long ld, const uint8_t* __res
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
   float oacc[8][4];
   zero_acc(oacc);
+  for (int kb = 0; kb < NP; kb += 64)
+    attn_fwd_block<kCausal>(qf, sK, sV, kb, sFlag + kb, kb, row, scale_log2, m, l, oacc);
+  attn_fwd_finish(oacc, m, l, row, o + (long long)b * n * ldo + h * kAttnDh, ldo, q0 + r0,
+                  lse + ((long long)b * H + h) * n, n);
+}
 
-  for (int kb = 0; kb < NP; kb += 64) {
-    float s[8][4];
-    zero_acc(s);
-    mma_abt(s, qf, sK, kb);
-    float mx[2] = {-INFINITY, -INFINITY};
-#pragma unroll
-    for (int nt = 0; nt < 8; ++nt)
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int col = kb + nt * 8 + 2 * (lane & 3) + (e & 1);
-        const float t = attn_t(s[nt][e], scale_log2, sFlag[col], kCausal && col > row[e >> 1]);
-        s[nt][e] = t;
-        mx[e >> 1] = fmaxf(mx[e >> 1], t);
-      }
-#pragma unroll
-    for (int hh = 0; hh < 2; ++hh) {
-      mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
-      mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 2));
-      const float mn = fmaxf(m[hh], mx[hh]);
-      const float corr = exp2f(m[hh] - mn);
-      m[hh] = mn;
-      l[hh] *= corr;
-#pragma unroll
-      for (int nt = 0; nt < 8; ++nt) {
-        oacc[nt][2 * hh] *= corr;
-        oacc[nt][2 * hh + 1] *= corr;
-      }
+// streaming: the CTA's Q block stays; K, V and key flags of 64-key block i + 1 are fetched into the
+// other ring stage while block i is computed (flags through a register, K and V by cp.async)
+template <bool kCausal>
+__global__ void __launch_bounds__(kAttnThreads)
+attn_fwd_stream_kernel(const bf16* __restrict__ qkv, long long ld, const uint8_t* __restrict__ mask,
+                       bf16* __restrict__ o, long long ldo, float* __restrict__ lse, int n, int H,
+                       float scale_log2) {
+  extern __shared__ __align__(128) uint8_t sm[];
+  uint8_t* sQ = sm;
+  uint8_t* ring = sQ + kAttnTile;            // stage s: K tile at ring + 2 s kAttnTile, V tile after it
+  uint8_t* sFlag = ring + 4 * kAttnTile;     // stage s: 64 key flags at sFlag + 64 s
+  const int nblk = (n + 63) / kAttnRows, bh_ = blockIdx.x / nblk;
+  const int b = bh_ / H, h = bh_ % H;
+  const int q0 = (blockIdx.x % nblk) * kAttnRows;
+  const bf16* base = qkv + (long long)b * n * ld;
+  const bf16* gK = base + (H + h) * kAttnDh;
+  const bf16* gV = base + (2 * H + h) * kAttnDh;
+  attn_load_rows(sQ, base + h * kAttnDh, ld, q0, kAttnRows, n);
+  attn_load_rows(ring, gK, ld, 0, kAttnRows, n);
+  attn_load_rows(ring + kAttnTile, gV, ld, 0, kAttnRows, n);
+  load_key_flags(sFlag, mask, b, n, 0, kAttnRows);
+  cp_async_wait_all();
+  __syncthreads();
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int r0 = warp * 16;
+  uint32_t qf[4][4];
+  load_a_frags(sQ, r0, qf);
+  const int row[2] = {q0 + r0 + (lane >> 2), q0 + r0 + (lane >> 2) + 8};
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  float oacc[8][4];
+  zero_acc(oacc);
+  for (int i = 0; i < nblk; ++i) {
+    const int kb = i * kAttnRows, nxt = (i + 1) & 1;
+    const bool more = i + 1 < nblk;
+    uint8_t next_flag = 0;
+    if (more) {
+      attn_load_rows(ring + nxt * 2 * kAttnTile, gK, ld, kb + kAttnRows, kAttnRows, n);
+      attn_load_rows(ring + nxt * 2 * kAttnTile + kAttnTile, gV, ld, kb + kAttnRows, kAttnRows, n);
+      if (threadIdx.x < kAttnRows) next_flag = key_flag(mask, b, n, kb + kAttnRows + threadIdx.x);
     }
-#pragma unroll
-    for (int nt = 0; nt < 8; ++nt)
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const float pv = exp2f(s[nt][e] - m[e >> 1]);
-        s[nt][e] = pv;
-        l[e >> 1] += pv;
-      }
-    uint32_t pf[4][4];
-    acc_to_a(s, pf);
-    mma_ab(oacc, pf, sV, kb);
+    const uint8_t* cur = ring + (i & 1) * 2 * kAttnTile;
+    attn_fwd_block<kCausal>(qf, cur, cur + kAttnTile, 0, sFlag + (i & 1) * kAttnRows, kb, row, scale_log2,
+                            m, l, oacc);
+    if (more && threadIdx.x < kAttnRows) sFlag[nxt * kAttnRows + threadIdx.x] = next_flag;
+    cp_async_wait_all();   // block i + 1 landed, and no thread reads stage i & 1 any more
+    __syncthreads();
   }
-#pragma unroll
-  for (int hh = 0; hh < 2; ++hh) {
-    l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 1);
-    l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 2);
-  }
-  const float inv[2] = {1.f / l[0], 1.f / l[1]};
-#pragma unroll
-  for (int nt = 0; nt < 8; ++nt)
-#pragma unroll
-    for (int e = 0; e < 4; ++e) oacc[nt][e] *= inv[e >> 1];
-  store_rows(o + (long long)b * n * ldo + h * kAttnDh, ldo, q0 + r0, n, oacc, 1.f);
-  if ((lane & 3) == 0) {
-#pragma unroll
-    for (int hh = 0; hh < 2; ++hh)
-      if (row[hh] < n) lse[((long long)b * H + h) * n + row[hh]] = m[hh] + log2f(l[hh]);
-  }
+  attn_fwd_finish(oacc, m, l, row, o + (long long)b * n * ldo + h * kAttnDh, ldo, q0 + r0,
+                  lse + ((long long)b * H + h) * n, n);
 }
 
 // delta[b,h,i] = sum_d dO[b,i,h,d] * O[b,i,h,d]; one warp per (token, 4 heads at a time)
@@ -272,9 +416,9 @@ attn_delta_kernel(const bf16* __restrict__ o, long long ldo, const bf16* __restr
   }
 }
 
+// ---- backward -----------------------------------------------------------------------------------
 // dK, dV of the 64 keys [k0, k0 + 64) of one (batch, head): loops over all queries.
-// The warp's accumulators are S^T / dP^T (keys x queries), so P^T and dS^T feed the next MMAs
-// straight from registers.
+// resident: the head's whole Q, dO, lse and delta in shared memory
 template <bool kCausal>
 __global__ void __launch_bounds__(kAttnThreads)
 attn_bwd_dkdv_kernel(const bf16* __restrict__ qkv, long long ld, const uint8_t* __restrict__ mask,
@@ -284,8 +428,8 @@ attn_bwd_dkdv_kernel(const bf16* __restrict__ qkv, long long ld, const uint8_t* 
   extern __shared__ __align__(128) uint8_t sm[];
   const int NP = (n + 63) & ~63;
   uint8_t* sK = sm;
-  uint8_t* sV = sK + kAttnRows * 128;
-  uint8_t* sQ = sV + kAttnRows * 128;
+  uint8_t* sV = sK + kAttnTile;
+  uint8_t* sQ = sV + kAttnTile;
   uint8_t* sdO = sQ + NP * 128;
   float* sLse = reinterpret_cast<float*>(sdO + NP * 128);
   float* sDelta = sLse + NP;
@@ -313,33 +457,79 @@ attn_bwd_dkdv_kernel(const bf16* __restrict__ qkv, long long ld, const uint8_t* 
   load_a_frags(sK, r0, kf);
   load_a_frags(sV, r0, vf);
   const int kr[2] = {r0 + (lane >> 2), r0 + (lane >> 2) + 8};   // key rows inside the block
+  const int key[2] = {k0 + kr[0], k0 + kr[1]};
   const int flag[2] = {sFlag[kr[0]], sFlag[kr[1]]};
   float dk[8][4], dv[8][4];
   zero_acc(dk);
   zero_acc(dv);
+  for (int qb = 0; qb < NP; qb += 64)
+    attn_dkdv_block<kCausal>(kf, vf, sQ, sdO, qb, sLse + qb, sDelta + qb, qb, key, flag, n, scale_log2, dk, dv);
+  bf16* out = dqkv + (long long)b * n * ldd;
+  store_rows(out + (H + h) * kAttnDh, ldd, k0 + r0, n, dk, scale);
+  store_rows(out + (2 * H + h) * kAttnDh, ldd, k0 + r0, n, dv, 1.f);
+}
 
-  for (int qb = 0; qb < NP; qb += 64) {
-    float st[8][4], dpt[8][4];
-    zero_acc(st);
-    zero_acc(dpt);
-    mma_abt(st, kf, sQ, qb);
-    mma_abt(dpt, vf, sdO, qb);
-#pragma unroll
-    for (int nt = 0; nt < 8; ++nt)
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int q = qb + nt * 8 + 2 * (lane & 3) + (e & 1);
-        const int key = k0 + kr[e >> 1];
-        const float t = q < n ? attn_t(st[nt][e], scale_log2, flag[e >> 1], kCausal && key > q) : -INFINITY;
-        const float pv = exp2f(t - sLse[q]);
-        st[nt][e] = pv;
-        dpt[nt][e] = pv * (dpt[nt][e] - sDelta[q]);
-      }
-    uint32_t pf[4][4], df[4][4];
-    acc_to_a(st, pf);
-    acc_to_a(dpt, df);
-    mma_ab(dv, pf, sdO, qb);
-    mma_ab(dk, df, sQ, qb);
+// streaming: the CTA's K, V block stays; Q, dO (cp.async) and the 64 lse / delta values (through a
+// register) of query block i + 1 are fetched into the other ring stage while block i is computed
+template <bool kCausal>
+__global__ void __launch_bounds__(kAttnThreads)
+attn_bwd_dkdv_stream_kernel(const bf16* __restrict__ qkv, long long ld, const uint8_t* __restrict__ mask,
+                            const bf16* __restrict__ d_o, long long lddo, const float* __restrict__ lse,
+                            const float* __restrict__ delta, bf16* __restrict__ dqkv, long long ldd, int n,
+                            int H, float scale, float scale_log2) {
+  extern __shared__ __align__(128) uint8_t sm[];
+  uint8_t* sK = sm;
+  uint8_t* sV = sK + kAttnTile;
+  uint8_t* ring = sV + kAttnTile;                            // stage s: Q tile, dO tile at ring + 2 s kAttnTile
+  float* sStat = reinterpret_cast<float*>(ring + 4 * kAttnTile);   // stage s: 64 lse, 64 delta at sStat + 128 s
+  uint8_t* sFlag = reinterpret_cast<uint8_t*>(sStat + 4 * kAttnRows);
+  const int nblk = (n + 63) / kAttnRows, bh_ = blockIdx.x / nblk;
+  const int b = bh_ / H, h = bh_ % H;
+  const int k0 = (blockIdx.x % nblk) * kAttnRows;
+  const bf16* base = qkv + (long long)b * n * ld;
+  const bf16* gQ = base + h * kAttnDh;
+  const bf16* gdO = d_o + (long long)b * n * lddo + h * kAttnDh;
+  const long long bh = (long long)b * H + h;
+  // thread t < 64 carries lse of query qb + t, thread 64 + t delta of query qb + t
+  const float* gStat = (threadIdx.x < kAttnRows ? lse : delta) + bh * n;
+  const int srow = threadIdx.x & (kAttnRows - 1);
+  attn_load_rows(sK, base + (H + h) * kAttnDh, ld, k0, kAttnRows, n);
+  attn_load_rows(sV, base + (2 * H + h) * kAttnDh, ld, k0, kAttnRows, n);
+  attn_load_rows(ring, gQ, ld, 0, kAttnRows, n);
+  attn_load_rows(ring + kAttnTile, gdO, lddo, 0, kAttnRows, n);
+  sStat[threadIdx.x] = srow < n ? gStat[srow] : 0.f;
+  load_key_flags(sFlag, mask, b, n, k0, kAttnRows);
+  cp_async_wait_all();
+  __syncthreads();
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int r0 = warp * 16;
+  uint32_t kf[4][4], vf[4][4];
+  load_a_frags(sK, r0, kf);
+  load_a_frags(sV, r0, vf);
+  const int kr[2] = {r0 + (lane >> 2), r0 + (lane >> 2) + 8};
+  const int key[2] = {k0 + kr[0], k0 + kr[1]};
+  const int flag[2] = {sFlag[kr[0]], sFlag[kr[1]]};
+  float dk[8][4], dv[8][4];
+  zero_acc(dk);
+  zero_acc(dv);
+  for (int i = 0; i < nblk; ++i) {
+    const int qb = i * kAttnRows, nxt = (i + 1) & 1;
+    const bool more = i + 1 < nblk;
+    float next_stat = 0.f;
+    if (more) {
+      attn_load_rows(ring + nxt * 2 * kAttnTile, gQ, ld, qb + kAttnRows, kAttnRows, n);
+      attn_load_rows(ring + nxt * 2 * kAttnTile + kAttnTile, gdO, lddo, qb + kAttnRows, kAttnRows, n);
+      const int q = qb + kAttnRows + srow;
+      if (q < n) next_stat = gStat[q];
+    }
+    const uint8_t* cur = ring + (i & 1) * 2 * kAttnTile;
+    const float* st = sStat + (i & 1) * 2 * kAttnRows;
+    attn_dkdv_block<kCausal>(kf, vf, cur, cur + kAttnTile, 0, st, st + kAttnRows, qb, key, flag, n, scale_log2,
+                             dk, dv);
+    if (more) sStat[nxt * 2 * kAttnRows + threadIdx.x] = next_stat;
+    cp_async_wait_all();   // block i + 1 landed, and no thread reads stage i & 1 any more
+    __syncthreads();
   }
   bf16* out = dqkv + (long long)b * n * ldd;
   store_rows(out + (H + h) * kAttnDh, ldd, k0 + r0, n, dk, scale);
@@ -347,6 +537,7 @@ attn_bwd_dkdv_kernel(const bf16* __restrict__ qkv, long long ld, const uint8_t* 
 }
 
 // dQ of the 64 queries [q0, q0 + 64) of one (batch, head): loops over all keys.
+// resident: the head's whole K, V and key flags in shared memory
 template <bool kCausal>
 __global__ void __launch_bounds__(kAttnThreads)
 attn_bwd_dq_kernel(const bf16* __restrict__ qkv, long long ld, const uint8_t* __restrict__ mask,
@@ -356,8 +547,8 @@ attn_bwd_dq_kernel(const bf16* __restrict__ qkv, long long ld, const uint8_t* __
   extern __shared__ __align__(128) uint8_t sm[];
   const int NP = (n + 63) & ~63;
   uint8_t* sQ = sm;
-  uint8_t* sdO = sQ + kAttnRows * 128;
-  uint8_t* sK = sdO + kAttnRows * 128;
+  uint8_t* sdO = sQ + kAttnTile;
+  uint8_t* sK = sdO + kAttnTile;
   uint8_t* sV = sK + NP * 128;
   uint8_t* sFlag = sV + NP * 128;
   const int nblk = NP / kAttnRows, bh_ = blockIdx.x / nblk;
@@ -387,24 +578,68 @@ attn_bwd_dq_kernel(const bf16* __restrict__ qkv, long long ld, const uint8_t* __
   }
   float dq[8][4];
   zero_acc(dq);
-  for (int kb = 0; kb < NP; kb += 64) {
-    float s[8][4], dp[8][4];
-    zero_acc(s);
-    zero_acc(dp);
-    mma_abt(s, qf, sK, kb);
-    mma_abt(dp, of, sV, kb);
+  for (int kb = 0; kb < NP; kb += 64)
+    attn_dq_block<kCausal>(qf, of, sK, sV, kb, sFlag + kb, kb, row, n, lr, dr, scale_log2, dq);
+  store_rows(dqkv + (long long)b * n * ldd + h * kAttnDh, ldd, q0 + r0, n, dq, scale);
+}
+
+// streaming: the CTA's Q, dO block stays; K, V and key flags of 64-key block i + 1 are fetched into
+// the other ring stage while block i is computed
+template <bool kCausal>
+__global__ void __launch_bounds__(kAttnThreads)
+attn_bwd_dq_stream_kernel(const bf16* __restrict__ qkv, long long ld, const uint8_t* __restrict__ mask,
+                          const bf16* __restrict__ d_o, long long lddo, const float* __restrict__ lse,
+                          const float* __restrict__ delta, bf16* __restrict__ dqkv, long long ldd, int n,
+                          int H, float scale, float scale_log2) {
+  extern __shared__ __align__(128) uint8_t sm[];
+  uint8_t* sQ = sm;
+  uint8_t* sdO = sQ + kAttnTile;
+  uint8_t* ring = sdO + kAttnTile;           // stage s: K tile at ring + 2 s kAttnTile, V tile after it
+  uint8_t* sFlag = ring + 4 * kAttnTile;     // stage s: 64 key flags at sFlag + 64 s
+  const int nblk = (n + 63) / kAttnRows, bh_ = blockIdx.x / nblk;
+  const int b = bh_ / H, h = bh_ % H;
+  const int q0 = (blockIdx.x % nblk) * kAttnRows;
+  const bf16* base = qkv + (long long)b * n * ld;
+  const bf16* gK = base + (H + h) * kAttnDh;
+  const bf16* gV = base + (2 * H + h) * kAttnDh;
+  attn_load_rows(sQ, base + h * kAttnDh, ld, q0, kAttnRows, n);
+  attn_load_rows(sdO, d_o + (long long)b * n * lddo + h * kAttnDh, lddo, q0, kAttnRows, n);
+  attn_load_rows(ring, gK, ld, 0, kAttnRows, n);
+  attn_load_rows(ring + kAttnTile, gV, ld, 0, kAttnRows, n);
+  load_key_flags(sFlag, mask, b, n, 0, kAttnRows);
+  cp_async_wait_all();
+  __syncthreads();
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int r0 = warp * 16;
+  uint32_t qf[4][4], of[4][4];
+  load_a_frags(sQ, r0, qf);
+  load_a_frags(sdO, r0, of);
+  const long long bh = (long long)b * H + h;
+  const int row[2] = {q0 + r0 + (lane >> 2), q0 + r0 + (lane >> 2) + 8};
+  float lr[2], dr[2];
 #pragma unroll
-    for (int nt = 0; nt < 8; ++nt)
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int col = kb + nt * 8 + 2 * (lane & 3) + (e & 1);
-        const float t = attn_t(s[nt][e], scale_log2, sFlag[col], kCausal && col > row[e >> 1]);
-        const float pv = row[e >> 1] < n ? exp2f(t - lr[e >> 1]) : 0.f;
-        s[nt][e] = pv * (dp[nt][e] - dr[e >> 1]);
-      }
-    uint32_t df[4][4];
-    acc_to_a(s, df);
-    mma_ab(dq, df, sK, kb);
+  for (int hh = 0; hh < 2; ++hh) {
+    lr[hh] = row[hh] < n ? lse[bh * n + row[hh]] : 0.f;
+    dr[hh] = row[hh] < n ? delta[bh * n + row[hh]] : 0.f;
+  }
+  float dq[8][4];
+  zero_acc(dq);
+  for (int i = 0; i < nblk; ++i) {
+    const int kb = i * kAttnRows, nxt = (i + 1) & 1;
+    const bool more = i + 1 < nblk;
+    uint8_t next_flag = 0;
+    if (more) {
+      attn_load_rows(ring + nxt * 2 * kAttnTile, gK, ld, kb + kAttnRows, kAttnRows, n);
+      attn_load_rows(ring + nxt * 2 * kAttnTile + kAttnTile, gV, ld, kb + kAttnRows, kAttnRows, n);
+      if (threadIdx.x < kAttnRows) next_flag = key_flag(mask, b, n, kb + kAttnRows + threadIdx.x);
+    }
+    const uint8_t* cur = ring + (i & 1) * 2 * kAttnTile;
+    attn_dq_block<kCausal>(qf, of, cur, cur + kAttnTile, 0, sFlag + (i & 1) * kAttnRows, kb, row, n, lr, dr,
+                           scale_log2, dq);
+    if (more && threadIdx.x < kAttnRows) sFlag[nxt * kAttnRows + threadIdx.x] = next_flag;
+    cp_async_wait_all();   // block i + 1 landed, and no thread reads stage i & 1 any more
+    __syncthreads();
   }
   store_rows(dqkv + (long long)b * n * ldd + h * kAttnDh, ldd, q0 + r0, n, dq, scale);
 }
@@ -420,7 +655,6 @@ extern "C" int xclip_attn_fwd(const void* qkv, int64_t ld_qkv, const uint8_t* ke
   if (rc) return rc;
   XCLIP_REQUIRE(qkv && o && lse, "attn_fwd: null pointer");
   XCLIP_REQUIRE(B > 0 && heads > 0 && n > 0, "attn_fwd: bad sizes B=%d n=%d heads=%d", B, n, heads);
-  XCLIP_REQUIRE(n <= 320, "attn_fwd: sequence length %d > 320 is not supported by this kernel", n);
   XCLIP_REQUIRE(scale > 0.f, "attn_fwd: scale must be positive");
   XCLIP_REQUIRE(ld_qkv % 8 == 0 && ld_qkv >= 3 * heads * kAttnDh, "attn_fwd: bad ld_qkv");
   XCLIP_REQUIRE(ldo % 8 == 0 && ldo >= heads * kAttnDh, "attn_fwd: bad ldo");
@@ -429,17 +663,20 @@ extern "C" int xclip_attn_fwd(const void* qkv, int64_t ld_qkv, const uint8_t* ke
                 "attn_fwd: misaligned pointer");
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   const int NP = (n + 63) & ~63;
-  const int smem = kAttnRows * 128 + 2 * NP * 128 + NP;
+  const bool streaming = n > kAttnResidentMaxN || tune(XCLIP_TUNE_ATTN_STREAM) != 0;
+  // resident: Q block + the head's K, V and flags; streaming: Q block + 2 stages of (K, V, 64 flags)
+  const int smem = streaming ? 5 * kAttnTile + 2 * kAttnRows : kAttnTile + 2 * NP * 128 + NP;
   const long long blocks = (long long)(NP / kAttnRows) * B * heads;
   XCLIP_REQUIRE(blocks <= 0x7fffffffLL, "attn: B=%d x heads=%d is too large", B, heads);
   const dim3 grid((unsigned)blocks);
-  auto kern = causal ? attn_fwd_kernel<true> : attn_fwd_kernel<false>;
+  auto kern = streaming ? (causal ? attn_fwd_stream_kernel<true> : attn_fwd_stream_kernel<false>)
+                        : (causal ? attn_fwd_kernel<true> : attn_fwd_kernel<false>);
   rc = ensure_dynamic_smem(reinterpret_cast<const void*>(kern), smem);
   if (rc) return rc;
   kern<<<grid, kAttnThreads, smem, s>>>(reinterpret_cast<const bf16*>(qkv), ld_qkv, key_mask,
                                         reinterpret_cast<bf16*>(o), ldo, lse, n, heads,
                                         scale * kLog2e);
-  XCLIP_LAUNCH_CHECK("attn_fwd_kernel");
+  XCLIP_LAUNCH_CHECK(streaming ? "attn_fwd_stream_kernel" : "attn_fwd_kernel");
   return XCLIP_OK;
 }
 
@@ -452,8 +689,7 @@ extern "C" int xclip_attn_bwd(const void* qkv, int64_t ld_qkv, const uint8_t* ke
   int rc = xclip_init();
   if (rc) return rc;
   XCLIP_REQUIRE(qkv && o && d_o && lse && delta && dqkv, "attn_bwd: null pointer");
-  XCLIP_REQUIRE(B > 0 && heads > 0 && n > 0 && n <= 320, "attn_bwd: bad sizes B=%d n=%d heads=%d",
-                B, n, heads);
+  XCLIP_REQUIRE(B > 0 && heads > 0 && n > 0, "attn_bwd: bad sizes B=%d n=%d heads=%d", B, n, heads);
   XCLIP_REQUIRE(ld_qkv % 8 == 0 && ld_qkv >= 3 * heads * kAttnDh && ld_dqkv % 8 == 0 &&
                     ld_dqkv >= 3 * heads * kAttnDh && ldo % 8 == 0 && lddo % 8 == 0 &&
                     ldo >= heads * kAttnDh && lddo >= heads * kAttnDh,
@@ -478,23 +714,30 @@ extern "C" int xclip_attn_bwd(const void* qkv, int64_t ld_qkv, const uint8_t* ke
   const bf16* g = reinterpret_cast<const bf16*>(d_o);
   bf16* d = reinterpret_cast<bf16*>(dqkv);
   const float sl2 = scale * kLog2e;
+  const bool streaming = n > kAttnResidentMaxN || tune(XCLIP_TUNE_ATTN_STREAM) != 0;
   {
-    const int smem = 2 * kAttnRows * 128 + 2 * NP * 128 + 2 * NP * 4 + kAttnRows;
-    auto kern = causal ? attn_bwd_dkdv_kernel<true> : attn_bwd_dkdv_kernel<false>;
+    // resident: K, V block + the head's Q, dO, lse, delta; streaming: K, V block + 2 stages of
+    // (Q, dO, 64 lse, 64 delta); both + the block's 64 key flags
+    const int smem = streaming ? 6 * kAttnTile + 4 * kAttnRows * 4 + kAttnRows
+                               : 2 * kAttnTile + 2 * NP * 128 + 2 * NP * 4 + kAttnRows;
+    auto kern = streaming ? (causal ? attn_bwd_dkdv_stream_kernel<true> : attn_bwd_dkdv_stream_kernel<false>)
+                          : (causal ? attn_bwd_dkdv_kernel<true> : attn_bwd_dkdv_kernel<false>);
     rc = ensure_dynamic_smem(reinterpret_cast<const void*>(kern), smem);
     if (rc) return rc;
     kern<<<grid, kAttnThreads, smem, s>>>(q, ld_qkv, key_mask, g, lddo, lse, delta, d, ld_dqkv, n, heads,
                                           scale, sl2);
-    XCLIP_LAUNCH_CHECK("attn_bwd_dkdv_kernel");
+    XCLIP_LAUNCH_CHECK(streaming ? "attn_bwd_dkdv_stream_kernel" : "attn_bwd_dkdv_kernel");
   }
   {
-    const int smem = 2 * kAttnRows * 128 + 2 * NP * 128 + NP;
-    auto kern = causal ? attn_bwd_dq_kernel<true> : attn_bwd_dq_kernel<false>;
+    // resident: Q, dO block + the head's K, V and flags; streaming: Q, dO block + 2 stages of (K, V, 64 flags)
+    const int smem = streaming ? 6 * kAttnTile + 2 * kAttnRows : 2 * kAttnTile + 2 * NP * 128 + NP;
+    auto kern = streaming ? (causal ? attn_bwd_dq_stream_kernel<true> : attn_bwd_dq_stream_kernel<false>)
+                          : (causal ? attn_bwd_dq_kernel<true> : attn_bwd_dq_kernel<false>);
     rc = ensure_dynamic_smem(reinterpret_cast<const void*>(kern), smem);
     if (rc) return rc;
     kern<<<grid, kAttnThreads, smem, s>>>(q, ld_qkv, key_mask, g, lddo, lse, delta, d, ld_dqkv, n, heads,
                                           scale, sl2);
-    XCLIP_LAUNCH_CHECK("attn_bwd_dq_kernel");
+    XCLIP_LAUNCH_CHECK(streaming ? "attn_bwd_dq_stream_kernel" : "attn_bwd_dq_kernel");
   }
   return XCLIP_OK;
 }

@@ -143,7 +143,8 @@ int tune(int knob) { return (knob >= 0 && knob < 8) ? g_tune[knob] : 0; }
 extern "C" {
 
 int xclip_tune_set(int knob, int value) {
-  if (knob != XCLIP_TUNE_LN_FWD_BLOCKS && knob != XCLIP_TUNE_LN_BWD_BLOCKS) return -1;
+  if (knob != XCLIP_TUNE_LN_FWD_BLOCKS && knob != XCLIP_TUNE_LN_BWD_BLOCKS && knob != XCLIP_TUNE_ATTN_STREAM)
+    return -1;
   const int prev = xclip::g_tune[knob];
   xclip::g_tune[knob] = value;
   return prev;
