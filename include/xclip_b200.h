@@ -160,7 +160,10 @@ int xclip_nce_bwd(const void* a, const void* b, int R, int C, int D, const float
  *          transposed) - the masked mean over text tokens (:807) / mean over image tokens (:811).
  * nce_fwd/bwd : row-wise InfoNCE / DCL on an [R,C] fp32 similarity matrix (R local texts, C all
  *          images, positive of row x at column x + diag_off) (:821-847); bwd writes
- *          g = *gscale * (softmax_row - [positive]).
+ *          g = *gscale * (softmax_row - [positive]).  row_valid (optional, one byte per row): a
+ *          row with row_valid[x] == 0 (the image-to-text row of a caption without valid tokens)
+ *          adds no loss, gets g = 0 and lse = 0 - as in the reference, where that row is
+ *          exp(-inf) = 0 in both the positive and the denominator.
  * expand : rows [row0,row0+rows) of the backward operand G[R,C] (bf16): at the argmax column
  *          of each (row, sample) the value *temp_exp * wmat[row/rows_per_sample, sample] *
  *          rowscale[row], zero elsewhere; *dtemp += sum w * seg_max.  d rows = G @ b and
@@ -170,10 +173,12 @@ int xclip_filip_segmax(const void* a, const void* b, int R, int C, int D, const 
                        int* seg_arg, xclip_stream_t stream);
 int xclip_filip_reduce(const float* seg_max, const float* weights, int samples, int len, int nseg,
                        float* out, int transpose_out, xclip_stream_t stream);
-int xclip_filip_nce_fwd(const float* s, int R, int C, int diag_off, int dcl, float* lse,
-                        float* loss_accum, float loss_scale, xclip_stream_t stream);
+int xclip_filip_nce_fwd(const float* s, int R, int C, int diag_off, int dcl,
+                        const unsigned char* row_valid, float* lse, float* loss_accum,
+                        float loss_scale, xclip_stream_t stream);
 int xclip_filip_nce_bwd(const float* s, const float* lse, int R, int C, int diag_off, int dcl,
-                        const float* gscale, float* g, xclip_stream_t stream);
+                        const unsigned char* row_valid, const float* gscale, float* g,
+                        xclip_stream_t stream);
 int xclip_filip_expand(const int* seg_arg, const float* seg_max, const float* wmat,
                        const float* rowscale, const float* temp_exp, int row0, int rows,
                        int rows_per_sample, int seg_len, int nseg, void* g, int64_t ldg,

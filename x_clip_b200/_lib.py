@@ -85,10 +85,10 @@ SIGNATURES = {
                                    c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "xclip_filip_reduce": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int,
                                    c_void_p]),
-    "xclip_filip_nce_fwd": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_float,
-                                    c_void_p]),
+    "xclip_filip_nce_fwd": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                    c_float, c_void_p]),
     "xclip_filip_nce_bwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
-                                    c_void_p]),
+                                    c_void_p, c_void_p]),
     "xclip_filip_expand": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
                                    c_int, c_int, c_int, c_void_p, c_int64, c_void_p, c_void_p]),
 }

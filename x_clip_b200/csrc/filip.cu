@@ -36,13 +36,21 @@ filip_reduce_kernel(const float* __restrict__ m, const float* __restrict__ w, in
 }
 
 // one warp per row of an [R,C] fp32 matrix (R local texts x C global images; the positive of row
-// x is column x + diag_off): lse (optionally without the positive), loss partial
+// x is column x + diag_off): lse (optionally without the positive), loss partial.
+// row_valid (optional): a row with row_valid[x] == 0 - the image-to-text row of a caption without
+// any valid token - has no loss term and no gradient (the reference's row is exp(-inf) = 0 in the
+// positive and in the denominator alike); its lse is written as 0.
 __global__ void __launch_bounds__(256)
 filip_nce_fwd_kernel(const float* __restrict__ s, int R, int C, int diag_off, int dcl,
-                     float* __restrict__ lse, float* __restrict__ loss_accum, float scale) {
+                     const unsigned char* __restrict__ row_valid, float* __restrict__ lse,
+                     float* __restrict__ loss_accum, float scale) {
   const int lane = threadIdx.x & 31;
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= R) return;
+  if (row_valid != nullptr && !row_valid[row]) {          // warp-uniform
+    if (lane == 0) lse[row] = 0.f;
+    return;
+  }
   const float* r = s + (long long)row * C;
   const int pos = row + diag_off;
   float mx = -INFINITY;
@@ -60,14 +68,19 @@ filip_nce_fwd_kernel(const float* __restrict__ s, int R, int C, int diag_off, in
   }
 }
 
-// g[x,y] = gscale * (exp(s - lse_x) [skipped on the positive when dcl] - [y == x + diag_off])
+// g[x,y] = gscale * (exp(s - lse_x) [skipped on the positive when dcl] - [y == x + diag_off]);
+// rows with row_valid[x] == 0 get g = 0 (see filip_nce_fwd_kernel)
 __global__ void __launch_bounds__(256)
 filip_nce_bwd_kernel(const float* __restrict__ s, const float* __restrict__ lse, int R, int C,
-                     int diag_off, int dcl, const float* __restrict__ gscale,
-                     float* __restrict__ g) {
+                     int diag_off, int dcl, const unsigned char* __restrict__ row_valid,
+                     const float* __restrict__ gscale, float* __restrict__ g) {
   const long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (idx >= (long long)R * C) return;
   const int x = (int)(idx / C), y = (int)(idx % C);
+  if (row_valid != nullptr && !row_valid[x]) {
+    g[idx] = 0.f;
+    return;
+  }
   const bool is_pos = (y == x + diag_off);
   float v = 0.f;
   if (!(dcl && is_pos)) v = __expf(s[idx] - lse[x]);
@@ -172,26 +185,28 @@ extern "C" int xclip_filip_reduce(const float* seg_max, const float* weights, in
   return XCLIP_OK;
 }
 
-extern "C" int xclip_filip_nce_fwd(const float* s, int R, int C, int diag_off, int dcl, float* lse,
-                                   float* loss_accum, float loss_scale, xclip_stream_t stream) {
+extern "C" int xclip_filip_nce_fwd(const float* s, int R, int C, int diag_off, int dcl,
+                                   const unsigned char* row_valid, float* lse, float* loss_accum,
+                                   float loss_scale, xclip_stream_t stream) {
   int rc = xclip_init();
   if (rc) return rc;
   XCLIP_REQUIRE(s && lse && R > 0 && C > 0 && diag_off >= 0 && diag_off + R <= C,
                 "filip_nce_fwd: bad arguments");
   filip_nce_fwd_kernel<<<(R + 7) / 8, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      s, R, C, diag_off, dcl, lse, loss_accum, loss_scale);
+      s, R, C, diag_off, dcl, row_valid, lse, loss_accum, loss_scale);
   XCLIP_LAUNCH_CHECK("filip_nce_fwd_kernel");
   return XCLIP_OK;
 }
 
 extern "C" int xclip_filip_nce_bwd(const float* s, const float* lse, int R, int C, int diag_off,
-                                   int dcl, const float* gscale, float* g, xclip_stream_t stream) {
+                                   int dcl, const unsigned char* row_valid, const float* gscale,
+                                   float* g, xclip_stream_t stream) {
   int rc = xclip_init();
   if (rc) return rc;
   XCLIP_REQUIRE(s && lse && gscale && g && R > 0 && C > 0, "filip_nce_bwd: bad arguments");
   const long long n = (long long)R * C;
   filip_nce_bwd_kernel<<<(int)((n + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      s, lse, R, C, diag_off, dcl, gscale, g);
+      s, lse, R, C, diag_off, dcl, row_valid, gscale, g);
   XCLIP_LAUNCH_CHECK("filip_nce_bwd_kernel");
   return XCLIP_OK;
 }

@@ -55,24 +55,30 @@ class FilipLossFn(torch.autograd.Function):
         m2, a2 = K.filip_segmax(rows_i, cols_t, temp_exp, T, col_mul, col_add)   # [B*I, b]
         i2t = K.filip_reduce(m2, w_i, B, I, b, transpose=True)                   # [b, B] (text, image)
 
+        # A caption without any valid token (an empty string) has every i2t similarity at the
+        # -FLT_MAX fill: the reference's mean overflows to -inf and that row adds neither loss nor
+        # gradient.  Its t2i row is 0 (the masked mean of nothing) and is an ordinary row.
+        has_tokens = text_mask.any(dim=1).contiguous()
+
         loss = torch.zeros(1, device=dev, dtype=F32)
         lse_t = K.filip_nce_fwd(t2i, off, dcl, loss, 1.0 / (2 * B))
-        lse_i = K.filip_nce_fwd(i2t, off, dcl, loss, 1.0 / (2 * B))
+        lse_i = K.filip_nce_fwd(i2t, off, dcl, loss, 1.0 / (2 * B), row_valid=has_tokens)
         if world > 1:
             D_.all_reduce_sum_(loss)
 
         ctx.cfg = (dcl, extra, rank, world, b, B, T, I, D, off)
-        ctx.stuff = (temp_exp, ops, img_all, w_t, w_i, m1, a1, m2, a2, t2i, i2t, lse_t, lse_i)
+        ctx.stuff = (temp_exp, ops, img_all, w_t, w_i, m1, a1, m2, a2, t2i, i2t, lse_t, lse_i, has_tokens)
         return loss.reshape(())
 
     @staticmethod
     def backward(ctx, gloss):
         dcl, extra, rank, world, b, B, T, I, D, off = ctx.cfg
-        temp_exp, ops, img_all, w_t, w_i, m1, a1, m2, a2, t2i, i2t, lse_t, lse_i = ctx.stuff
+        temp_exp, ops, img_all, w_t, w_i, m1, a1, m2, a2, t2i, i2t, lse_t, lse_i, has_tokens = ctx.stuff
         dev = gloss.device
         gscale = (gloss.detach().float() / (2.0 * B)).reshape(1)
         g_t = K.filip_nce_bwd(t2i, lse_t, off, dcl, gscale)                      # [x local, y all]
-        g_i = K.filip_nce_bwd(i2t, lse_i, off, dcl, gscale).t().contiguous()     # -> [y all, x local]
+        g_i = K.filip_nce_bwd(i2t, lse_i, off, dcl, gscale,                      # -> [y all, x local]
+                              row_valid=has_tokens).t().contiguous()
         dtemp = torch.zeros(1, device=dev, dtype=F32)
 
         def one_pass(seg_arg, seg_max, wmat, rowscale, rows_per_sample, seg_len, nseg, row_hi, col_hi):

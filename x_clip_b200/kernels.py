@@ -446,19 +446,28 @@ def filip_reduce(seg_max, weights, samples, length, nseg, transpose):
     return out
 
 
-def filip_nce_fwd(s, diag_off, dcl, loss_accum, loss_scale):
+def _row_valid(row_valid, s):
+    if row_valid is not None and (row_valid.dtype != torch.bool or row_valid.numel() != s.shape[0]
+                                  or not row_valid.is_contiguous() or row_valid.device != s.device):
+        raise _lib.XClipB200Error("filip_nce: row_valid must be a contiguous bool [R] on the device of s")
+    return _ptr(row_valid)
+
+
+def filip_nce_fwd(s, diag_off, dcl, loss_accum, loss_scale, row_valid=None):
+    """lse [R] of the rows of s (rows with row_valid False: no loss term, lse 0)."""
     R, C = s.shape
     lse = torch.empty((R,), device=s.device, dtype=F32)
     _call(s, "filip_small", 0.0, 4.0 * s.numel(), "xclip_filip_nce_fwd", s.data_ptr(), R, C,
-          int(diag_off), 1 if dcl else 0, lse.data_ptr(), _ptr(loss_accum), float(loss_scale))
+          int(diag_off), 1 if dcl else 0, _row_valid(row_valid, s), lse.data_ptr(), _ptr(loss_accum),
+          float(loss_scale))
     return lse
 
 
-def filip_nce_bwd(s, lse, diag_off, dcl, gscale):
+def filip_nce_bwd(s, lse, diag_off, dcl, gscale, row_valid=None):
     R, C = s.shape
     g = torch.empty_like(s)
     _call(s, "filip_small", 0.0, 8.0 * s.numel(), "xclip_filip_nce_bwd", s.data_ptr(), lse.data_ptr(), R,
-          C, int(diag_off), 1 if dcl else 0, gscale.data_ptr(), g.data_ptr())
+          C, int(diag_off), 1 if dcl else 0, _row_valid(row_valid, s), gscale.data_ptr(), g.data_ptr())
     return g
 
 
