@@ -133,14 +133,17 @@ int xclip_attn_bwd(const void* qkv, int64_t ld_qkv, const uint8_t* key_mask, con
  *   r + diag_offset.  dcl != 0 removes the positive from the denominator (:834-836).
  * fwd:  lse[r] = log sum_c exp(s[r,c]);  pos[r] = s[r, r+diag_offset];
  *       *loss_accum += loss_scale * sum_r (lse[r] - pos[r])     (loss_accum may be NULL)
- *       part_ws: f32 scratch [2 * xclip_nce_num_col_blocks(C) * R] (per block: max, sum; the
- *       log-sum-exp uses an online maximum, so any temperature works).
- *       (the reference's +1e-20 inside its logs, :51-52, is below fp32 resolution here)
+ *       part_ws: f32 scratch [2 * xclip_nce_num_col_blocks(C) * R], 8-byte aligned (per block:
+ *       max, sum; the log-sum-exp uses an online maximum, so any temperature works).
+ *       (the reference's +1e-20 inside its logs, :51-52, is below fp32 resolution here, except
+ *       for an empty denominator - dcl with C == 1 - where lse = ln(1e-20) as in the reference)
  * bwd:  g[r,c] = *gscale * (w_row*exp(s - lse_row[r]) + w_col*exp(s - lse_col[c])
  *                           - w_diag*[c == r+diag])     (gscale: DEVICE scalar, upstream grad
  *       / (2*B_global); exp terms skipped on the positive when dcl).  Written as
  *       bf16 temp_exp*g [R, ldg>=roundup8(C)], so the latent gradient is dA = (that) @ b via
- *       xclip_gemm_bf16;  *dtemp += sum g*s (d loss / d temperature) when dtemp != NULL. */
+ *       xclip_gemm_bf16;  *dtemp += sum g*s (d loss / d temperature) when dtemp != NULL.
+ *       lse_col (f32 [C]) is read with 16-byte vector loads: when w_col != 0 it must be 16-byte
+ *       aligned, or the call returns XCLIP_ERR_INVALID without launching. */
 int xclip_nce_num_col_blocks(int C);
 int xclip_nce_fwd(const void* a, const void* b, int R, int C, int D, const float* temp_exp,
                   int diag_offset, int dcl, float* part_ws, float* pos, float* lse,
@@ -215,7 +218,8 @@ int xclip_text_embed_bwd(const int64_t* ids, const void* dx, float* dtok, float*
  *                     gdh = dx w2g (reads u, stats, ab; the [M, 4d] gradient never exists in HBM).
  *   ff_w2_grad_post : in place on raw = dxs^T hp (f32 [d, 4d]): dW2[j,k] = g[k] * (raw[j,k] - vsum[j]);
  *                     with w2/dg also dg[k] += sum_j (raw[j,k] - vsum[j]) * w2[j,k] (gain gradient).
- * d in 256*{1,2,3,4}; all matrices row-major, bf16 unless stated. */
+ * d in 256*{1,2,3,4}; all matrices row-major, bf16 unless stated.  Matrices, rowsum and colvec must
+ * be 16-byte aligned; stats and ab (read and written as float pairs) 8-byte aligned. */
 int xclip_ff_permute_cast(const float* w1, void* out, int d, xclip_stream_t stream);
 int xclip_ff_scale_cast(const float* w2, const float* g, void* w2g, float* colvec, int d,
                         xclip_stream_t stream);

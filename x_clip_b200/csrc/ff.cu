@@ -86,6 +86,7 @@ static int launch_ff(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmP
 using namespace xclip;
 
 #define FF_ALIGNED(p) ((reinterpret_cast<uintptr_t>(p) & 15) == 0)
+#define FF_ALIGNED8(p) ((reinterpret_cast<uintptr_t>(p) & 7) == 0)     // float2 accesses
 
 extern "C" int xclip_ff_permute_cast(const float* w1, void* out, int d, xclip_stream_t stream) {
   int rc = xclip_init();
@@ -120,7 +121,8 @@ extern "C" int xclip_ff_up(const void* x, int64_t ldx, const void* w1p, void* u,
   XCLIP_REQUIRE(M > 0 && d > 0 && d % 256 == 0, "ff_up: M=%d d=%d (d %% 256)", M, d);
   XCLIP_REQUIRE(ldx % 8 == 0 && ldx >= d && ldu % 8 == 0 && ldu >= 8 * d && ldhp % 8 == 0 && ldhp >= 4 * d,
                 "ff_up: bad leading dimensions");
-  XCLIP_REQUIRE(FF_ALIGNED(x) && FF_ALIGNED(w1p) && FF_ALIGNED(u) && FF_ALIGNED(hp), "ff_up: misaligned pointer");
+  XCLIP_REQUIRE(FF_ALIGNED(x) && FF_ALIGNED(w1p) && FF_ALIGNED(u) && FF_ALIGNED(hp) && FF_ALIGNED(rowsum),
+                "ff_up: misaligned pointer");
   CUtensorMap tmA, tmB;
   if ((rc = encode_2d_bf16(&tmA, x, (uint64_t)d, (uint64_t)M, (uint64_t)ldx, 64, kGemmBlockM))) return rc;
   if ((rc = encode_2d_bf16(&tmB, w1p, (uint64_t)d, (uint64_t)(8 * d), (uint64_t)d, 64, 128))) return rc;
@@ -144,7 +146,8 @@ extern "C" int xclip_ff_down(const void* hp, int64_t ldhp, const void* w2g, cons
                     (!residual || (ldr % 8 == 0 && ldr >= d)),
                 "ff_down: bad leading dimensions");
   XCLIP_REQUIRE(FF_ALIGNED(hp) && FF_ALIGNED(w2g) && FF_ALIGNED(out) && FF_ALIGNED(acc_out) &&
-                    FF_ALIGNED(colvec) && (!residual || FF_ALIGNED(residual)),
+                    FF_ALIGNED(colvec) && FF_ALIGNED(rowsum) && FF_ALIGNED8(stats) &&
+                    (!residual || FF_ALIGNED(residual)),
                 "ff_down: misaligned pointer");
   CUtensorMap tmA, tmB;
   if ((rc = encode_2d_bf16(&tmA, hp, (uint64_t)(4 * d), (uint64_t)M, (uint64_t)ldhp, 64, kGemmBlockM))) return rc;
@@ -168,7 +171,9 @@ extern "C" int xclip_ff_bwd(const void* dx, int64_t lddx, const void* w2g, const
   XCLIP_REQUIRE(M > 0 && d > 0 && d % 256 == 0, "ff_bwd: M=%d d=%d (d %% 256)", M, d);
   XCLIP_REQUIRE(lddx % 8 == 0 && lddx >= d && ldu % 8 == 0 && ldu >= 8 * d && lddu % 8 == 0 && lddu >= 8 * d,
                 "ff_bwd: bad leading dimensions");
-  XCLIP_REQUIRE(FF_ALIGNED(dx) && FF_ALIGNED(w2g) && FF_ALIGNED(u) && FF_ALIGNED(du), "ff_bwd: misaligned pointer");
+  XCLIP_REQUIRE(FF_ALIGNED(dx) && FF_ALIGNED(w2g) && FF_ALIGNED(u) && FF_ALIGNED(du) && FF_ALIGNED8(stats) &&
+                    FF_ALIGNED8(ab),
+                "ff_bwd: misaligned pointer");
   CUtensorMap tmA, tmB;
   if ((rc = encode_2d_bf16(&tmA, dx, (uint64_t)d, (uint64_t)M, (uint64_t)lddx, 64, kGemmBlockM))) return rc;
   // B = w2g [d, 4d] consumed MN-major: contraction index d on rows, 64 x 64 boxes

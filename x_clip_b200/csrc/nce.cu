@@ -18,6 +18,8 @@
 
 namespace xclip {
 
+constexpr float kLogEmptyDenominator = -46.051701859880914f;   // ln(1e-20)
+
 __global__ void __launch_bounds__(1024)
 nce_finalize_kernel(const float* __restrict__ part, int nblk, const float* __restrict__ pos,
                     int rows, const float* __restrict__ alpha_dev, float* __restrict__ lse,
@@ -33,7 +35,9 @@ nce_finalize_kernel(const float* __restrict__ part, int nblk, const float* __res
       const float2 ps = part2[(long long)k * rows + r];
       if (ps.x > -INFINITY) s += ps.y * exp2f(ps.x - m);
     }
-    const float l = (m + log2f(s)) * 0.6931471805599453f;
+    // Every partial empty: a DCL row whose only column is its own positive (global batch 1).  The
+    // reference adds 1e-20 inside the log (x_clip.py:51-52); take its value instead of -inf.
+    const float l = m > -INFINITY ? (m + log2f(s)) * 0.6931471805599453f : kLogEmptyDenominator;
     lse[r] = l;
     local += l - pos[r];
   }
@@ -100,6 +104,8 @@ extern "C" int xclip_nce_fwd(const void* a, const void* b, int R, int C, int D,
   int rc = nce_common(a, b, R, C, D, &p, &tmA, &tmB, &block_n, &grid);
   if (rc) return rc;
   XCLIP_REQUIRE(part_ws && pos && lse && temp_exp, "nce_fwd: null workspace/output");
+  XCLIP_REQUIRE((reinterpret_cast<uintptr_t>(part_ws) & 7) == 0,
+                "nce_fwd: part_ws must be 8-byte aligned (float2 partials)");
   XCLIP_REQUIRE(diag_offset >= 0 && diag_offset + R <= C, "nce_fwd: positives outside the columns");
   p.alpha_dev = temp_exp; p.diag_offset = diag_offset; p.dcl = dcl;
   p.nce_part = part_ws; p.nce_pos = pos;
@@ -129,6 +135,8 @@ extern "C" int xclip_nce_bwd(const void* a, const void* b, int R, int C, int D,
   XCLIP_REQUIRE(g && ldg % 8 == 0 && ldg >= (C + 7) / 8 * 8, "nce_bwd: g needs ld >= roundup8(C)");
   XCLIP_REQUIRE((reinterpret_cast<uintptr_t>(g) & 15) == 0, "nce_bwd: misaligned g");
   XCLIP_REQUIRE((w_row == 0.f || lse_row) && (w_col == 0.f || lse_col), "nce_bwd: missing lse");
+  XCLIP_REQUIRE(w_col == 0.f || (reinterpret_cast<uintptr_t>(lse_col) & 15) == 0,
+                "nce_bwd: lse_col must be 16-byte aligned (it is read as float4)");
   XCLIP_REQUIRE(temp_exp && gscale, "nce_bwd: temp_exp / gscale device scalars required");
   p.alpha_dev = temp_exp; p.gscale_dev = gscale; p.diag_offset = diag_offset; p.dcl = dcl;
   p.lse_row = lse_row; p.lse_col = lse_col;

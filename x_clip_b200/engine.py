@@ -455,7 +455,9 @@ class ContrastiveLossFn(torch.autograd.Function):
         ctx.cfg = (dcl, extra, rank, world, b, D, Bg, off)
         ctx.temp_exp = temp_exp
         ctx.rows, ctx.cols = rows, cols
-        ctx.lse = (lse_t, lse_i, gstats[0].contiguous(), gstats[2].contiguous())
+        # xclip_nce_bwd reads lse_col with 16-byte vector loads.  Row k of the [4, Bg] stats starts
+        # 4*k*Bg bytes in, so row 2 is misaligned for odd Bg: clone the rows into storage of their own.
+        ctx.lse = (lse_t, lse_i, gstats[0].clone(), gstats[2].clone())
         return loss
 
     @staticmethod
