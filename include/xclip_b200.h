@@ -153,6 +153,30 @@ int xclip_nce_bwd(const void* a, const void* b, int R, int C, int D, const float
                   float w_row, float w_col, float w_diag, const float* gscale, void* g,
                   int64_t ldg, float* dtemp, xclip_stream_t stream);
 
+/* ---- similarity regularisation (arXiv 2309.08773; x_clip/x_clip.py:771-784, :870-873) ----------
+ * E[r,c] = <t_r, t_c> - <v_r, v_c> for LOCAL rows r and ALL columns c of the global batch, formed in
+ * the fp32 accumulator as one contraction a . b^T of the concatenated operands
+ *   a = [zrow_t | zrow_v]  bf16 [R, K],   b = [zcol_t | -zcol_v]  bf16 [C, K],   K = 6*D
+ * (zrow / zcol: the split-bf16 operands of xclip_l2norm_fwd, each [rows, 3D]).  Row r's own sample is
+ * column r + diag_offset; that column and nothing beyond C takes part.  a, b: 16-byte aligned,
+ * K % 8 == 0.  diag_offset < 0 or diag_offset + R > C returns XCLIP_ERR_INVALID without a launch.
+ * pack : out bf16 [rows, 2k] = [t | v] (negate_v = 0) or [t | -v] (negate_v != 0); t, v bf16 [rows, k]
+ *        contiguous, k % 8 == 0, t / v / out 16-byte aligned.  Negation is exact.
+ * fwd  : rowsum[r] = sum_{c != r+diag_offset} E[r,c]^2 (f32 [R], may be NULL);
+ *        *loss_accum += loss_scale * sum_r rowsum[r]   (loss_accum may be NULL).
+ *        part_ws: f32 scratch [xclip_nce_num_col_blocks(C) * R], 4-byte aligned.
+ * bwd  : g[r,c] = bf16(*gscale * E[r,c]) (gscale: DEVICE scalar), 0 at c == r+diag_offset and in
+ *        the pad columns [C, ldg); g [R, ldg >= roundup8(C)], ldg % 8 == 0, 16-byte aligned.  With
+ *        gscale = upstream * 2 w / (B (B-1)) the latent gradients of w * L_sim are dT = g @ T and
+ *        dV = -(g @ V) over the columns' latents (xclip_gemm_bf16). */
+int xclip_simreg_pack(const void* t, const void* v, int rows, int k, int negate_v, void* out,
+                      xclip_stream_t stream);
+int xclip_simreg_fwd(const void* a, const void* b, int R, int C, int K, int diag_offset,
+                     float* part_ws, float* rowsum, float* loss_accum, float loss_scale,
+                     xclip_stream_t stream);
+int xclip_simreg_bwd(const void* a, const void* b, int R, int C, int K, int diag_offset,
+                     const float* gscale, void* g, int64_t ldg, xclip_stream_t stream);
+
 /* ---- FILIP fine-grained loss (x_clip/x_clip.py:799-811 + :821-847) -----------------------
  * segmax : a bf16 [R,D] token latents of one modality, b bf16 [C,D] token latents of the other,
  *          C = n_samples * seg_len (seg_len tokens per sample, multiple of 16, <= 256).  For

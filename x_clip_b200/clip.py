@@ -11,8 +11,11 @@ Sequence length is not limited by the non-causal attention: image towers such as
 320 tokens).  Feature combinations the kernels do not cover raise at construction (never a silent
 CPU or eager fallback): dim_head != 64, model dims not multiples of 256, a causal text tower longer than
 128 tokens, rotary + causal together (broken in the reference itself: n+1 angles for n tokens,
-x_clip.py:328), dropout > 0, the similarity-regularisation term and conv-downsampled image
-latents.  MLM, SimSiam / SimCLR and the multiview term run through the fast encoders (aux.py).
+x_clip.py:328), dropout > 0 and conv-downsampled image latents.  MLM, SimSiam / SimCLR and the
+multiview term run through the fast encoders (aux.py).  The similarity-regularisation term
+(`sim_reg_loss_weight > 0`) runs fused with the contrastive loss (engine.ContrastiveLossFn) where the
+reference itself runs it: with `extra_latent_projection=True`, without FILIP and with a single view;
+the other combinations fail inside the reference (x_clip.py:779) and raise `Unsupported` here.
 """
 from __future__ import annotations
 
@@ -317,7 +320,14 @@ class CLIP(nn.Module):
         assert not (text_causal_mask and text_eos_id is None), \
             'text EOS token id must be given if using causal mask in text transformer'
         _require(not downsample_image_embeds, "downsample_image_embeds is not implemented")
-        _require(sim_reg_loss_weight == 0., "sim_reg_loss_weight > 0 is not implemented")
+        if sim_reg_loss_weight > 0.:
+            # without the extra projection the reference's einsum at x_clip.py:779 gets the 2-D
+            # un-rearranged text_latents_extra and fails; with FILIP its [1, B, B] mask cannot index
+            # the [m, t, B, B] token similarities
+            _require(extra_latent_projection,
+                     "sim_reg_loss_weight > 0 needs extra_latent_projection=True (the reference fails at x_clip.py:779 without it)")
+            _require(not use_all_token_embeds,
+                     "sim_reg_loss_weight > 0 with use_all_token_embeds (the reference's mask at x_clip.py:779 does not fit the token similarities)")
         _require(dim_latent % 256 == 0 and dim_latent <= 1024, "dim_latent must be 256/512/768/1024")
         _require(dim_text % 8 == 0 and dim_image % 8 == 0, "dim_text / dim_image must be multiples of 8")
 
@@ -391,8 +401,9 @@ class CLIP(nn.Module):
         self.last_step_plan = None      # filled by engine.ChunkedClipLossFn: chunks / retained / bytes
         # latched at construction, like the reference (:591): the process group must exist first
         self.requires_all_gather = dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1
+        # similarity regularisation (https://arxiv.org/abs/2309.08773), fused into ContrastiveLossFn
         self.sim_reg_loss_weight = sim_reg_loss_weight
-        self.has_sim_reg_loss = False
+        self.has_sim_reg_loss = sim_reg_loss_weight > 0.
 
     # -- helpers ---------------------------------------------------------------------
     def _eos_to_front(self, enc_text, text):
@@ -449,6 +460,10 @@ class CLIP(nn.Module):
         aug_text=None,
         aug_image=None,
     ):
+        # the reference's [1, B, B] off-diagonal mask (x_clip.py:779) cannot index the [m, B, B] view
+        # similarities: it raises for every multiview step, so this one refuses before any encoder runs
+        _require(not (self.has_sim_reg_loss and (aug_text is not None or aug_image is not None)),
+                 "sim_reg_loss_weight > 0 with aug_text / aug_image (the reference fails at x_clip.py:779)")
         _require(text.is_cuda and image.is_cuda, "inputs must live on a CUDA (sm_90) device")
 
         text_mask = text != self.text_pad_id
@@ -528,18 +543,29 @@ class CLIP(nn.Module):
             from .filip import filip_loss
             return filip_loss(self, zt, zi, zt_x, zi_x, ops, text_mask)
 
-        def cl(tsl, isl):
-            """contrastive loss of text view rows `tsl` against image view rows `isl`"""
+        def cl(tsl, isl, *sim_reg):
+            """contrastive loss of text view rows `tsl` against image view rows `isl`; sim_reg =
+            (weight, contrastive weight) adds the similarity regularisation (ContrastiveLossFn)"""
             o = [(ops[0][0][tsl], ops[0][1][tsl]), (ops[1][0][isl], ops[1][1][isl])]
             if self.extra_latent_projection:
                 o += [(ops[2][0][tsl], ops[2][1][tsl]), (ops[3][0][isl], ops[3][1][isl])]
             return E.ContrastiveLossFn.apply(
                 zt[tsl], zi[isl], zt_x[tsl] if self.extra_latent_projection else None,
                 zi_x[isl] if self.extra_latent_projection else None, self.temperature,
-                tuple(o), self.decoupled_contrastive_learning, self.requires_all_gather)
+                tuple(o), self.decoupled_contrastive_learning, self.requires_all_gather, *sim_reg)
 
         if not has_aux:
+            if self.has_sim_reg_loss:
+                return cl(slice(None), slice(None), self.sim_reg_loss_weight, 1.0)
             return cl(slice(None), slice(None))
+
+        if self.has_sim_reg_loss:
+            # single view (multiview was refused above): cl_w * contrastive + w * L_sim in one call,
+            # the auxiliary terms added as in the reference (:860-873)
+            cl_w = 1 - (self.text_ssl_loss_weight + self.image_ssl_loss_weight)
+            loss = cl(slice(None), slice(None), self.sim_reg_loss_weight, cl_w)
+            return loss + text_ssl_loss * self.text_ssl_loss_weight \
+                + image_ssl_loss * self.image_ssl_loss_weight
 
         # every (text view m, image view n) pair is its own InfoNCE problem; [0] is the main loss,
         # the others are averaged into the multiview term (reference :750-755, :851-868)

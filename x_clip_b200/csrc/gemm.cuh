@@ -10,7 +10,8 @@
 //
 // This one kernel covers the reference's nn.Linear call sites on the hot path
 // (x_clip/x_clip.py:191,195,209,210,358,368,556,570) and their autograd backward, the logits of the
-// contrastive loss (NCE / FILIP epilogues) and the fused feed-forward (FF epilogues, see ff.cu).
+// contrastive loss (NCE / FILIP epilogues), the similarity regularisation (SIMREG epilogues, see
+// simreg.cu) and the fused feed-forward (FF epilogues, see ff.cu).
 //
 // Structure (one CTA per SM, 288 threads), output tile 128 x BLOCK_N:
 //   warps 0-3 : consumer warpgroup 0 - wgmma on columns [0, BLOCK_N/2) of the tile, then the epilogue
@@ -101,6 +102,13 @@ constexpr int EPI_SEGMAX = 3;   // per row and column segment: max and argmax of
 constexpr int EPI_FF_UP = 4;
 constexpr int EPI_FF_DOWN = 5;
 constexpr int EPI_FF_BWD = 6;
+// Similarity regularisation (simreg.cu): acc = E = T T^T - V V^T, formed inside the accumulator by
+// contracting [T | V] against [T | -V] (K = 2 x the split-bf16 width).  The positive column
+// r + diag_offset and the columns >= N are excluded.
+//   EPI_SIMREG_FWD  nce_part[n_blk * M + row] = sum over the tile's columns of E^2
+//   EPI_SIMREG_BWD  C = bf16(*gscale_dev * E), zero on the excluded columns up to ldc
+constexpr int EPI_SIMREG_FWD = 7;
+constexpr int EPI_SIMREG_BWD = 8;
 
 constexpr int kGemmBlockM = 128;
 constexpr int kGemmBlockK = 64;
@@ -536,6 +544,47 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       if (p.dtemp != nullptr) {
         tsum = warp_sum(tsum);
         if (lane == 0) atomicAdd(p.dtemp, tsum);
+      }
+    } else if constexpr (EPI == EPI_SIMREG_FWD) {
+      const int diag_col = row + p.diag_offset;
+      float s4[4] = {0.f, 0.f, 0.f, 0.f};          // four chains: the fma latency is not serialised
+#pragma unroll 1
+      for (int c = 0; c < BLOCK_N / 32; ++c) {
+        need(c * 32);
+        const int col0 = n_blk * BLOCK_N + c * 32;
+        if (col0 >= p.N) continue;
+        float v[32];
+        acc_ld32(acc_row, c * 32, v);
+        if (!(col0 + 32 <= p.N && (diag_col < col0 || diag_col >= col0 + 32))) {
+#pragma unroll
+          for (int i = 0; i < 32; ++i) {
+            const int col = col0 + i;
+            if (col >= p.N || col == diag_col) v[i] = 0.f;
+          }
+        }
+#pragma unroll
+        for (int i = 0; i < 32; ++i) s4[i & 3] = fmaf(v[i], v[i], s4[i & 3]);
+      }
+      if (row_ok) p.nce_part[(long long)n_blk * p.M + row] = (s4[0] + s4[1]) + (s4[2] + s4[3]);
+    } else if constexpr (EPI == EPI_SIMREG_BWD) {
+      const float gs = __ldg(p.gscale_dev);
+      const int diag_col = row + p.diag_offset;
+#pragma unroll 1
+      for (int c = 0; c < BLOCK_N / 32; ++c) {
+        need(c * 32);
+        const int col0 = n_blk * BLOCK_N + c * 32;
+        if (!row_ok || col0 >= (int)p.ldc) continue;   // pad columns [N, ldc) get zeros
+        float v[32];
+        acc_ld32(acc_row, c * 32, v);
+#pragma unroll
+        for (int i = 0; i < 32; ++i) {
+          const int col = col0 + i;
+          v[i] = (col < p.N && col != diag_col) ? gs * v[i] : 0.f;
+        }
+        bf16* grow = reinterpret_cast<bf16*>(p.c) + (long long)row * p.ldc + col0;
+#pragma unroll
+        for (int i = 0; i < 32; i += 8)
+          if (col0 + i < (int)p.ldc) st_bf16x8(grow + i, v + i);
       }
     } else if constexpr (EPI == EPI_FF_UP) {
       // tile columns [0,64) = value, [64,128) = gate of hidden units [64 n_blk, +64)

@@ -425,11 +425,23 @@ class ContrastiveLossFn(torch.autograd.Function):
     x_clip/distributed.py:14-39), each rank evaluates only its own row blocks, and a second tiny
     all-gather exchanges (lse, pos) so every rank returns the same global loss.  Backward
     reproduces AllGather.backward's contract (distributed.py:50-54): latent grads are
-    d loss / d(local latents); d temperature is the full-batch gradient on every rank."""
+    d loss / d(local latents); d temperature is the full-batch gradient on every rank.
+
+    sim_reg_weight w > 0 (extra latents only) adds the similarity regularisation (x_clip.py:771-784,
+    :870-873): w/2 * (mean_{i!=j} E_ij^2 + mean_{i!=j} E'_ij^2), E = T T^T - V V^T over the global
+    batch, E' the same over the extra pair (xclip_simreg_*).  It reuses the gathered column operands and
+    rides in the statistics gather, so a step still makes one latent all-gather.  The returned value
+    is then cl_weight * contrastive + w * L_sim (cl_weight lets the auxiliary-loss path weigh the two
+    terms as the reference does).  Global batch 1 gives NaN, the mean of nothing, and no gradient from
+    the term - the reference's behaviour."""
 
     @staticmethod
-    def forward(ctx, zt, zi, zt_x, zi_x, temperature, ops, dcl: bool, use_gather: bool):
+    def forward(ctx, zt, zi, zt_x, zi_x, temperature, ops, dcl: bool, use_gather: bool,
+                sim_reg_weight: float = 0.0, cl_weight: float = 1.0):
         extra = len(ops) == 4
+        sim_w = float(sim_reg_weight)
+        if sim_w != 0.0 and not extra:
+            raise ValueError("the similarity regularisation needs the extra latent pair")
         rank, world = D_.world() if use_gather else (0, 1)
         b = ops[0][0].shape[0]
         D = ops[0][0].shape[1] // 3
@@ -448,11 +460,24 @@ class ContrastiveLossFn(torch.autograd.Function):
         else:
             lse_i, pos_i = K.nce_fwd(rows[I], cols[T], temp_exp, off, dcl)
 
-        stats = torch.stack([lse_t, pos_t, lse_i, pos_i])                      # [4, b]
+        sim_ops = None
+        if sim_w != 0.0:
+            # E = [T | V] . [T | -V]^T per pair: the difference forms inside the fp32 accumulator
+            sim_ops = [(K.simreg_pack(rows[t], rows[v], False), K.simreg_pack(cols[t], cols[v], True))
+                       for t, v in ((T, I), (TX, IX))]
+            sim_rows = [K.simreg_fwd(a, c, off) for a, c in sim_ops]
+
+        stats = torch.stack([lse_t, pos_t, lse_i, pos_i] + (sim_rows if sim_ops else []))   # [4 or 6, b]
         gstats = D_.gather_stats(stats) if world > 1 else stats
         loss = ((gstats[0] - gstats[1]).sum() + (gstats[2] - gstats[3]).sum()) / (2.0 * Bg)
+        if sim_ops:
+            # mean over the Bg (Bg - 1) off-diagonal entries; 0 / 0 = NaN at Bg = 1 like the reference
+            loss = cl_weight * loss + sim_w * ((gstats[4].sum() + gstats[5].sum()) / (2.0 * Bg * (Bg - 1)))
+        elif cl_weight != 1.0:
+            loss = cl_weight * loss
 
         ctx.cfg = (dcl, extra, rank, world, b, D, Bg, off)
+        ctx.sim = (sim_w, float(cl_weight), sim_ops)
         ctx.temp_exp = temp_exp
         ctx.rows, ctx.cols = rows, cols
         # xclip_nce_bwd reads lse_col with 16-byte vector loads.  Row k of the [4, Bg] stats starts
@@ -466,7 +491,9 @@ class ContrastiveLossFn(torch.autograd.Function):
         temp_exp = ctx.temp_exp
         rows, cols = ctx.rows, ctx.cols
         lse_t, lse_i, lse_t_all, lse_i_all = ctx.lse
-        gscale = (gloss.detach().float() / (2.0 * Bg)).reshape(1)
+        sim_w, cl_weight, sim_ops = ctx.sim
+        gl = gloss.detach().float()
+        gscale = ((gl if cl_weight == 1.0 else gl * cl_weight) / (2.0 * Bg)).reshape(1)
         dtemp = torch.zeros(1, device=gloss.device, dtype=F32)
         T, I, TX, IX = 0, 1, 2, 3
 
@@ -485,10 +512,20 @@ class ContrastiveLossFn(torch.autograd.Function):
             dzi = latent_grad(I, T, None, lse_t_all, 0.0, 1.0, 1.0, False)
             dzi_x = latent_grad(IX, TX, lse_i, None, 1.0, 0.0, 1.0, True)
             dzt_x = latent_grad(TX, IX, None, lse_i_all, 0.0, 1.0, 1.0, False)
+        if sim_ops and Bg > 1:
+            # d(w L_sim)/dt_r = (2w/N) sum_j E_rj t_j, d/dv_r = -(2w/N) sum_j E_rj v_j over the global j
+            sgs = (gloss.detach().float() * (2.0 * sim_w / (Bg * (Bg - 1.0)))).reshape(1)
+            for (a, c), t, v, dt_, dv_ in zip(sim_ops, (T, TX), (I, IX), (dzt, dzt_x), (dzi, dzi_x)):
+                g = K.simreg_bwd(a, c, off, sgs)
+                K.gemm(g, _pad_rows(cols[t][:, :D], g.shape[1]), b_major=1, out=dt_, accumulate=True)
+                K.gemm(g, _pad_rows(cols[v][:, :D], g.shape[1]), b_major=1, out=dv_, alpha=-1.0,
+                       accumulate=True)
+                del g
         if world > 1:
             D_.all_reduce_sum_(dtemp)       # every rank holds the full-batch d loss / d temperature
-        ctx.rows = ctx.cols = None
-        return (dzt, dzi, dzt_x, dzi_x, dtemp.reshape(()), None, None, None)
+        ctx.rows = ctx.cols = ctx.sim = None
+        grads = (dzt, dzi, dzt_x, dzi_x, dtemp.reshape(()))
+        return grads + (None,) * (len(ctx.needs_input_grad) - len(grads))
 
 
 def _pad_rows(m: torch.Tensor, rows: int) -> torch.Tensor:
@@ -509,7 +546,9 @@ def _avail_bytes(dev) -> int:
 
 
 # HBM head-room the retention planner leaves untouched: contrastive-loss workspace (g[b, B_g] bf16
-# per direction, gathered operands), gradient buckets, allocator slack.
+# per direction, gathered operands), gradient buckets, allocator slack.  The similarity
+# regularisation adds its packed operands, 24 (b + B_g) D bytes for the two latent pairs, and one
+# more transient g[b, B_g] bf16 at a time: 0.72 GB at b = 4096, B_g = 32768, D = 512 - inside the margin.
 RETAIN_MARGIN_BYTES = 10 << 30
 # transient buffers of one chunk's backward (du 8d + a few d-wide rows of one layer) relative to
 # the chunk's saved activations (22 d per token-layer x depth)
@@ -620,7 +659,8 @@ class ChunkedClipLossFn(torch.autograd.Function):
             loss = ContrastiveLossFn.apply(
                 leaves[0], leaves[1], leaves[2] if nsets == 4 else None,
                 leaves[3] if nsets == 4 else None, temp_leaf, ops_all,
-                clip.decoupled_contrastive_learning, clip.requires_all_gather)
+                clip.decoupled_contrastive_learning, clip.requires_all_gather,
+                *((clip.sim_reg_loss_weight, 1.0) if clip.has_sim_reg_loss else ()))
         ctx.clip, ctx.inputs = clip, (text, image, text_mask)
         ctx.bounds, ctx.rng_states, ctx.kept = bounds, rng_states, kept
         ctx.graph = (loss, leaves, temp_leaf)

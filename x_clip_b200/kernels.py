@@ -425,6 +425,50 @@ def nce_bwd(a, b, temp_exp, diag_offset, dcl, lse_row, lse_col, w_row, w_col, w_
     return g
 
 
+def simreg_pack(t, v, negate_v):
+    """bf16 [rows, 2k] = [t | v] or [t | -v] (see xclip_simreg_pack)."""
+    _need(t, BF16, "t"); _need(v, BF16, "v")
+    if t.shape != v.shape or t.dim() != 2 or not (t.is_contiguous() and v.is_contiguous()):
+        raise _lib.XClipB200Error("simreg_pack: t and v must be contiguous 2-D tensors of one shape")
+    rows, k = t.shape
+    out = torch.empty((rows, 2 * k), device=t.device, dtype=BF16)
+    _call(t, "simreg_small", 0.0, 8.0 * rows * k, "xclip_simreg_pack", t.data_ptr(), v.data_ptr(), rows, k,
+          1 if negate_v else 0, out.data_ptr())
+    return out
+
+
+def simreg_fwd(a, b, diag_offset, loss_accum=None, loss_scale=0.0):
+    """Row sums over the columns c != r + diag_offset of E^2, E = a @ b^T (f32 [R]); see xclip_simreg_fwd."""
+    _need(a, BF16, "a"); _need(b, BF16, "b"); _rows2d(a, "a"); _rows2d(b, "b")
+    if not (a.is_contiguous() and b.is_contiguous()) or a.shape[1] != b.shape[1]:
+        raise _lib.XClipB200Error("simreg_fwd: a and b must be contiguous with one width")
+    R, Kd = a.shape
+    C = b.shape[0]
+    nblk = _lib.load().xclip_nce_num_col_blocks(C)
+    part = torch.empty((nblk, R), device=a.device, dtype=F32)
+    rowsum = torch.empty((R,), device=a.device, dtype=F32)
+    if loss_accum is not None:
+        _need(loss_accum, F32, "loss_accum")
+    _call(a, "simreg_fwd", 2.0 * R * C * Kd, 2.0 * (R + C) * Kd + 4.0 * R, "xclip_simreg_fwd", a.data_ptr(),
+          b.data_ptr(), R, C, Kd, int(diag_offset), part.data_ptr(), rowsum.data_ptr(), _ptr(loss_accum),
+          float(loss_scale))
+    return rowsum
+
+
+def simreg_bwd(a, b, diag_offset, gscale):
+    """bf16 gscale * E [R, roundup8(C)] (diagonal and columns >= C zero); see xclip_simreg_bwd."""
+    _need(a, BF16, "a"); _need(b, BF16, "b"); _need(gscale, F32, "gscale"); _rows2d(a, "a"); _rows2d(b, "b")
+    if not (a.is_contiguous() and b.is_contiguous()) or a.shape[1] != b.shape[1]:
+        raise _lib.XClipB200Error("simreg_bwd: a and b must be contiguous with one width")
+    R, Kd = a.shape
+    C = b.shape[0]
+    ldg = (C + 7) // 8 * 8
+    g = torch.empty((R, ldg), device=a.device, dtype=BF16)
+    _call(a, "simreg_bwd", 2.0 * R * C * Kd, 2.0 * (R + C) * Kd + 2.0 * R * C, "xclip_simreg_bwd", a.data_ptr(),
+          b.data_ptr(), R, C, Kd, int(diag_offset), gscale.data_ptr(), g.data_ptr(), ldg)
+    return g
+
+
 def filip_segmax(a, b, temp_exp, seg_len, col_mul, col_add):
     """Per row of a and per seg_len-long block of rows of b: max / argmax of temp * <a_r, b_c>."""
     _need(a, BF16, "a"); _need(b, BF16, "b")
