@@ -157,7 +157,7 @@ extern "C" int xclip_ff_down(const void* hp, int64_t ldhp, const void* w2g, cons
   p.c = out; p.ldc = ldo;
   p.residual = reinterpret_cast<const bf16*>(residual); p.ldr = ldr;
   p.ff_rowsum = const_cast<float*>(rowsum); p.ff_colvec = colvec; p.ff_stats = stats;
-  p.ff_eps = eps; p.ff_hidden = 4 * d;
+  p.ff_eps = eps; p.ff_hidden = 4 * d; p.ff_inv_hidden = 1.f / (float)(4 * d);
   p.ff_out2 = reinterpret_cast<bf16*>(acc_out); p.ff_ld2 = ldacc;
   return launch_ff<EPI_FF_DOWN>(tmA, tmB, p, reinterpret_cast<cudaStream_t>(stream));
 }

@@ -61,7 +61,13 @@ extern "C" int xclip_gemm_bf16(const void* a, int64_t lda, int a_major, const vo
   }
   if (bias) XCLIP_REQUIRE((reinterpret_cast<uintptr_t>(bias) & 15) == 0, "gemm: bias misaligned");
 
-  const int block_n = (N % 256 == 0 || N > 1024) ? 256 : 128;
+  // 128-wide tiles (ping-pong schedule) when 256 would waste columns, and where the output is narrow
+  // and K short: there a tile's epilogue is large against its k-loop, and hiding it behind the other
+  // warpgroup's k-loop beats the operand reuse of 256-wide tiles (H100, tools/gemm_bench.py: ViT
+  // d = 768 out / dgrad and text d = 512 out fwd / dgrad 4-6 % faster).  Longer K and wider N measure
+  // faster on 256.
+  const bool narrow_short_k = N <= 768 && K <= 768;
+  const int block_n = ((N % 256 != 0 && N <= 1024) || narrow_short_k) ? 128 : 256;
 
   CUtensorMap tmA, tmB;
   if (a_major == 0) {
