@@ -114,7 +114,13 @@ int xclip_cast_f32_bf16(const float* src, void* dst, int64_t n, xclip_stream_t s
  * per CTA for any n).  Both compute the same blocks in the same order: bit-identical results.
  * qkv bf16 [B*n, ld_qkv] holds q | k | v, each heads*64 wide, head-major inside.
  * key_mask uint8 [B, n] (1 = attend; may be NULL).  o bf16 [B*n, ldo] (heads merged).
- * lse f32 [B, heads, n]: base-2 log-sum-exp of scale*log2(e)*scores (saved for backward). */
+ * lse f32 [B, heads, n]: base-2 log-sum-exp of scale*log2(e)*scores (saved for backward).
+ * A row with no visible key (all its keys masked, or masked and above the causal diagonal) gets, as
+ * in the reference, the uniform softmax over all n keys, and lse = -FLT_MAX.  Its backward follows
+ * masked_fill: no gradient reaches a masked score, so the row's dq is 0, it adds nothing to dk, and
+ * it adds dO / n to the dv of every key.
+ * scale must be > 0, ld_* multiples of 8 and at least their operand's width, and qkv, o, d_o and
+ * dqkv 16-byte aligned; otherwise both calls return XCLIP_ERR_INVALID without launching. */
 int xclip_attn_fwd(const void* qkv, int64_t ld_qkv, const uint8_t* key_mask, void* o, int64_t ldo,
                    float* lse, int B, int n, int heads, float scale, int causal,
                    xclip_stream_t stream);

@@ -17,7 +17,12 @@
 // Masking follows the reference: a masked key (key_mask = 0, or j > i under the causal mask of
 // :233-236) gets the score -FLT_MAX after scaling; keys beyond n do not exist (-inf).  Causal blocks
 // wholly above the diagonal are not skipped: a row whose visible keys are all key-masked gets the
-// reference's uniform softmax over all n keys.
+// reference's uniform softmax over all n keys, and lse = -FLT_MAX (-FLT_MAX + log2(n) rounds to
+// -FLT_MAX; no row with a visible key can have that lse).  Its backward follows masked_fill, which
+// passes no gradient to a masked score: dq = 0, nothing into dk, and dO / n into the dv of every key.
+// The backward kernels read such a row's lse as +inf, so the block bodies give it p = 0 everywhere
+// (on every other row a hidden score already has p = 0 exactly, hence ds = 0), and the dK / dV
+// kernels add its dO / n to dv after the key loop (attn_dv_empty_rows).
 #include "common.cuh"
 #include "host.h"
 
@@ -158,6 +163,32 @@ __device__ __forceinline__ void store_rows(bf16* dst, long long ld, int r0, int 
   }
 }
 
+// lse as the backward reads it: +inf for a row with no visible key (-FLT_MAX), so that the block
+// bodies give it p = exp2(t - lse) = 0 on every key, hence ds = 0 and nothing into dq, dk or dv
+__device__ __forceinline__ float attn_bwd_lse(float lse) { return lse == -FLT_MAX ? INFINITY : lse; }
+
+// dv += (sum of dO_i over the head's rows i with no visible key) / n: the reference's uniform p = 1/n
+// of those rows, the same for every key.  Called by all threads after the key loop when such a row
+// exists; `scratch` is 128 floats of shared memory that the key loop does not read.
+__device__ __forceinline__ void attn_dv_empty_rows(float (&dv)[8][4], const bf16* dO, long long lddo,
+                                                   const float* lse_bh, int n, float* scratch) {
+  const int lane = threadIdx.x & 31, d = threadIdx.x & 63;
+  float sum = 0.f;
+  for (int i = threadIdx.x >> 6; i < n; i += 2)
+    if (lse_bh[i] == -FLT_MAX) sum += __bfloat162float(dO[(long long)i * lddo + d]);
+  __syncthreads();   // no warp still loads its fragments from the scratch tile
+  scratch[threadIdx.x] = sum;
+  __syncthreads();
+  const float inv_n = 1.f / (float)n;
+#pragma unroll
+  for (int nt = 0; nt < 8; ++nt)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int c = nt * 8 + 2 * (lane & 3) + (e & 1);
+      dv[nt][e] += (scratch[c] + scratch[kAttnRows + c]) * inv_n;
+    }
+}
+
 // ---- per-block bodies, shared by the resident and the streaming kernels ---------------------------
 // Each processes one 64-row block of the streamed operand for the warp's 16 rows.  The block's tiles
 // sit at rows [c0, c0 + 64) of tK / tV (tQ / tdO); kb (qb) is the block's first global row and
@@ -265,7 +296,7 @@ __device__ __forceinline__ void attn_dkdv_block(const uint32_t (&kf)[4][4], cons
   mma_ab(dk, df, tQ, c0);
 }
 
-// dQ: ds = p (dp - delta) over one block of keys, dq += ds k
+// dQ: ds = p (dp - delta) over one block of keys, dq += ds k (a hidden score has p = 0, so ds = 0)
 template <bool kCausal>
 __device__ __forceinline__ void attn_dq_block(const uint32_t (&qf)[4][4], const uint32_t (&of)[4][4],
                                               const uint8_t* tK, const uint8_t* tV, int c0,
@@ -443,13 +474,16 @@ attn_bwd_dkdv_kernel(const bf16* __restrict__ qkv, long long ld, const uint8_t* 
   attn_load_rows(sQ, base + h * kAttnDh, ld, 0, NP, n);
   attn_load_rows(sdO, d_o + (long long)b * n * lddo + h * kAttnDh, lddo, 0, NP, n);
   const long long bh = (long long)b * H + h;
+  bool empty = false;   // some row of the head has no visible key
   for (int i = threadIdx.x; i < NP; i += kAttnThreads) {
-    sLse[i] = i < n ? lse[bh * n + i] : 0.f;
+    const float l = i < n ? lse[bh * n + i] : 0.f;
+    empty |= l == -FLT_MAX;
+    sLse[i] = attn_bwd_lse(l);
     sDelta[i] = i < n ? delta[bh * n + i] : 0.f;
   }
   load_key_flags(sFlag, mask, b, n, k0, kAttnRows);
   cp_async_wait_all();
-  __syncthreads();
+  const bool any_empty = __syncthreads_or(empty);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int r0 = warp * 16;
@@ -464,6 +498,9 @@ attn_bwd_dkdv_kernel(const bf16* __restrict__ qkv, long long ld, const uint8_t* 
   zero_acc(dv);
   for (int qb = 0; qb < NP; qb += 64)
     attn_dkdv_block<kCausal>(kf, vf, sQ, sdO, qb, sLse + qb, sDelta + qb, qb, key, flag, n, scale_log2, dk, dv);
+  if (any_empty)
+    attn_dv_empty_rows(dv, d_o + (long long)b * n * lddo + h * kAttnDh, lddo, lse + bh * n, n,
+                       reinterpret_cast<float*>(sK));
   bf16* out = dqkv + (long long)b * n * ldd;
   store_rows(out + (H + h) * kAttnDh, ldd, k0 + r0, n, dk, scale);
   store_rows(out + (2 * H + h) * kAttnDh, ldd, k0 + r0, n, dv, 1.f);
@@ -497,7 +534,10 @@ attn_bwd_dkdv_stream_kernel(const bf16* __restrict__ qkv, long long ld, const ui
   attn_load_rows(sV, base + (2 * H + h) * kAttnDh, ld, k0, kAttnRows, n);
   attn_load_rows(ring, gQ, ld, 0, kAttnRows, n);
   attn_load_rows(ring + kAttnTile, gdO, lddo, 0, kAttnRows, n);
-  sStat[threadIdx.x] = srow < n ? gStat[srow] : 0.f;
+  const bool is_lse = threadIdx.x < kAttnRows;
+  float stat0 = srow < n ? gStat[srow] : 0.f;
+  bool empty = is_lse && stat0 == -FLT_MAX;   // some row of the head has no visible key
+  sStat[threadIdx.x] = is_lse ? attn_bwd_lse(stat0) : stat0;
   load_key_flags(sFlag, mask, b, n, k0, kAttnRows);
   cp_async_wait_all();
   __syncthreads();
@@ -522,6 +562,10 @@ attn_bwd_dkdv_stream_kernel(const bf16* __restrict__ qkv, long long ld, const ui
       attn_load_rows(ring + nxt * 2 * kAttnTile + kAttnTile, gdO, lddo, qb + kAttnRows, kAttnRows, n);
       const int q = qb + kAttnRows + srow;
       if (q < n) next_stat = gStat[q];
+      if (is_lse) {
+        empty |= next_stat == -FLT_MAX;
+        next_stat = attn_bwd_lse(next_stat);
+      }
     }
     const uint8_t* cur = ring + (i & 1) * 2 * kAttnTile;
     const float* st = sStat + (i & 1) * 2 * kAttnRows;
@@ -531,6 +575,8 @@ attn_bwd_dkdv_stream_kernel(const bf16* __restrict__ qkv, long long ld, const ui
     cp_async_wait_all();   // block i + 1 landed, and no thread reads stage i & 1 any more
     __syncthreads();
   }
+  if (__syncthreads_or(empty))
+    attn_dv_empty_rows(dv, gdO, lddo, lse + bh * n, n, reinterpret_cast<float*>(sK));
   bf16* out = dqkv + (long long)b * n * ldd;
   store_rows(out + (H + h) * kAttnDh, ldd, k0 + r0, n, dk, scale);
   store_rows(out + (2 * H + h) * kAttnDh, ldd, k0 + r0, n, dv, 1.f);
@@ -573,7 +619,7 @@ attn_bwd_dq_kernel(const bf16* __restrict__ qkv, long long ld, const uint8_t* __
   float lr[2], dr[2];
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {
-    lr[hh] = row[hh] < n ? lse[bh * n + row[hh]] : 0.f;
+    lr[hh] = row[hh] < n ? attn_bwd_lse(lse[bh * n + row[hh]]) : 0.f;
     dr[hh] = row[hh] < n ? delta[bh * n + row[hh]] : 0.f;
   }
   float dq[8][4];
@@ -620,7 +666,7 @@ attn_bwd_dq_stream_kernel(const bf16* __restrict__ qkv, long long ld, const uint
   float lr[2], dr[2];
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {
-    lr[hh] = row[hh] < n ? lse[bh * n + row[hh]] : 0.f;
+    lr[hh] = row[hh] < n ? attn_bwd_lse(lse[bh * n + row[hh]]) : 0.f;
     dr[hh] = row[hh] < n ? delta[bh * n + row[hh]] : 0.f;
   }
   float dq[8][4];
@@ -690,6 +736,7 @@ extern "C" int xclip_attn_bwd(const void* qkv, int64_t ld_qkv, const uint8_t* ke
   if (rc) return rc;
   XCLIP_REQUIRE(qkv && o && d_o && lse && delta && dqkv, "attn_bwd: null pointer");
   XCLIP_REQUIRE(B > 0 && heads > 0 && n > 0, "attn_bwd: bad sizes B=%d n=%d heads=%d", B, n, heads);
+  XCLIP_REQUIRE(scale > 0.f, "attn_bwd: scale must be positive");
   XCLIP_REQUIRE(ld_qkv % 8 == 0 && ld_qkv >= 3 * heads * kAttnDh && ld_dqkv % 8 == 0 &&
                     ld_dqkv >= 3 * heads * kAttnDh && ldo % 8 == 0 && lddo % 8 == 0 &&
                     ldo >= heads * kAttnDh && lddo >= heads * kAttnDh,

@@ -241,6 +241,9 @@ def attn_fwd(qkv, key_mask, B, n, heads, scale, causal=False):
 
 def attn_bwd(qkv, key_mask, o, d_o, lse, B, n, heads, scale, causal=False):
     _need(d_o, BF16, "d_o"); _rows2d(d_o, "d_o")
+    if key_mask is not None:
+        if key_mask.dtype != torch.bool or tuple(key_mask.shape) != (B, n) or not key_mask.is_contiguous():
+            raise _lib.XClipB200Error("attn_bwd: key_mask must be a contiguous bool [B, n]")
     dqkv = torch.empty_like(qkv)
     delta = torch.empty((B, heads, n), device=qkv.device, dtype=F32)
     _call(qkv, "attn_bwd", 10.0 * B * heads * n * n * 64, 2.0 * B * n * heads * 64 * 8, "xclip_attn_bwd", qkv.data_ptr(), qkv.stride(0), _ptr(key_mask), o.data_ptr(),
