@@ -189,6 +189,14 @@ int xclip_simreg_bwd(const void* a, const void* b, int R, int C, int K, int diag
  *          every row r and sample y: seg_max[r,y] = max_i s, seg_arg[r,y] = argmax_i s with
  *          s = *temp_exp * <a_r, b_(y,i)> (optionally s*col_mul[c] + col_add[c]: padded text
  *          tokens get col_mul 0 / col_add -FLT_MAX, the reference's masked_fill at :810).
+ *          Ties go to the lowest index; a segment whose columns are all masked gives -FLT_MAX at
+ *          index 0.
+ * segmax_any : segmax for any seg_len >= 1 (C % seg_len == 0), same values, ties and masks.
+ *          keys: caller-owned workspace of 8 * R * (C / seg_len) bytes, 8-byte aligned, no
+ *          initialisation needed (the call zeroes it; it holds nothing of use afterwards).  a, b
+ *          16-byte aligned; temp_exp, seg_max, seg_arg, col_mul, col_add 4-byte aligned.
+ *          Refused without a launch: seg_len < 1, C not a whole number of segments, null or
+ *          misaligned pointers, only one of col_mul / col_add.
  * reduce : out[a,b] = sum_k weights[a*len+k] * seg_max[(a*len+k), b]  ([samples, nseg] or
  *          transposed) - the masked mean over text tokens (:807) / mean over image tokens (:811).
  * nce_fwd/bwd : row-wise InfoNCE / DCL on an [R,C] fp32 similarity matrix (R local texts, C all
@@ -200,10 +208,17 @@ int xclip_simreg_bwd(const void* a, const void* b, int R, int C, int K, int diag
  * expand : rows [row0,row0+rows) of the backward operand G[R,C] (bf16): at the argmax column
  *          of each (row, sample) the value *temp_exp * wmat[row/rows_per_sample, sample] *
  *          rowscale[row], zero elsewhere; *dtemp += sum w * seg_max.  d rows = G @ b and
- *          d cols += G^T @ a then run on xclip_gemm_bf16. */
+ *          d cols += G^T @ a then run on xclip_gemm_bf16.  Any seg_len >= 1; g is [rows, ldg]
+ *          with ldg % 8 == 0 and ldg >= nseg * seg_len, 16-byte aligned.  Columns
+ *          [nseg * seg_len, roundup8(nseg * seg_len)) are written as zeros, the rest of the row is
+ *          left alone; the gradient GEMMs take G[:, :nseg * seg_len] and never read past it. */
 int xclip_filip_segmax(const void* a, const void* b, int R, int C, int D, const float* temp_exp,
                        int seg_len, const float* col_mul, const float* col_add, float* seg_max,
                        int* seg_arg, xclip_stream_t stream);
+int xclip_filip_segmax_any(const void* a, const void* b, int R, int C, int D,
+                           const float* temp_exp, int seg_len, const float* col_mul,
+                           const float* col_add, float* seg_max, int* seg_arg, void* keys,
+                           xclip_stream_t stream);
 int xclip_filip_reduce(const float* seg_max, const float* weights, int samples, int len, int nseg,
                        float* out, int transpose_out, xclip_stream_t stream);
 int xclip_filip_nce_fwd(const float* s, int R, int C, int diag_off, int dcl,

@@ -88,6 +88,8 @@ SIGNATURES = {
                                      c_void_p]),
     "xclip_filip_segmax": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int,
                                    c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "xclip_filip_segmax_any": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int,
+                                       c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "xclip_filip_reduce": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int,
                                    c_void_p]),
     "xclip_filip_nce_fwd": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,

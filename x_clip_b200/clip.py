@@ -8,7 +8,9 @@ done by the CUDA kernels behind include/xclip_b200.h, scheduled by x_clip_b200.e
 
 Sequence length is not limited by the non-causal attention: image towers such as ViT-B/16 at 384 px
 (576 patches) and long text towers run on the same kernels (streamed through shared memory above
-320 tokens).  Feature combinations the kernels do not cover raise at construction (never a silent
+320 tokens).  The FILIP loss (`use_all_token_embeds=True`) takes any number of text and image
+tokens: cfg3's 77 x 196 (98 under patch dropout), 576-patch towers and grids smaller than 16 tokens
+run on the same segment-max kernels.  Feature combinations the kernels do not cover raise at construction (never a silent
 CPU or eager fallback): dim_head != 64, model dims not multiples of 256, a causal text tower longer than
 128 tokens, rotary + causal together (broken in the reference itself: n+1 angles for n tokens,
 x_clip.py:328), dropout > 0 and conv-downsampled image latents.  MLM, SimSiam / SimCLR and the

@@ -8,6 +8,9 @@
 // The 6-D similarity tensor (68.7 G elements at cfg4) is never materialised:
 //   xclip_filip_segmax : the wgmma GEMM with the EPI_SEGMAX epilogue produces, per token row and
 //                        per sample of the other modality, max + argmax over that sample's tokens
+//                        (multiples of 16 tokens, <= 256: tiles hold whole samples)
+//   xclip_filip_segmax_any : the same for any token count (EPI_SEGMAX_ANY: 256-column tiles,
+//                        samples cut by a tile edge merged through 64-bit keys, then unpacked)
 //   xclip_filip_reduce : [tokens, B] maxima -> [B, B] similarity (masked mean / mean)
 //   xclip_filip_nce_*  : row-wise InfoNCE / DCL on a [B,B] fp32 matrix (warp-shuffle reductions)
 //   xclip_filip_expand : backward: one-hot (at the argmax) weighted bf16 operand G[rows, cols]
@@ -127,6 +130,67 @@ filip_expand_kernel(const int* __restrict__ seg_arg, const float* __restrict__ s
   }
 }
 
+// filip_expand_kernel for seg_len % 8 != 0: an 8-column vector may hold the end of one segment and
+// the start of the next (several when seg_len < 8), so every column steps its own (segment,
+// position).  Columns [nseg * seg_len, roundup8) of the last vector are written as zeros.
+__global__ void __launch_bounds__(256)
+filip_expand_any_kernel(const int* __restrict__ seg_arg, const float* __restrict__ seg_max,
+                        const float* __restrict__ wmat, const float* __restrict__ rowscale,
+                        const float* __restrict__ alpha_dev, int row0, int rows, int rows_per_sample,
+                        int seg_len, int nseg, bf16* __restrict__ g, long long ldg,
+                        float* __restrict__ dtemp) {
+  const float alpha = __ldg(alpha_dev);
+  const int C = nseg * seg_len;
+  const int vec_per_row = (C + 7) / 8;
+  float tsum = 0.f;
+  for (long long v = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+       v < (long long)rows * vec_per_row; v += (long long)gridDim.x * blockDim.x) {
+    const int lr = (int)(v / vec_per_row);
+    const int c0 = (int)(v % vec_per_row) * 8;
+    const long long r = row0 + lr;
+    const int* arg_row = seg_arg + r * nseg;
+    const float* w_row = wmat + (r / rows_per_sample) * nseg;
+    int seg = c0 / seg_len;
+    int pos = c0 - seg * seg_len;
+    int a = arg_row[seg];
+    bf16 vals[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      vals[k] = __float2bfloat16_rn(0.f);
+      if (c0 + k < C) {
+        if (pos == a) {
+          const float w = w_row[seg] * rowscale[r];
+          if (w != 0.f) {
+            tsum += w * seg_max[r * nseg + seg];
+            vals[k] = __float2bfloat16_rn(w * alpha);
+          }
+        }
+        if (++pos == seg_len) {
+          pos = 0;
+          if (++seg < nseg) a = arg_row[seg];
+        }
+      }
+    }
+    *reinterpret_cast<uint4*>(g + lr * ldg + c0) = *reinterpret_cast<const uint4*>(vals);
+  }
+  if (dtemp != nullptr) {
+    tsum = warp_sum(tsum);
+    if ((threadIdx.x & 31) == 0 && tsum != 0.f) atomicAdd(dtemp, tsum);
+  }
+}
+
+// keys of EPI_SEGMAX_ANY -> seg_max (f32) and seg_arg (int32)
+__global__ void __launch_bounds__(256)
+filip_unpack_keys_kernel(const unsigned long long* __restrict__ keys, long long n,
+                         float* __restrict__ seg_max, int* __restrict__ seg_arg) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n;
+       i += (long long)gridDim.x * blockDim.x) {
+    const unsigned long long k = keys[i];
+    seg_max[i] = segmax_key_value(k);
+    seg_arg[i] = segmax_key_index(k);
+  }
+}
+
 }  // namespace xclip
 
 using namespace xclip;
@@ -169,6 +233,60 @@ extern "C" int xclip_filip_segmax(const void* a, const void* b, int R, int C, in
   }
   kern<<<grid, kGemmThreads, S::kTotal, reinterpret_cast<cudaStream_t>(stream)>>>(tmA, tmB, p);
   XCLIP_LAUNCH_CHECK("gemm_bf16_kernel<segmax>");
+  return XCLIP_OK;
+}
+
+extern "C" int xclip_filip_segmax_any(const void* a, const void* b, int R, int C, int D,
+                                      const float* temp_exp, int seg_len, const float* col_mul,
+                                      const float* col_add, float* seg_max, int* seg_arg, void* keys,
+                                      xclip_stream_t stream) {
+  int rc = xclip_init();
+  if (rc) return rc;
+  XCLIP_REQUIRE(a && b && temp_exp && seg_max && seg_arg && keys, "filip_segmax_any: null pointer");
+  XCLIP_REQUIRE(R > 0 && C > 0 && D > 0 && D % 8 == 0, "filip_segmax_any: bad sizes");
+  XCLIP_REQUIRE(seg_len >= 1 && C % seg_len == 0,
+                "filip_segmax_any: C (%d) must be a whole number of segments of seg_len (%d) >= 1 tokens",
+                C, seg_len);
+  XCLIP_REQUIRE((col_mul == nullptr) == (col_add == nullptr), "filip_segmax_any: mask tables mismatch");
+  XCLIP_REQUIRE(((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b)) & 15) == 0,
+                "filip_segmax_any: misaligned latents");
+  XCLIP_REQUIRE(((reinterpret_cast<uintptr_t>(temp_exp) | reinterpret_cast<uintptr_t>(seg_max) |
+                  reinterpret_cast<uintptr_t>(seg_arg) | reinterpret_cast<uintptr_t>(col_mul) |
+                  reinterpret_cast<uintptr_t>(col_add)) & 3) == 0,
+                "filip_segmax_any: misaligned fp32 / int32 pointer");
+  XCLIP_REQUIRE((reinterpret_cast<uintptr_t>(keys) & 7) == 0, "filip_segmax_any: misaligned keys");
+  const int nseg = C / seg_len;
+  const long long nkeys = (long long)R * nseg;
+  CUtensorMap tmA, tmB;
+  rc = encode_2d_bf16(&tmA, a, (uint64_t)D, (uint64_t)R, (uint64_t)D, 64, kGemmBlockM);
+  if (rc) return rc;
+  rc = encode_2d_bf16(&tmB, b, (uint64_t)D, (uint64_t)C, (uint64_t)D, 64, 256);
+  if (rc) return rc;
+  GemmParams p = {};
+  p.M = R; p.N = C; p.K = D; p.split_k = 1;
+  p.raster_m_fast = (R <= C) ? 1 : 0;
+  p.alpha_dev = temp_exp;
+  p.seg_len = seg_len;
+  p.n_segs = nseg;
+  p.col_mul = col_mul; p.col_add = col_add;
+  p.seg_keys = reinterpret_cast<unsigned long long*>(keys);
+  const long long tiles = (long long)((R + kGemmBlockM - 1) / kGemmBlockM) * ((C + 255) / 256);
+  const int grid = (int)(tiles < num_sms() ? tiles : num_sms());
+  using S = GemmSmem<256>;
+  auto kern = gemm_bf16_kernel<256, kMajorK, kMajorK, EPI_SEGMAX_ANY>;
+  {
+    const int rc_attr = ensure_dynamic_smem(reinterpret_cast<const void*>(kern), S::kTotal);
+    if (rc_attr) return rc_attr;
+  }
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  XCLIP_CUDA(cudaMemsetAsync(keys, 0, (size_t)nkeys * 8, st));
+  kern<<<grid, kGemmThreads, S::kTotal, st>>>(tmA, tmB, p);
+  XCLIP_LAUNCH_CHECK("gemm_bf16_kernel<segmax_any>");
+  long long blocks = (nkeys + 255) / 256;
+  if (blocks > (long long)num_sms() * 16) blocks = (long long)num_sms() * 16;
+  filip_unpack_keys_kernel<<<(int)blocks, 256, 0, st>>>(
+      reinterpret_cast<const unsigned long long*>(keys), nkeys, seg_max, seg_arg);
+  XCLIP_LAUNCH_CHECK("filip_unpack_keys_kernel");
   return XCLIP_OK;
 }
 
@@ -218,16 +336,23 @@ extern "C" int xclip_filip_expand(const int* seg_arg, const float* seg_max, cons
   int rc = xclip_init();
   if (rc) return rc;
   XCLIP_REQUIRE(seg_arg && seg_max && wmat && rowscale && temp_exp && g, "filip_expand: null pointer");
-  XCLIP_REQUIRE(rows > 0 && rows_per_sample > 0 && seg_len % 8 == 0 && nseg > 0 &&
+  XCLIP_REQUIRE(rows > 0 && rows_per_sample > 0 && seg_len >= 1 && nseg > 0 &&
                     ldg >= (int64_t)nseg * seg_len && ldg % 8 == 0,
                 "filip_expand: bad sizes");
   XCLIP_REQUIRE((reinterpret_cast<uintptr_t>(g) & 15) == 0, "filip_expand: misaligned g");
-  const long long vecs = (long long)rows * nseg * seg_len / 8;
+  const long long vecs = (long long)rows * ((nseg * seg_len + 7) / 8);
   long long blocks = (vecs + 255) / 256;
   if (blocks > (long long)num_sms() * 16) blocks = (long long)num_sms() * 16;
-  filip_expand_kernel<<<(int)blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      seg_arg, seg_max, wmat, rowscale, temp_exp, row0, rows, rows_per_sample, seg_len, nseg,
-      reinterpret_cast<bf16*>(g), ldg, dtemp);
-  XCLIP_LAUNCH_CHECK("filip_expand_kernel");
+  if (seg_len % 8 == 0) {
+    filip_expand_kernel<<<(int)blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+        seg_arg, seg_max, wmat, rowscale, temp_exp, row0, rows, rows_per_sample, seg_len, nseg,
+        reinterpret_cast<bf16*>(g), ldg, dtemp);
+    XCLIP_LAUNCH_CHECK("filip_expand_kernel");
+  } else {
+    filip_expand_any_kernel<<<(int)blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+        seg_arg, seg_max, wmat, rowscale, temp_exp, row0, rows, rows_per_sample, seg_len, nseg,
+        reinterpret_cast<bf16*>(g), ldg, dtemp);
+    XCLIP_LAUNCH_CHECK("filip_expand_any_kernel");
+  }
   return XCLIP_OK;
 }

@@ -90,6 +90,10 @@ struct GemmParams {
   bf16* ff_out2;           // UP: hp [M, 4d];  DOWN: bf16(acc) [M, d]
   long long ff_ld2;
   const float* ff_ab;      // BWD: [M,2] per-row (mean_k(gdh), mean_k(gdh * hn)) from xclip_ff_bwd_prep
+  // ---- FILIP segment-max epilogue for any segment length (EPI_SEGMAX_ANY): seg_len, n_segs,
+  // col_mul and col_add as above; the result goes to one packed key per (row, segment)
+  // (segmax_key), zeroed before the launch
+  unsigned long long* seg_keys;  // [M, n_segs]
 };
 
 constexpr int EPI_STORE = 0;    // C = alpha*acc (+bias) (+residual)
@@ -121,6 +125,11 @@ constexpr int EPI_FF_BWD = 6;
 //   EPI_SIMREG_BWD  C = bf16(*gscale_dev * E), zero on the excluded columns up to ldc
 constexpr int EPI_SIMREG_FWD = 7;
 constexpr int EPI_SIMREG_BWD = 8;
+// FILIP segment max for any seg_len >= 1 (BLOCK_N = 256).  Tiles advance by 256 columns whatever
+// seg_len is, so a segment may start or end anywhere in a tile, and may span several tiles.  Each
+// (row, segment) result is one 64-bit key (segmax_key); a segment wholly inside the tile stores it,
+// a piece cut by a tile edge merges it with atom.max.  filip.cu unpacks the keys afterwards.
+constexpr int EPI_SEGMAX_ANY = 9;
 
 constexpr int kGemmBlockM = 128;
 constexpr int kGemmBlockK = 64;
@@ -190,6 +199,23 @@ __device__ __forceinline__ void st_bf16x8(bf16* dst, const float* f) {
   *reinterpret_cast<uint4*>(dst) = o;
 }
 __device__ __forceinline__ float bf16_rn(float x) { return __bfloat162float(__float2bfloat16_rn(x)); }
+
+// (value, index) of a segment maximum as one unsigned 64-bit key whose integer order is the order
+// of the results: high word = the order-preserving image of the fp32 value (negative values
+// bit-inverted, positive ones with the sign bit set), low word = 0xFFFFFFFF - index, so that on
+// equal values the lower index is the larger key.  Every key, -FLT_MAX and -inf included, is > 0.
+__device__ __forceinline__ unsigned long long segmax_key(float v, int idx) {
+  const uint32_t b = __float_as_uint(v);
+  const uint32_t o = (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+  return (static_cast<unsigned long long>(o) << 32) | (0xFFFFFFFFu - static_cast<uint32_t>(idx));
+}
+__device__ __forceinline__ float segmax_key_value(unsigned long long k) {
+  const uint32_t o = static_cast<uint32_t>(k >> 32);
+  return __uint_as_float((o & 0x80000000u) ? (o & 0x7FFFFFFFu) : ~o);
+}
+__device__ __forceinline__ int segmax_key_index(unsigned long long k) {
+  return static_cast<int>(0xFFFFFFFFu - static_cast<uint32_t>(k));
+}
 
 // Epilogue of one 128 x BLOCK_N tile for EPI_STORE; `stage(c)` makes column c of the tile readable.
 template <int BLOCK_N, class Stage>
@@ -545,6 +571,58 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           p.seg_arg[o] = best_i;
         }
       }
+    } else if constexpr (EPI == EPI_SEGMAX_ANY) {
+      // (segment, position) of the tile's first column from one division, then stepped per column;
+      // the column walk is the same for every thread of the CTA, so its branches do not diverge.
+      // Values and the strict '>' scan are those of EPI_SEGMAX.
+      const float alpha = __ldg(p.alpha_dev);
+      const int L = p.seg_len;
+      const int col_base = n_blk * BLOCK_N;
+      const int valid = min(BLOCK_N, p.N - col_base);
+      int seg = col_base / L;
+      int pos = col_base - seg * L;
+      bool whole = pos == 0;                       // the current segment starts inside this tile
+      float best = -INFINITY;
+      int best_i = 0;
+      unsigned long long* keys = p.seg_keys + (long long)(row_ok ? row : 0) * p.n_segs;
+      auto close_segment = [&]() {                 // the current segment ends at this column
+        if (row_ok) {
+          const unsigned long long k = segmax_key(best, best_i);
+          if (whole) keys[seg] = k;
+          else atomicMax(keys + seg, k);
+        }
+        ++seg; pos = 0; whole = true; best = -INFINITY; best_i = 0;
+      };
+#pragma unroll 1
+      for (int c0 = 0; c0 < valid; c0 += 16) {
+        need(c0);
+        float v[16];
+        acc_ld16(acc_row, acc_sw, c0, v);
+        const int col0 = col_base + c0;
+        if (c0 + 16 <= valid && pos + 16 <= L) {  // the whole chunk lies inside one segment
+#pragma unroll
+          for (int i = 0; i < 16; ++i) {
+            float sv = v[i] * alpha;
+            if (p.col_mul != nullptr) sv = fmaf(v[i] * alpha, p.col_mul[col0 + i], p.col_add[col0 + i]);
+            if (sv > best) { best = sv; best_i = pos + i; }
+          }
+          pos += 16;
+          if (pos == L) close_segment();
+        } else {                                   // segment boundaries inside the chunk, or C ends
+#pragma unroll
+          for (int i = 0; i < 16; ++i) {
+            if (c0 + i < valid) {
+              float sv = v[i] * alpha;
+              if (p.col_mul != nullptr) sv = fmaf(v[i] * alpha, p.col_mul[col0 + i], p.col_add[col0 + i]);
+              if (sv > best) { best = sv; best_i = pos; }
+              if (++pos == L) close_segment();
+            }
+          }
+        }
+      }
+      // a segment that goes on in the next tile: merge this piece (C is a whole number of
+      // segments, so this happens only on a full tile)
+      if (pos != 0 && row_ok) atomicMax(keys + seg, segmax_key(best, best_i));
     } else if constexpr (EPI == EPI_NCE_BWD) {
       const float alpha = __ldg(p.alpha_dev);
       const float gs = __ldg(p.gscale_dev);

@@ -14,7 +14,6 @@ import torch
 
 from . import kernels as K
 from . import distributed as D_
-from .clip import Unsupported
 
 F32 = torch.float32
 
@@ -120,10 +119,6 @@ class FilipLossFn(torch.autograd.Function):
 
 
 def filip_loss(clip, zt, zi, zt_x, zi_x, ops, text_mask):
-    T, I = zt.shape[1], zi.shape[1]
-    if T % 16 or I % 16 or T > 256 or I > 256:
-        raise Unsupported(f"x_clip_b200: FILIP needs token counts that are multiples of 16 and <= 256 "
-                          f"(got {T} text, {I} image tokens)")
     extra = clip.extra_latent_projection
     return FilipLossFn.apply(zt, zi, zt_x if extra else None, zi_x if extra else None,
                              clip.temperature, tuple(ops), text_mask.contiguous(),

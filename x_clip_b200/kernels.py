@@ -473,16 +473,24 @@ def simreg_bwd(a, b, diag_offset, gscale):
 
 
 def filip_segmax(a, b, temp_exp, seg_len, col_mul, col_add):
-    """Per row of a and per seg_len-long block of rows of b: max / argmax of temp * <a_r, b_c>."""
+    """Per row of a and per seg_len-long block of rows of b: max / argmax of temp * <a_r, b_c>.
+    Multiples of 16 up to 256 tokens run xclip_filip_segmax (tiles of whole segments); every other
+    token count runs xclip_filip_segmax_any with a temporary key buffer."""
     _need(a, BF16, "a"); _need(b, BF16, "b")
     R, D = a.shape
     C = b.shape[0]
     nseg = C // seg_len
     seg_max = torch.empty((R, nseg), device=a.device, dtype=F32)
     seg_arg = torch.empty((R, nseg), device=a.device, dtype=torch.int32)
-    _call(a, "filip_segmax", 2.0 * R * C * D, 2.0 * (R + C) * D + 8.0 * R * nseg, "xclip_filip_segmax",
+    if seg_len % 16 == 0 and seg_len <= 256:
+        _call(a, "filip_segmax", 2.0 * R * C * D, 2.0 * (R + C) * D + 8.0 * R * nseg, "xclip_filip_segmax",
+              a.data_ptr(), b.data_ptr(), R, C, D, temp_exp.data_ptr(), int(seg_len), _ptr(col_mul),
+              _ptr(col_add), seg_max.data_ptr(), seg_arg.data_ptr())
+        return seg_max, seg_arg
+    keys = torch.empty((R, nseg), device=a.device, dtype=torch.int64)
+    _call(a, "filip_segmax", 2.0 * R * C * D, 2.0 * (R + C) * D + 32.0 * R * nseg, "xclip_filip_segmax_any",
           a.data_ptr(), b.data_ptr(), R, C, D, temp_exp.data_ptr(), int(seg_len), _ptr(col_mul),
-          _ptr(col_add), seg_max.data_ptr(), seg_arg.data_ptr())
+          _ptr(col_add), seg_max.data_ptr(), seg_arg.data_ptr(), keys.data_ptr())
     return seg_max, seg_arg
 
 
@@ -520,12 +528,15 @@ def filip_nce_bwd(s, lse, diag_off, dcl, gscale, row_valid=None):
 
 def filip_expand(seg_arg, seg_max, wmat, rowscale, temp_exp, row0, rows, rows_per_sample, seg_len,
                  nseg, dtemp):
-    g = torch.empty((rows, nseg * seg_len), device=seg_arg.device, dtype=BF16)
+    """bf16 G [rows, C] (C = nseg * seg_len): a view of a [rows, roundup8(C)] buffer, so that its row
+    stride stays a multiple of 8 elements for the gradient GEMMs; see xclip_filip_expand."""
+    C = nseg * seg_len
+    g = torch.empty((rows, (C + 7) // 8 * 8), device=seg_arg.device, dtype=BF16)
     _call(seg_arg, "filip_expand", 0.0, 2.0 * g.numel(), "xclip_filip_expand", seg_arg.data_ptr(),
           seg_max.data_ptr(), wmat.data_ptr(), rowscale.data_ptr(), temp_exp.data_ptr(), int(row0),
           int(rows), int(rows_per_sample), int(seg_len), int(nseg), g.data_ptr(), g.stride(0),
           _ptr(dtemp))
-    return g
+    return g[:, :C]
 
 
 def text_embed_fwd(ids, tok, pos, cls):
