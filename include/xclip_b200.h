@@ -184,14 +184,13 @@ int xclip_simreg_bwd(const void* a, const void* b, int R, int C, int K, int diag
                      const float* gscale, void* g, int64_t ldg, xclip_stream_t stream);
 
 /* ---- FILIP fine-grained loss (x_clip/x_clip.py:799-811 + :821-847) -----------------------
- * segmax : a bf16 [R,D] token latents of one modality, b bf16 [C,D] token latents of the other,
- *          C = n_samples * seg_len (seg_len tokens per sample, multiple of 16, <= 256).  For
- *          every row r and sample y: seg_max[r,y] = max_i s, seg_arg[r,y] = argmax_i s with
+ * segmax_any : a bf16 [R,D] token latents of one modality, b bf16 [C,D] token latents of the
+ *          other, C = n_samples * seg_len (seg_len >= 1 tokens per sample).  For every row r and
+ *          sample y: seg_max[r,y] = max_i s, seg_arg[r,y] = argmax_i s with
  *          s = *temp_exp * <a_r, b_(y,i)> (optionally s*col_mul[c] + col_add[c]: padded text
  *          tokens get col_mul 0 / col_add -FLT_MAX, the reference's masked_fill at :810).
  *          Ties go to the lowest index; a segment whose columns are all masked gives -FLT_MAX at
  *          index 0.
- * segmax_any : segmax for any seg_len >= 1 (C % seg_len == 0), same values, ties and masks.
  *          keys: caller-owned workspace of 8 * R * (C / seg_len) bytes, 8-byte aligned, no
  *          initialisation needed (the call zeroes it; it holds nothing of use afterwards).  a, b
  *          16-byte aligned; temp_exp, seg_max, seg_arg, col_mul, col_add 4-byte aligned.
@@ -212,9 +211,6 @@ int xclip_simreg_bwd(const void* a, const void* b, int R, int C, int K, int diag
  *          with ldg % 8 == 0 and ldg >= nseg * seg_len, 16-byte aligned.  Columns
  *          [nseg * seg_len, roundup8(nseg * seg_len)) are written as zeros, the rest of the row is
  *          left alone; the gradient GEMMs take G[:, :nseg * seg_len] and never read past it. */
-int xclip_filip_segmax(const void* a, const void* b, int R, int C, int D, const float* temp_exp,
-                       int seg_len, const float* col_mul, const float* col_add, float* seg_max,
-                       int* seg_arg, xclip_stream_t stream);
 int xclip_filip_segmax_any(const void* a, const void* b, int R, int C, int D,
                            const float* temp_exp, int seg_len, const float* col_mul,
                            const float* col_add, float* seg_max, int* seg_arg, void* keys,

@@ -21,7 +21,7 @@ sys.path.insert(0, str(Path(__file__).resolve().parent))
 import make_golden as M  # noqa: E402
 
 # 48 text tokens, 192 px / patch 16 -> 144 image tokens: the segment-max GEMMs run with seg_len 144
-# (tile stride 144) over the image tokens and seg_len 48 (tile stride 240) over the text tokens
+# over the image tokens and seg_len 48 over the text tokens, neither a divisor of the 256-column tile
 FILIP_T48_I144 = dict(M.TINY, text_seq_len=48, visual_image_size=192, use_all_token_embeds=True)
 
 CASES = {

@@ -1,6 +1,7 @@
 """FILIP models at token counts other than 16, 32, 64 and 256: 48 text tokens against 144 image tokens
-(192 px / patch 16), so the segment-max GEMMs run with seg_len 144 (tile stride 144) and seg_len 48
-(tile stride 240, segments restarting inside a 128-column staging pass).  Goldens:
+(192 px / patch 16), so the segment-max GEMMs run with seg_len 144 and seg_len 48: neither divides
+the 256-column tile, so segments are cut by tile edges and restart inside a 128-column staging pass.
+Goldens:
 tests/golden/{filip_t48_i144, filip_t48_i144_dcl_extra}.json, written by
 tests/golden/make_golden_filip.py."""
 import json

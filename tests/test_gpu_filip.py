@@ -65,7 +65,7 @@ SEGMAX_GATE = 2.0 ** -16
 
 
 def _run_segmax(za, zb, temp, seg_len, col_mul=None, col_add=None):
-    """xclip_filip_segmax on the split operands of za [R, D] x zb [C, D], checked against fp64:
+    """kernels.filip_segmax on the split operands of za [R, D] x zb [C, D], checked against fp64:
     seg_max elementwise, seg_arg by value (the fp64 similarity at the returned column must be within
     the gate of the fp64 maximum: near-ties may legitimately pick the other index).
     Returns (seg_max, seg_arg, max value error / gate, max arg error / gate)."""
@@ -98,7 +98,8 @@ def _run_segmax(za, zb, temp, seg_len, col_mul=None, col_add=None):
 
 
 def _nseg_for(seg_len):
-    """Segments that fill three output tiles and spill one segment into a fourth (partial) tile."""
+    """3 * (256 // seg_len) + 1 segments: two to four 256-column output tiles, most of them ending in
+    a partial one.  Lengths that do not divide 256 have segments cut by a tile edge."""
     return 3 * (256 // seg_len) + 1
 
 
@@ -108,8 +109,8 @@ SEG_LENS = list(range(16, 257, 16))
 @pytest.mark.parametrize("D", [256, 512, 72])          # K = 3D = 216: not a multiple of the 64-wide k-block
 @pytest.mark.parametrize("seg_len", SEG_LENS)
 def test_segmax_matches_fp64(cuda_device, seg_len, D):
-    """Every token count from 16 to 256: tile strides (256 / seg_len) * seg_len of 256, 240, 224, 144...,
-    segments that restart inside a 128-column staging pass, several tiles ending in a partial one.
+    """Every token count from 16 to 256: segments wholly inside a tile where seg_len divides 256, cut by
+    a tile edge elsewhere (48, 80, 144...), segments that restart inside a 128-column staging pass.
     R = 1 / 127 / 129 / 1100: ragged last row tile; 129 < C (m-fastest raster), 1100 > C (n-fastest)."""
     gen = _gen(cuda_device, 1000 * seg_len + D)
     C = _nseg_for(seg_len) * seg_len

@@ -1,5 +1,5 @@
-"""FILIP at any token count: xclip_filip_segmax_any (the EPI_SEGMAX_ANY epilogue: 256-column tiles
-whatever the segment length, segments cut by a tile edge merged through 64-bit keys), filip_expand
+"""FILIP at any token count: the segment max at lengths that are not multiples of 16 or exceed a
+256-column tile (segments cut by one or more tile edges, merged through 64-bit keys), filip_expand
 at segment lengths that are not multiples of 8, and FilipLossFn at cfg3's 77 x 98 / 77 x 196, at
 300 x 576 and at 7 x 9 tokens, against the fp64 references and gates of test_gpu_filip."""
 import math
@@ -8,8 +8,8 @@ import pytest
 import torch
 
 from test_gpu_filip import (_check_expand, _col_mask_tables, _compare_filip, _filip_inputs,
-                            _gen, _nseg_for, _oracle_filip, _report_peak, _run_filip_loss,
-                            _run_segmax, _split, _start_peak, _unit, oracle_filip_chunked)
+                            _gen, _oracle_filip, _report_peak, _run_filip_loss, _run_segmax,
+                            _start_peak, _unit, oracle_filip_chunked)
 
 pytestmark = pytest.mark.gpu
 
@@ -26,22 +26,6 @@ def _nseg_any(seg_len):
     if (nseg * seg_len) % TILE == 0:
         nseg += 1
     return nseg
-
-
-def _segmax_any(a, b, temp, seg_len, col_mul=None, col_add=None):
-    """xclip_filip_segmax_any called directly (kernels.filip_segmax routes multiples of 16 <= 256 to
-    xclip_filip_segmax)."""
-    from x_clip_b200 import kernels as K
-    R, D = a.shape
-    C = b.shape[0]
-    nseg = C // seg_len
-    seg_max = torch.empty((R, nseg), device=a.device, dtype=F32)
-    seg_arg = torch.empty((R, nseg), device=a.device, dtype=torch.int32)
-    keys = torch.empty((R, nseg), device=a.device, dtype=torch.int64)
-    K._call(a, "filip_segmax", 0.0, 0.0, "xclip_filip_segmax_any", a.data_ptr(), b.data_ptr(), R, C, D,
-            temp.data_ptr(), int(seg_len), K._ptr(col_mul), K._ptr(col_add), seg_max.data_ptr(),
-            seg_arg.data_ptr(), keys.data_ptr())
-    return seg_max, seg_arg
 
 
 def _edges_crossed(seg_len, nseg):
@@ -143,31 +127,6 @@ def test_segmax_any_ties_across_a_tile_edge_go_to_the_lowest_index(cuda_device, 
     assert crossing > 0
     _, arg, _, _ = _run_segmax(za, zb.reshape(-1, D), 100.0, seg_len)
     assert torch.equal(arg.long().cpu(), p[None, :].expand(R, nseg))
-
-
-@pytest.mark.parametrize("masked", [False, True])
-@pytest.mark.parametrize("seg_len", list(range(16, 257, 16)))
-def test_segmax_any_equals_the_specialised_path(cuda_device, seg_len, masked):
-    """At the token counts xclip_filip_segmax covers, xclip_filip_segmax_any gives bit-identical seg_max
-    and seg_arg: every output element sees the same k-order in both kernels, and the values and the
-    strict '>' scan are the same."""
-    from x_clip_b200 import kernels as K
-    gen = _gen(cuda_device, 77 + seg_len)
-    D, nseg = 256, _nseg_for(seg_len)
-    C = nseg * seg_len
-    zb = _unit((C, D), gen, cuda_device)
-    col_mul = col_add = None
-    if masked:
-        mask = torch.rand((nseg, seg_len), generator=gen, device=cuda_device) < 0.5
-        mask[0] = False
-        col_mul, col_add = _col_mask_tables(mask)
-    _, b_col = _split(zb)
-    t = torch.tensor([100.0], device=cuda_device, dtype=F32)
-    for R in (129, 1100):
-        a_row, _ = _split(_unit((R, D), gen, cuda_device))
-        m0, a0 = K.filip_segmax(a_row, b_col, t, seg_len, col_mul, col_add)
-        m1, a1 = _segmax_any(a_row, b_col, t, seg_len, col_mul, col_add)
-        assert torch.equal(m0, m1) and torch.equal(a0, a1), (seg_len, R, masked)
 
 
 # --------------------------------------------------------------------------- expand

@@ -5,10 +5,8 @@ project's towers.
 
 (1) Segment-max passes, D = 512 (K = 3 D = 1536), local batch 256: for T text tokens against I
     image tokens, pass A is (256 T) rows x (256 I) columns in segments of I, pass B (256 I) x (256 T)
-    in segments of T.  Algorithmic TFLOP/s = 2 R C 3D / time.  At the counts xclip_filip_segmax
-    covers (cfg4: 256 x 64 / 32; 48 x 144) both entries run, alternated in one window each, so the two
-    paths are compared under the same conditions.  Also one rank's pass A at an 8-GPU cfg3 batch
-    (256 x 77 rows against 2048 x 98 columns).
+    in segments of T.  Algorithmic TFLOP/s = 2 R C 3D / time.  Also one rank's pass A at an 8-GPU
+    cfg3 batch (256 x 77 rows against 2048 x 98 columns).
 (2) FilipLossFn forward + backward at the same (T, I), batch 256, no encoder.
 (3) The cfg3 step of bench.py with FILIP against the same step with InfoNCE (256 pairs, patch
     dropout 0.5): FILIP's share of the step.
@@ -61,33 +59,14 @@ def _unit(shape, dev):
     return torch.nn.functional.normalize(torch.randn(shape, device=dev), dim=-1)
 
 
-def segmax_pass(R, C, seg_len, D, dev, reps, both):
+def segmax_pass(R, C, seg_len, D, dev, reps):
     from x_clip_b200 import kernels as K
     a, _ = _split(_unit((R, D), dev))
     _, b = _split(_unit((C, D), dev))
     t = torch.tensor([100.0], device=dev, dtype=F32)
-    nseg = C // seg_len
-    m = torch.empty((R, nseg), device=dev, dtype=F32)
-    arg = torch.empty((R, nseg), device=dev, dtype=torch.int32)
-    keys = torch.empty((R, nseg), device=dev, dtype=torch.int64)
-
-    def any_path():
-        K._call(a, "filip_segmax", 0.0, 0.0, "xclip_filip_segmax_any", a.data_ptr(), b.data_ptr(), R, C, 3 * D,
-                t.data_ptr(), seg_len, None, None, m.data_ptr(), arg.data_ptr(), keys.data_ptr())
-
-    def specialised():
-        K._call(a, "filip_segmax", 0.0, 0.0, "xclip_filip_segmax", a.data_ptr(), b.data_ptr(), R, C, 3 * D,
-                t.data_ptr(), seg_len, None, None, m.data_ptr(), arg.data_ptr())
-
+    (ms,) = _time([lambda: K.filip_segmax(a, b, t, seg_len, None, None)], reps)
     fl = 2.0 * R * C * 3 * D
-    out = dict(R=R, C=C, seg_len=seg_len)
-    if both:
-        ms_s, ms_a = _time([specialised, any_path], reps)
-        out.update(segmax_ms=round(ms_s, 3), segmax_tflops=round(fl / ms_s / 1e9, 1))
-    else:
-        (ms_a,) = _time([any_path], reps)
-    out.update(segmax_any_ms=round(ms_a, 3), segmax_any_tflops=round(fl / ms_a / 1e9, 1))
-    return out
+    return dict(R=R, C=C, seg_len=seg_len, segmax_ms=round(ms, 3), segmax_tflops=round(fl / ms / 1e9, 1))
 
 
 def loss_fn(B, T, I, D, dev, reps):
@@ -130,15 +109,15 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("filip_bench needs a GPU")
     D, b = 512, 256
-    shapes = [(256, 64, True), (256, 32, True), (48, 144, True), (77, 98, False), (77, 196, False), (77, 576, False)]
+    shapes = [(256, 64), (256, 32), (48, 144), (77, 98), (77, 196), (77, 576)]
     res = dict(card=_card(dev), segmax=[], loss_fn=[])
-    for T, I, both in shapes:
-        res["segmax"].append(dict(pass_="A", **segmax_pass(b * T, b * I, I, D, dev, args.reps, both)))
-        res["segmax"].append(dict(pass_="B", **segmax_pass(b * I, b * T, T, D, dev, args.reps, both)))
+    for T, I in shapes:
+        res["segmax"].append(dict(pass_="A", **segmax_pass(b * T, b * I, I, D, dev, args.reps)))
+        res["segmax"].append(dict(pass_="B", **segmax_pass(b * I, b * T, T, D, dev, args.reps)))
         torch.cuda.empty_cache()
     res["segmax"].append(dict(pass_="A, one rank of 8 (B_g 2048)",
-                              **segmax_pass(b * 77, 2048 * 98, 98, D, dev, args.reps, False)))
-    for T, I, _ in shapes:
+                              **segmax_pass(b * 77, 2048 * 98, 98, D, dev, args.reps)))
+    for T, I in shapes:
         torch.cuda.reset_peak_memory_stats(dev)
         res["loss_fn"].append(loss_fn(b, T, I, D, dev, max(3, args.reps // 4)))
         torch.cuda.empty_cache()

@@ -86,8 +86,6 @@ SIGNATURES = {
                                  c_float, c_float, c_int, c_float, c_void_p]),
     "xclip_rotary_inplace": (c_int, [c_void_p, c_int64, c_int64, c_int, c_int, c_void_p, c_void_p, c_int,
                                      c_void_p]),
-    "xclip_filip_segmax": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int,
-                                   c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "xclip_filip_segmax_any": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int,
                                        c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "xclip_filip_reduce": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int,

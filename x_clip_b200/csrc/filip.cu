@@ -6,11 +6,10 @@
 //              [text,image] orientation for i2t as well)
 //
 // The 6-D similarity tensor (68.7 G elements at cfg4) is never materialised:
-//   xclip_filip_segmax : the wgmma GEMM with the EPI_SEGMAX epilogue produces, per token row and
-//                        per sample of the other modality, max + argmax over that sample's tokens
-//                        (multiples of 16 tokens, <= 256: tiles hold whole samples)
-//   xclip_filip_segmax_any : the same for any token count (EPI_SEGMAX_ANY: 256-column tiles,
-//                        samples cut by a tile edge merged through 64-bit keys, then unpacked)
+//   xclip_filip_segmax_any : the wgmma GEMM with the EPI_SEGMAX epilogue produces, per token row
+//                        and per sample of the other modality, max + argmax over that sample's
+//                        tokens, for any token count (256-column tiles, samples cut by a tile
+//                        edge merged through 64-bit keys, then unpacked)
 //   xclip_filip_reduce : [tokens, B] maxima -> [B, B] similarity (masked mean / mean)
 //   xclip_filip_nce_*  : row-wise InfoNCE / DCL on a [B,B] fp32 matrix (warp-shuffle reductions)
 //   xclip_filip_expand : backward: one-hot (at the argmax) weighted bf16 operand G[rows, cols]
@@ -179,7 +178,7 @@ filip_expand_any_kernel(const int* __restrict__ seg_arg, const float* __restrict
   }
 }
 
-// keys of EPI_SEGMAX_ANY -> seg_max (f32) and seg_arg (int32)
+// keys of EPI_SEGMAX -> seg_max (f32) and seg_arg (int32)
 __global__ void __launch_bounds__(256)
 filip_unpack_keys_kernel(const unsigned long long* __restrict__ keys, long long n,
                          float* __restrict__ seg_max, int* __restrict__ seg_arg) {
@@ -194,47 +193,6 @@ filip_unpack_keys_kernel(const unsigned long long* __restrict__ keys, long long 
 }  // namespace xclip
 
 using namespace xclip;
-
-extern "C" int xclip_filip_segmax(const void* a, const void* b, int R, int C, int D,
-                                  const float* temp_exp, int seg_len, const float* col_mul,
-                                  const float* col_add, float* seg_max, int* seg_arg,
-                                  xclip_stream_t stream) {
-  int rc = xclip_init();
-  if (rc) return rc;
-  XCLIP_REQUIRE(a && b && temp_exp && seg_max && seg_arg, "filip_segmax: null pointer");
-  XCLIP_REQUIRE(R > 0 && C > 0 && D > 0 && D % 8 == 0, "filip_segmax: bad sizes");
-  XCLIP_REQUIRE(seg_len % 16 == 0 && seg_len <= 256 && C % seg_len == 0,
-                "filip_segmax: tokens per sample (%d) must be a multiple of 16, <= 256", seg_len);
-  XCLIP_REQUIRE((col_mul == nullptr) == (col_add == nullptr), "filip_segmax: mask tables mismatch");
-  XCLIP_REQUIRE(((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b)) & 15) == 0,
-                "filip_segmax: misaligned latents");
-  CUtensorMap tmA, tmB;
-  rc = encode_2d_bf16(&tmA, a, (uint64_t)D, (uint64_t)R, (uint64_t)D, 64, kGemmBlockM);
-  if (rc) return rc;
-  rc = encode_2d_bf16(&tmB, b, (uint64_t)D, (uint64_t)C, (uint64_t)D, 64, 256);
-  if (rc) return rc;
-  GemmParams p = {};
-  p.M = R; p.N = C; p.K = D; p.split_k = 1;
-  p.raster_m_fast = (R <= C) ? 1 : 0;
-  p.alpha_dev = temp_exp;
-  p.seg_len = seg_len;
-  p.n_tile_stride = (256 / seg_len) * seg_len;
-  p.n_segs = C / seg_len;
-  p.col_mul = col_mul; p.col_add = col_add;
-  p.seg_max = seg_max; p.seg_arg = seg_arg;
-  const long long tiles = (long long)((R + kGemmBlockM - 1) / kGemmBlockM) *
-                          ((C + p.n_tile_stride - 1) / p.n_tile_stride);
-  const int grid = (int)(tiles < num_sms() ? tiles : num_sms());
-  using S = GemmSmem<256>;
-  auto kern = gemm_bf16_kernel<256, kMajorK, kMajorK, EPI_SEGMAX>;
-  {
-    const int rc_attr = ensure_dynamic_smem(reinterpret_cast<const void*>(kern), S::kTotal);
-    if (rc_attr) return rc_attr;
-  }
-  kern<<<grid, kGemmThreads, S::kTotal, reinterpret_cast<cudaStream_t>(stream)>>>(tmA, tmB, p);
-  XCLIP_LAUNCH_CHECK("gemm_bf16_kernel<segmax>");
-  return XCLIP_OK;
-}
 
 extern "C" int xclip_filip_segmax_any(const void* a, const void* b, int R, int C, int D,
                                       const float* temp_exp, int seg_len, const float* col_mul,
@@ -273,7 +231,7 @@ extern "C" int xclip_filip_segmax_any(const void* a, const void* b, int R, int C
   const long long tiles = (long long)((R + kGemmBlockM - 1) / kGemmBlockM) * ((C + 255) / 256);
   const int grid = (int)(tiles < num_sms() ? tiles : num_sms());
   using S = GemmSmem<256>;
-  auto kern = gemm_bf16_kernel<256, kMajorK, kMajorK, EPI_SEGMAX_ANY>;
+  auto kern = gemm_bf16_kernel<256, kMajorK, kMajorK, EPI_SEGMAX>;
   {
     const int rc_attr = ensure_dynamic_smem(reinterpret_cast<const void*>(kern), S::kTotal);
     if (rc_attr) return rc_attr;
@@ -281,7 +239,7 @@ extern "C" int xclip_filip_segmax_any(const void* a, const void* b, int R, int C
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   XCLIP_CUDA(cudaMemsetAsync(keys, 0, (size_t)nkeys * 8, st));
   kern<<<grid, kGemmThreads, S::kTotal, st>>>(tmA, tmB, p);
-  XCLIP_LAUNCH_CHECK("gemm_bf16_kernel<segmax_any>");
+  XCLIP_LAUNCH_CHECK("gemm_bf16_kernel<segmax>");
   long long blocks = (nkeys + 255) / 256;
   if (blocks > (long long)num_sms() * 16) blocks = (long long)num_sms() * 16;
   filip_unpack_keys_kernel<<<(int)blocks, 256, 0, st>>>(

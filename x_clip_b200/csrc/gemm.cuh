@@ -70,13 +70,12 @@ struct GemmParams {
   const float* alpha_dev;  // NCE: exp(temperature) read from device memory (no host sync)
   const float* gscale_dev; // BWD: upstream scalar gradient / (2*B_global), multiplies the weights
   // ---- FILIP segment-max epilogue (EPI_SEGMAX): columns are grouped in segments of seg_len
-  // tokens (one segment = one sample of the other modality); n_tile_stride = columns a tile
-  // advances by (a whole number of segments, <= BLOCK_N)
-  int seg_len, n_tile_stride, n_segs;
+  // tokens (one segment = one sample of the other modality); the result goes to one packed key
+  // per (row, segment) (segmax_key), zeroed before the launch
+  int seg_len, n_segs;
   const float* col_mul;    // [N] or null: per-column multiplier (0 for masked text tokens)
   const float* col_add;    // [N] or null: per-column addend (-FLT_MAX for masked text tokens)
-  float* seg_max;          // [M, n_segs]  max_i s
-  int* seg_arg;            // [M, n_segs]  argmax (index inside the segment)
+  unsigned long long* seg_keys;  // [M, n_segs]
   // ---- fused feed-forward epilogues (EPI_FF_*)
   float* ff_rowsum;        // [M, 4d/64, 2] per-box (sum, sum of squares) of the GEGLU output rows: UP writes, DOWN sums
   const float* ff_colvec;  // DOWN: c[N] = row sums of the gain-scaled down-projection weight
@@ -90,16 +89,16 @@ struct GemmParams {
   bf16* ff_out2;           // UP: hp [M, 4d];  DOWN: bf16(acc) [M, d]
   long long ff_ld2;
   const float* ff_ab;      // BWD: [M,2] per-row (mean_k(gdh), mean_k(gdh * hn)) from xclip_ff_bwd_prep
-  // ---- FILIP segment-max epilogue for any segment length (EPI_SEGMAX_ANY): seg_len, n_segs,
-  // col_mul and col_add as above; the result goes to one packed key per (row, segment)
-  // (segmax_key), zeroed before the launch
-  unsigned long long* seg_keys;  // [M, n_segs]
 };
 
 constexpr int EPI_STORE = 0;    // C = alpha*acc (+bias) (+residual)
 constexpr int EPI_NCE_FWD = 1;  // row partial sums of exp(s - alpha) and the positives
 constexpr int EPI_NCE_BWD = 2;  // C = g = w_row*exp(s-lse_row) + w_col*exp(s-lse_col) - w_diag*[diag]
-constexpr int EPI_SEGMAX = 3;   // per row and column segment: max and argmax of alpha*acc (FILIP)
+// FILIP: per row and column segment of seg_len >= 1 columns, max and argmax of alpha*acc
+// (BLOCK_N = 256).  A segment may start or end anywhere in a tile, and may span several tiles.
+// Each (row, segment) result is one 64-bit key (segmax_key); a segment wholly inside the tile
+// stores it, a piece cut by a tile edge merges it with atom.max.  filip.cu unpacks the keys.
+constexpr int EPI_SEGMAX = 3;
 // Fused feed-forward (x_clip/x_clip.py:180-199), BLOCK_N = 128:
 //   EPI_FF_UP   B is the up-projection weight with its rows permuted so that a tile holds the value
 //               columns [64 t, 64 t + 64) and the MATCHING gate columns; writes u = [value | gate]
@@ -125,11 +124,6 @@ constexpr int EPI_FF_BWD = 6;
 //   EPI_SIMREG_BWD  C = bf16(*gscale_dev * E), zero on the excluded columns up to ldc
 constexpr int EPI_SIMREG_FWD = 7;
 constexpr int EPI_SIMREG_BWD = 8;
-// FILIP segment max for any seg_len >= 1 (BLOCK_N = 256).  Tiles advance by 256 columns whatever
-// seg_len is, so a segment may start or end anywhere in a tile, and may span several tiles.  Each
-// (row, segment) result is one 64-bit key (segmax_key); a segment wholly inside the tile stores it,
-// a piece cut by a tile edge merges it with atom.max.  filip.cu unpacks the keys afterwards.
-constexpr int EPI_SEGMAX_ANY = 9;
 
 constexpr int kGemmBlockM = 128;
 constexpr int kGemmBlockK = 64;
@@ -321,8 +315,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const int lane = threadIdx.x & 31;
 
   const int num_m = (p.M + kGemmBlockM - 1) / kGemmBlockM;
-  const int n_stride = (EPI == EPI_SEGMAX) ? p.n_tile_stride : BLOCK_N;
-  const int num_n = (p.N + n_stride - 1) / n_stride;
+  const int num_n = (p.N + BLOCK_N - 1) / BLOCK_N;
   const int num_kb = (p.K + kGemmBlockK - 1) / kGemmBlockK;
   const int splits = p.split_k > 0 ? p.split_k : 1;
   const int kb_per_split = (num_kb + splits - 1) / splits;
@@ -368,12 +361,12 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                           m_blk * kGemmBlockM + g * 64, kb * kGemmBlockK);
           }
           if (B_MAJOR == kMajorK) {
-            tma_load_2d(sb, &tmB, &full_bar[stage], kb * kGemmBlockK, n_blk * n_stride);
+            tma_load_2d(sb, &tmB, &full_bar[stage], kb * kGemmBlockK, n_blk * BLOCK_N);
           } else {
 #pragma unroll
             for (int g = 0; g < BLOCK_N / 64; ++g)
               tma_load_2d(sb + g * (kGemmBlockK * 128), &tmB, &full_bar[stage],
-                          n_blk * n_stride + g * 64, kb * kGemmBlockK);
+                          n_blk * BLOCK_N + g * 64, kb * kGemmBlockK);
           }
           if (++stage == kStages) { stage = 0; phase ^= 1; }
         }
@@ -546,35 +539,9 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         *dst = make_float2(run_m, run_s);
       }
     } else if constexpr (EPI == EPI_SEGMAX) {
-      const float alpha = __ldg(p.alpha_dev);
-      const int col_base = n_blk * n_stride;
-      const int valid = min(n_stride, p.N - col_base);        // multiple of seg_len (and of 16)
-      float best = -INFINITY;
-      int best_i = 0;
-#pragma unroll 1
-      for (int c0 = 0; c0 < valid; c0 += 16) {
-        need(c0);
-        float v[16];
-        acc_ld16(acc_row, acc_sw, c0, v);
-        const int in_seg = c0 % p.seg_len;
-        if (in_seg == 0) { best = -INFINITY; best_i = 0; }
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          float sv = v[i] * alpha;
-          if (p.col_mul != nullptr)
-            sv = fmaf(v[i] * alpha, p.col_mul[col_base + c0 + i], p.col_add[col_base + c0 + i]);
-          if (sv > best) { best = sv; best_i = in_seg + i; }
-        }
-        if (in_seg + 16 == p.seg_len && row_ok) {
-          const long long o = (long long)row * p.n_segs + (col_base + c0) / p.seg_len;
-          p.seg_max[o] = best;
-          p.seg_arg[o] = best_i;
-        }
-      }
-    } else if constexpr (EPI == EPI_SEGMAX_ANY) {
       // (segment, position) of the tile's first column from one division, then stepped per column;
       // the column walk is the same for every thread of the CTA, so its branches do not diverge.
-      // Values and the strict '>' scan are those of EPI_SEGMAX.
+      // A strict '>' scan: ties go to the lowest index.
       const float alpha = __ldg(p.alpha_dev);
       const int L = p.seg_len;
       const int col_base = n_blk * BLOCK_N;

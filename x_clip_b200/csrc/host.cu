@@ -150,7 +150,7 @@ int xclip_tune_set(int knob, int value) {
   return prev;
 }
 
-int xclip_abi_version(void) { return 1; }
+int xclip_abi_version(void) { return 2; }
 
 const char* xclip_last_error(void) { return xclip::g_err; }
 

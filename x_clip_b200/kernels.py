@@ -473,20 +473,14 @@ def simreg_bwd(a, b, diag_offset, gscale):
 
 
 def filip_segmax(a, b, temp_exp, seg_len, col_mul, col_add):
-    """Per row of a and per seg_len-long block of rows of b: max / argmax of temp * <a_r, b_c>.
-    Multiples of 16 up to 256 tokens run xclip_filip_segmax (tiles of whole segments); every other
-    token count runs xclip_filip_segmax_any with a temporary key buffer."""
+    """Per row of a and per seg_len-long block of rows of b: max / argmax of temp * <a_r, b_c>, for
+    any seg_len >= 1.  xclip_filip_segmax_any needs a temporary key buffer of 8 bytes per result."""
     _need(a, BF16, "a"); _need(b, BF16, "b")
     R, D = a.shape
     C = b.shape[0]
     nseg = C // seg_len
     seg_max = torch.empty((R, nseg), device=a.device, dtype=F32)
     seg_arg = torch.empty((R, nseg), device=a.device, dtype=torch.int32)
-    if seg_len % 16 == 0 and seg_len <= 256:
-        _call(a, "filip_segmax", 2.0 * R * C * D, 2.0 * (R + C) * D + 8.0 * R * nseg, "xclip_filip_segmax",
-              a.data_ptr(), b.data_ptr(), R, C, D, temp_exp.data_ptr(), int(seg_len), _ptr(col_mul),
-              _ptr(col_add), seg_max.data_ptr(), seg_arg.data_ptr())
-        return seg_max, seg_arg
     keys = torch.empty((R, nseg), device=a.device, dtype=torch.int64)
     _call(a, "filip_segmax", 2.0 * R * C * D, 2.0 * (R + C) * D + 32.0 * R * nseg, "xclip_filip_segmax_any",
           a.data_ptr(), b.data_ptr(), R, C, D, temp_exp.data_ptr(), int(seg_len), _ptr(col_mul),
