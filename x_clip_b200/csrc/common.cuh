@@ -150,6 +150,23 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
       : "memory");
 }
 
+// shared -> global box store; completion is tracked per issuing thread by bulk groups
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* smem_src, int32_t c0, int32_t c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
+                   reinterpret_cast<uint64_t>(m)),
+               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// the issuing thread's bulk groups beyond the newest N have finished reading shared memory
+template <int N>
+__device__ __forceinline__ void bulk_wait_group_read() {
+  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
+// ... and their writes to global memory are complete
+template <int N>
+__device__ __forceinline__ void bulk_wait_group() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+
 // pull a tensor box towards L2 (no shared memory, no barrier): the later tma_load of the same box
 // then sees L2 instead of HBM latency
 __device__ __forceinline__ void tma_prefetch_l2_3d(const CUtensorMap* m, int32_t c0, int32_t c1, int32_t c2) {

@@ -68,15 +68,17 @@ ff_scale_cast_kernel(const float* __restrict__ w2, const float* __restrict__ g, 
   }
 }
 
+// tmU / tmOut: the activation maps of EPI_FF_UP / EPI_FF_BWD (see gemm_bf16_kernel)
 template <int EPI, int B_MAJOR = kMajorK>
-static int launch_ff(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, cudaStream_t stream) {
-  using S = GemmSmem<128>;
+static int launch_ff(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, const CUtensorMap& tmU,
+                     const CUtensorMap& tmOut, cudaStream_t stream) {
+  using S = GemmSmem<128, EPI>;
   auto kern = gemm_bf16_kernel<128, kMajorK, B_MAJOR, EPI>;
   const int rc = ensure_dynamic_smem(reinterpret_cast<const void*>(kern), S::kTotal);
   if (rc) return rc;
   const long long tiles = (long long)((p.M + kGemmBlockM - 1) / kGemmBlockM) * ((p.N + 127) / 128);
   const int grid = (int)(tiles < num_sms() ? tiles : num_sms());
-  kern<<<grid, kGemmThreads, S::kTotal, stream>>>(tmA, tmB, p);
+  kern<<<grid, kGemmThreads, S::kTotal, stream>>>(tmA, tmB, p, tmU, tmOut);
   XCLIP_LAUNCH_CHECK("gemm_bf16_kernel<ff>");
   return XCLIP_OK;
 }
@@ -129,9 +131,13 @@ extern "C" int xclip_ff_up(const void* x, int64_t ldx, const void* w1p, void* u,
   GemmParams p = {};
   p.M = M; p.N = 8 * d; p.K = d; p.split_k = 1; p.alpha = 1.f;
   p.ff_rowsum = rowsum; p.ff_hidden = 4 * d; p.ff_skip_u = skip_u ? 1 : 0;
-  p.ff_u = reinterpret_cast<bf16*>(u); p.ff_ldu = ldu;
-  p.ff_out2 = reinterpret_cast<bf16*>(hp); p.ff_ld2 = ldhp;
-  return launch_ff<EPI_FF_UP>(tmA, tmB, p, reinterpret_cast<cudaStream_t>(stream));
+  // u and hp leave in 128-row x 64-column boxes; the maps end at row M and column 8d / 4d, so TMA
+  // clips whatever of a box lies beyond them
+  CUtensorMap tmU = {}, tmHp;
+  if (!skip_u && (rc = encode_2d_bf16(&tmU, u, (uint64_t)(8 * d), (uint64_t)M, (uint64_t)ldu, 64, kGemmBlockM)))
+    return rc;
+  if ((rc = encode_2d_bf16(&tmHp, hp, (uint64_t)(4 * d), (uint64_t)M, (uint64_t)ldhp, 64, kGemmBlockM))) return rc;
+  return launch_ff<EPI_FF_UP>(tmA, tmB, p, tmU, tmHp, reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int xclip_ff_down(const void* hp, int64_t ldhp, const void* w2g, const float* colvec,
@@ -159,7 +165,7 @@ extern "C" int xclip_ff_down(const void* hp, int64_t ldhp, const void* w2g, cons
   p.ff_rowsum = const_cast<float*>(rowsum); p.ff_colvec = colvec; p.ff_stats = stats;
   p.ff_eps = eps; p.ff_hidden = 4 * d; p.ff_inv_hidden = 1.f / (float)(4 * d);
   p.ff_out2 = reinterpret_cast<bf16*>(acc_out); p.ff_ld2 = ldacc;
-  return launch_ff<EPI_FF_DOWN>(tmA, tmB, p, reinterpret_cast<cudaStream_t>(stream));
+  return launch_ff<EPI_FF_DOWN>(tmA, tmB, p, CUtensorMap{}, CUtensorMap{}, reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int xclip_ff_bwd(const void* dx, int64_t lddx, const void* w2g, const void* u, int64_t ldu,
@@ -180,8 +186,10 @@ extern "C" int xclip_ff_bwd(const void* dx, int64_t lddx, const void* w2g, const
   if ((rc = encode_2d_bf16(&tmB, w2g, (uint64_t)(4 * d), (uint64_t)d, (uint64_t)(4 * d), 64, kGemmBlockK))) return rc;
   GemmParams p = {};
   p.M = M; p.N = 4 * d; p.K = d; p.split_k = 1; p.alpha = 1.f;
-  p.c = du; p.ldc = lddu;
   p.ff_stats = const_cast<float*>(stats); p.ff_ab = ab; p.ff_hidden = 4 * d;
-  p.ff_u = const_cast<bf16*>(reinterpret_cast<const bf16*>(u)); p.ff_ldu = ldu;
-  return launch_ff<EPI_FF_BWD, kMajorMN>(tmA, tmB, p, reinterpret_cast<cudaStream_t>(stream));
+  // u is loaded and du stored in 128-row x 64-column boxes: rows >= M load as zeros and are not stored
+  CUtensorMap tmU, tmDu;
+  if ((rc = encode_2d_bf16(&tmU, u, (uint64_t)(8 * d), (uint64_t)M, (uint64_t)ldu, 64, kGemmBlockM))) return rc;
+  if ((rc = encode_2d_bf16(&tmDu, du, (uint64_t)(8 * d), (uint64_t)M, (uint64_t)lddu, 64, kGemmBlockM))) return rc;
+  return launch_ff<EPI_FF_BWD, kMajorMN>(tmA, tmB, p, tmU, tmDu, reinterpret_cast<cudaStream_t>(stream));
 }

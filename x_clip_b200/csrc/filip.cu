@@ -238,7 +238,7 @@ extern "C" int xclip_filip_segmax_any(const void* a, const void* b, int R, int C
   }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   XCLIP_CUDA(cudaMemsetAsync(keys, 0, (size_t)nkeys * 8, st));
-  kern<<<grid, kGemmThreads, S::kTotal, st>>>(tmA, tmB, p);
+  kern<<<grid, kGemmThreads, S::kTotal, st>>>(tmA, tmB, p, CUtensorMap{}, CUtensorMap{});
   XCLIP_LAUNCH_CHECK("gemm_bf16_kernel<segmax>");
   long long blocks = (nkeys + 255) / 256;
   if (blocks > (long long)num_sms() * 16) blocks = (long long)num_sms() * 16;

@@ -11,7 +11,7 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const Gem
   auto kern = gemm_bf16_kernel<BLOCK_N, A_MAJOR, B_MAJOR>;
   const int rc_attr = ensure_dynamic_smem(reinterpret_cast<const void*>(kern), S::kTotal);
   if (rc_attr) return rc_attr;
-  kern<<<grid, kGemmThreads, S::kTotal, stream>>>(tmA, tmB, p);
+  kern<<<grid, kGemmThreads, S::kTotal, stream>>>(tmA, tmB, p, CUtensorMap{}, CUtensorMap{});
   XCLIP_LAUNCH_CHECK("gemm_bf16_kernel");
   return XCLIP_OK;
 }

@@ -23,7 +23,9 @@
 // optional split-K; the producer fills the ring in tile order.  After its k-loop a warpgroup parks
 // its accumulator (fp32 registers) in a 128 x 128 staging tile in shared memory; the epilogue then
 // gives every thread one row (thread t = row t) and walks the columns, so row reductions (softmax
-// partials, segment maxima, LayerNorm sums) stay in registers.  Each warpgroup always computes a
+// partials, segment maxima, LayerNorm sums) stay in registers.  The feed-forward's elementwise UP and
+// BWD epilogues skip the staging tile: they work on the accumulator fragments and move their bf16
+// activations through a per-warpgroup shared-memory buffer by TMA.  Each warpgroup always computes a
 // 128 x 128 block (two m64n128k16 per k16 step); BLOCK_N picks the schedule at compile time:
 //   BLOCK_N = 128, ping-pong : each warpgroup owns whole tiles (the k-th tile of the CTA goes to
 //       warpgroup k & 1), has its own staging tile and runs its own epilogue, so one warpgroup's
@@ -84,9 +86,7 @@ struct GemmParams {
   float ff_inv_hidden;     // DOWN: 1 / ff_hidden, divided on the host (a device division is a call)
   int ff_hidden;           // 4*dim: LayerNorm width; column offset of the gate half inside u
   int ff_skip_u;           // UP: do not write u = [value | gate] (inference / no-grad sweeps need only hp)
-  bf16* ff_u;              // UP: [value | gate] output [M, 8d];  BWD: saved [value | gate] activations
-  long long ff_ldu;
-  bf16* ff_out2;           // UP: hp [M, 4d];  DOWN: bf16(acc) [M, d]
+  bf16* ff_out2;           // DOWN: bf16(acc) [M, d]
   long long ff_ld2;
   const float* ff_ab;      // BWD: [M,2] per-row (mean_k(gdh), mean_k(gdh * hn)) from xclip_ff_bwd_prep
 };
@@ -114,6 +114,8 @@ constexpr int EPI_SEGMAX = 3;
 //                 d value = dhp gelu(gate);  d gate = dhp value gelu'(gate)
 //               with the two row means a_r = mean_k gdh, b_r = mean_k gdh*hn supplied by
 //               xclip_ff_bwd_prep.  Reads u = [value | gate], writes du.
+// UP and BWD work on the accumulator fragments in registers and move their bf16 activations
+// through a per-warpgroup activation buffer in place of the fp32 staging tile (see GemmSmem).
 constexpr int EPI_FF_UP = 4;
 constexpr int EPI_FF_DOWN = 5;
 constexpr int EPI_FF_BWD = 6;
@@ -137,14 +139,24 @@ constexpr int kGemmConsumerRegs = 232;
 constexpr int kBarStage = 2;
 constexpr int kBarOrder = 4;
 
-template <int BLOCK_N>
+// Layout: ring stages | staging tiles | mbarriers.  For EPI_FF_UP / EPI_FF_BWD each warpgroup's
+// staging tile is instead a bf16 activation buffer of the same 64 KiB: four 128-row x 64-column
+// boxes in the 128-byte swizzle of their TMA maps (BWD: u value [128 n, +128), u gate, rewritten in
+// place as du; UP: u value, u gate, hp).  Their mbarriers act_full / act_empty[wg] follow the ring's;
+// only BWD, whose producer fills the buffer, waits on them (UP's store issuer waits for its own bulk
+// stores to have read the buffer before the warpgroup rewrites it).
+template <int BLOCK_N, int EPI = EPI_STORE>
 struct GemmSmem {
   static constexpr bool kPingPong = BLOCK_N == 128;
+  static constexpr bool kActTile = EPI == EPI_FF_UP || EPI == EPI_FF_BWD;
   static constexpr int kABytes = kGemmBlockM * kGemmBlockK * 2;  // 16 KiB
   static constexpr int kBBytes = BLOCK_N * kGemmBlockK * 2;      // 16/32 KiB
   static constexpr int kStageBytes = kABytes + kBBytes;
   static constexpr int kStages = 3;
   static constexpr int kAccBytes = kGemmBlockM * 128 * 4;        // fp32 staging tile, 128 columns
+  static constexpr int kActBoxBytes = kGemmBlockM * 64 * 2;      // one 128 x 64 bf16 box
+  static_assert(4 * kActBoxBytes == kAccBytes, "an activation buffer replaces a staging tile");
+  static_assert(!kActTile || kPingPong, "activation buffers are per ping-pong warpgroup");
   static constexpr int kAccTiles = kPingPong ? 2 : 1;            // one per warpgroup in ping-pong
   static constexpr int kBarrierBytes = 256;
   static constexpr int kTotal = kStages * kStageBytes + kAccTiles * kAccBytes + kBarrierBytes;
@@ -293,11 +305,153 @@ __device__ __forceinline__ void gemm_epilogue_store(const GemmParams& p, const f
   }
 }
 
+// ---- fused feed-forward epilogues on the accumulator fragments (ping-pong, one warpgroup) ----
+// Thread wt = 32 w + l of the warpgroup holds acc[h][j] at row 64 h + 16 w + l / 4 + 8 ((j / 2) % 2),
+// column 8 (j / 4) + 2 (l % 4) + j % 2.  A column pair is one 32-bit word of a 128 x 64 bf16
+// activation box; every fragment row of the thread has swizzle phase l / 4, so a warp's word
+// accesses hit 32 distinct banks.  ff_frag_off(h, j) = byte offset of acc[h][j]'s pair in its box
+// (column j / 4 mod 8 chunk); `frag` = (16 w + l / 4) * 128 + (l % 4) * 4, `sw` = l / 4.
+__device__ __forceinline__ uint32_t ff_frag_off(uint32_t frag, uint32_t sw, int h, int j) {
+  return frag + (h * 64 + 8 * ((j >> 1) & 1)) * 128 + ((((j >> 2) & 7) ^ sw) << 4);
+}
+
+// EPI_FF_UP.  Tile columns [0, 64) are the value and [64, 128) the gate columns of hidden units
+// [64 n_blk, +64): value column c and gate column 64 + c sit in the same thread (acc[h][j] and
+// acc[h][j + 32]).  Boxes: 0 = u value, 1 = u gate, 2 = hp; stored by TMA, rows >= M clipped.
+// `issuer` is the warpgroup's one thread that issues (and later waits on) the bulk stores.
+__device__ __forceinline__ void ff_up_epilogue(const GemmParams& p, const CUtensorMap* tm_u, const CUtensorMap* tm_out,
+                                               const float (&acc)[2][64], uint8_t* act, int wg, int wt, int m_blk,
+                                               int n_blk, bool issuer) {
+  constexpr int kBox = kGemmBlockM * 64 * 2;
+  const int lane = wt & 31;
+  const uint32_t frag = (uint32_t)((wt >> 5) * 16 + (lane >> 2)) * 128u + (lane & 3) * 4u;
+  const uint32_t sw = lane >> 2;
+  uint8_t* box_v = act;
+  uint8_t* box_g = act + kBox;
+  uint8_t* box_h = act + 2 * kBox;
+  // the previous tile's stores have read the buffer, and its rowsum reads are done
+  if (issuer) bulk_wait_group_read<0>();
+  named_bar_sync(kBarStage + wg, 128);
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int j = 0; j < 32; j += 2) {
+      const uint32_t off = ff_frag_off(frag, sw, h, j);
+      const float v0 = acc[h][j], v1 = acc[h][j + 1], g0 = acc[h][j + 32], g1 = acc[h][j + 33];
+      const GeluParts2 gp = gelu_parts2(g0, g1);
+      const f32x2 ge = f2_mul(f2_pack(g0, g1), gp.cdf);                                     // gelu(gate)
+      *reinterpret_cast<uint32_t*>(box_h + off) = f2_to_bf16x2(f2_mul(f2_pack(v0, v1), ge));  // hp
+      if (!p.ff_skip_u) {
+        *reinterpret_cast<uint32_t*>(box_v + off) = pack_bf16x2(v0, v1);
+        *reinterpret_cast<uint32_t*>(box_g + off) = pack_bf16x2(g0, g1);
+      }
+    }
+  fence_proxy_async_smem();
+  named_bar_sync(kBarStage + wg, 128);
+  const int m0 = m_blk * kGemmBlockM, hcol = n_blk * 64;
+  if (issuer) {
+    if (!p.ff_skip_u) {
+      tma_store_2d(tm_u, box_v, hcol, m0);
+      tma_store_2d(tm_u, box_g, p.ff_hidden + hcol, m0);
+    }
+    tma_store_2d(tm_out, box_h, hcol, m0);
+    bulk_commit_group();
+  }
+  // Per-row (sum, sum^2) of the bf16 hp the next GEMM reads: thread wt re-reads row wt and sums it in
+  // column order in two lanes (even / odd columns).  One slot per row and 64-column box, summed in a
+  // fixed order by the down-projection: the statistics (and the loss) are bit-reproducible.
+  f32x2 s1p = f2_splat(0.f), s2p = f2_splat(0.f);
+#pragma unroll
+  for (int q = 0; q < 8; ++q) {
+    const uint4 w4 = *reinterpret_cast<const uint4*>(box_h + swz128(wt, q));
+    const uint32_t w[4] = {w4.x, w4.y, w4.z, w4.w};
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const f32x2 hr = f2_from_bf16x2(w[k]);
+      s1p = f2_add(s1p, hr);
+      s2p = f2_fma(hr, hr, s2p);
+    }
+  }
+  const int row = m0 + wt;
+  if (row < p.M) {
+    const int nparts = p.ff_hidden >> 6;                     // 4d / 64 boxes per row
+    *reinterpret_cast<float2*>(p.ff_rowsum + 2ll * ((long long)row * nparts + n_blk)) =
+        make_float2(s1p.x + s1p.y, s2p.x + s2p.y);
+  }
+}
+
+// EPI_FF_BWD: (mean, rstd, a, b) of row r, zeros past M
+__device__ __forceinline__ float4 ff_row_stats(const GemmParams& p, int r) {
+  float2 st = make_float2(0.f, 0.f), ab = make_float2(0.f, 0.f);
+  if (r < p.M) {
+    st = *reinterpret_cast<const float2*>(p.ff_stats + 2ll * r);
+    ab = *reinterpret_cast<const float2*>(p.ff_ab + 2ll * r);
+  }
+  return make_float4(st.x, st.y, ab.x, ab.y);
+}
+
+// EPI_FF_BWD.  Tile columns = hidden units [128 n_blk, +128).  The producer has loaded u into boxes
+// 0, 1 (value) and 2, 3 (gate) and signalled act_full; du overwrites them in place and leaves by
+// TMA; act_empty hands the buffer back once the stores have read it.  The thread's four fragment
+// rows row0 + 64 h + 8 i (global row indices) are done one after the other, so that only one row's
+// statistics are in use and one more in flight: the 128 accumulators leave no room for more.
+// `rs` = ff_row_stats of row0, loaded by the caller.
+__device__ __forceinline__ void ff_bwd_epilogue(const GemmParams& p, const CUtensorMap* tm_out, const float (&acc)[2][64],
+                                                float4 rs, int row0, uint8_t* act, uint64_t* act_empty, int wg,
+                                                int wt, int m_blk, int n_blk, bool issuer) {
+  constexpr int kBox = kGemmBlockM * 64 * 2;
+  const int lane = wt & 31;
+  const uint32_t frag = (uint32_t)((wt >> 5) * 16 + (lane >> 2)) * 128u + (lane & 3) * 4u;
+  const uint32_t sw = lane >> 2;
+  float4 st = rs;
+#pragma unroll
+  for (int hi = 0; hi < 4; ++hi) {                          // row 64 h + 8 i of the fragment, hi = 2 h + i
+    const int h = hi >> 1;
+    float4 st_next = st;
+    if (hi < 3) st_next = ff_row_stats(p, row0 + 64 * ((hi + 1) >> 1) + 8 * ((hi + 1) & 1));
+#pragma unroll
+    for (int q = 0; q < 16; ++q) {                          // columns 8 q + 2 (l % 4) + {0, 1}
+      const int j = 4 * q + 2 * (hi & 1);
+      const f32x2 rstd2 = f2_splat(st.y), nmr = f2_splat(-st.x * st.y), namr = f2_splat(-st.z * st.y),
+                  nbmr = f2_splat(-st.w * st.y);
+      uint32_t* pv = reinterpret_cast<uint32_t*>(act + (j >> 5) * kBox + ff_frag_off(frag, sw, h, j));
+      uint32_t* pg = reinterpret_cast<uint32_t*>(reinterpret_cast<uint8_t*>(pv) + 2 * kBox);
+      const uint32_t wv = *pv, wgt = *pg;
+      const float g0 = __uint_as_float(wgt << 16), g1 = __uint_as_float(wgt & 0xffff0000u);
+      const f32x2 gate = f2_pack(g0, g1), val = f2_from_bf16x2(wv);
+      const GeluParts2 gp = gelu_parts2(g0, g1);
+      const f32x2 ge = f2_mul(gate, gp.cdf);                // gelu(gate)
+      const f32x2 gd = f2_fma(gate, gp.pdf, gp.cdf);        // gelu'(gate)
+      const f32x2 hn = f2_fma(f2_mul(val, ge), rstd2, nmr); // (val*ge - mean) rstd
+      f32x2 dhp = f2_fma(f2_pack(acc[h][j], acc[h][j + 1]), rstd2, namr);   // rstd (gdh - a)
+      dhp = f2_fma(hn, nbmr, dhp);                          //   - rstd b hn
+      *pv = f2_to_bf16x2(f2_mul(dhp, ge));
+      *pg = f2_to_bf16x2(f2_mul(f2_mul(dhp, val), gd));
+    }
+    st = st_next;
+  }
+  fence_proxy_async_smem();
+  named_bar_sync(kBarStage + wg, 128);
+  if (issuer) {
+    const int m0 = m_blk * kGemmBlockM, col = n_blk * 128;
+#pragma unroll
+    for (int b = 0; b < 4; ++b)
+      tma_store_2d(tm_out, act + b * kBox, (b >> 1) * p.ff_hidden + col + (b & 1) * 64, m0);
+    bulk_commit_group();
+    bulk_wait_group_read<0>();
+    mbar_arrive(act_empty);
+  }
+}
+
+// tmU / tmOut: 128-row x 64-column box maps of EPI_FF_UP (u [M, 8d] unless ff_skip_u, hp [M, 4d];
+// stores) and EPI_FF_BWD (u [M, 8d] loaded, du [M, 8d] stored).  Every other epilogue ignores them
+// (launch with empty maps); they follow p so that its parameter offsets do not depend on them.
 template <int BLOCK_N, int A_MAJOR, int B_MAJOR, int EPI = EPI_STORE>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                 const GemmParams p) {
-  using S = GemmSmem<BLOCK_N>;
+                 const GemmParams p, const __grid_constant__ CUtensorMap tmU,
+                 const __grid_constant__ CUtensorMap tmOut) {
+  using S = GemmSmem<BLOCK_N, EPI>;
   constexpr int kStages = S::kStages;
   constexpr bool kPingPong = S::kPingPong;
   constexpr int kPasses = kPingPong ? 1 : 2;   // trips of a tile through its 128-column staging tile
@@ -310,6 +464,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * S::kStageBytes + S::kAccTiles * S::kAccBytes);
   uint64_t* full_bar = bars;                    // [kStages]
   uint64_t* empty_bar = bars + kStages;         // [kStages]
+  uint64_t* act_full = bars + 2 * kStages;      // [2] activation buffers (S::kActTile)
+  uint64_t* act_empty = act_full + 2;           // [2]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -328,6 +484,12 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       // released by every warp that reads the stage: one warpgroup (ping-pong) or both
       mbar_init(&empty_bar[i], (kPingPong ? 128 : kGemmConsumerThreads) / 32);
     }
+    if constexpr (S::kActTile) {
+      for (int i = 0; i < 2; ++i) {
+        mbar_init(&act_full[i], 1);    // the producer's expect_tx
+        mbar_init(&act_empty[i], 1);   // the warpgroup's store issuer
+      }
+    }
     fence_barrier_init();
   }
   __syncthreads();
@@ -340,7 +502,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       tma_prefetch_desc(&tmB);
       int stage = 0;
       uint32_t phase = 0;
-      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+      int it = 0;                              // index of the tile among this CTA's tiles
+      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++it) {
         const int tmn = t % (num_n * num_m);
         const int n_blk = p.raster_m_fast ? tmn / num_m : tmn % num_n;
         const int m_blk = p.raster_m_fast ? tmn % num_m : tmn / num_n;
@@ -367,6 +530,20 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             for (int g = 0; g < BLOCK_N / 64; ++g)
               tma_load_2d(sb + g * (kGemmBlockK * 128), &tmB, &full_bar[stage],
                           n_blk * BLOCK_N + g * 64, kb * kGemmBlockK);
+          }
+          if constexpr (EPI == EPI_FF_BWD) {
+            // the tile's u (value and gate columns of hidden units [128 n_blk, +128)) lands in its
+            // warpgroup's activation buffer during the k-loop, once the buffer's last stores have read it
+            if (kb == kb0) {
+              const int w = it & 1;
+              mbar_wait_nocall(&act_empty[w], ((it >> 1) & 1) ^ 1);
+              mbar_arrive_expect_tx(&act_full[w], S::kAccBytes);
+              uint8_t* act = smem + kStages * S::kStageBytes + w * S::kAccBytes;
+#pragma unroll
+              for (int b = 0; b < 4; ++b)
+                tma_load_2d(act + b * S::kActBoxBytes, &tmU, &act_full[w],
+                            (b >> 1) * p.ff_hidden + n_blk * BLOCK_N + (b & 1) * 64, m_blk * kGemmBlockM);
+            }
           }
           if (++stage == kStages) { stage = 0; phase ^= 1; }
         }
@@ -446,11 +623,28 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       prev_stage = stage;
       if (++stage == kStages) { stage = 0; phase ^= 1; }
     }
+    // EPI_FF_BWD: (mean, rstd, a, b) of the thread's first fragment row, loaded while the last wgmma
+    // group runs
+    const int ff_row0 = m_blk * kGemmBlockM + (wt >> 5) * 16 + (lane >> 2);
+    float4 ff_rs;
+    if constexpr (EPI == EPI_FF_BWD) ff_rs = ff_row_stats(p, ff_row0);
     if (kPingPong && t + (int)gridDim.x < num_tiles)
       named_bar_arrive(kBarOrder + (wg ^ 1), kGemmConsumerThreads);
     wgmma_wait<0>();
     __syncwarp();
     if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+
+    if constexpr (S::kActTile) {
+      uint8_t* act = smem + kStages * S::kStageBytes + wg * S::kAccBytes;
+      const bool issuer = wt < 32 && XCLIP_ONE_LANE(lane);
+      if constexpr (EPI == EPI_FF_UP) {
+        ff_up_epilogue(p, &tmU, &tmOut, acc, act, wg, wt, m_blk, n_blk, issuer);
+      } else {
+        mbar_wait_nocall(&act_full[wg], (it >> 1) & 1);
+        ff_bwd_epilogue(p, &tmOut, acc, ff_rs, ff_row0, act, &act_empty[wg], wg, wt, m_blk, n_blk, issuer);
+      }
+      continue;
+    }
 
     // ---- accumulator -> staging tile (the warpgroup's 128 columns).  Ping-pong: one pass into the
     // warpgroup's own tile.  Cooperative: pass q holds tile columns [128 q, 128 q + 128), written by
@@ -705,45 +899,6 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         for (int i = 0; i < 32; i += 8)
           if (col0 + i < (int)p.ldc) st_bf16x8(grow + i, v + i);
       }
-    } else if constexpr (EPI == EPI_FF_UP) {
-      // tile columns [0,64) = value, [64,128) = gate of hidden units [64 n_blk, +64)
-      static_assert(BLOCK_N == 128, "the feed-forward epilogues use 128-column tiles");
-      need(0);
-      const int hcol = n_blk * 64;
-      f32x2 s1p = f2_splat(0.f), s2p = f2_splat(0.f);
-#pragma unroll 1
-      for (int c = 0; c < 64; c += 16) {
-        float vv[16], gg[16];
-        acc_ld16(acc_row, acc_sw, c, vv);
-        acc_ld16(acc_row, acc_sw, 64 + c, gg);
-        float hv[16];
-#pragma unroll
-        for (int i = 0; i < 16; i += 2) {
-          const GeluParts2 gp = gelu_parts2(gg[i], gg[i + 1]);
-          const f32x2 ge = f2_mul(f2_pack(gg[i], gg[i + 1]), gp.cdf);               // gelu(gate)
-          const uint32_t hw = f2_to_bf16x2(f2_mul(f2_pack(vv[i], vv[i + 1]), ge));   // hp, rounded to bf16
-          const f32x2 hr = f2_from_bf16x2(hw);           // statistics of what the next GEMM reads
-          s1p = f2_add(s1p, hr);
-          s2p = f2_fma(hr, hr, s2p);
-          hv[i] = hr.x; hv[i + 1] = hr.y;
-        }
-        if (row_ok) {
-          if (!p.ff_skip_u) {
-            bf16* urow = p.ff_u + (long long)row * p.ff_ldu + hcol + c;
-            st_bf16x8(urow, vv); st_bf16x8(urow + 8, vv + 8);
-            st_bf16x8(urow + p.ff_hidden, gg); st_bf16x8(urow + p.ff_hidden + 8, gg + 8);
-          }
-          bf16* hrow = p.ff_out2 + (long long)row * p.ff_ld2 + hcol + c;
-          st_bf16x8(hrow, hv); st_bf16x8(hrow + 8, hv + 8);
-        }
-      }
-      // one (sum, sum^2) slot per row and 64-column box: plain stores, summed in a fixed order by
-      // the down-projection -> the statistics (and the loss) are bit-reproducible run to run
-      if (row_ok) {
-        const int nparts = p.ff_hidden >> 6;                     // 4d / 64 boxes per row
-        *reinterpret_cast<float2*>(p.ff_rowsum + 2ll * ((long long)row * nparts + n_blk)) =
-            make_float2(s1p.x + s1p.y, s2p.x + s2p.y);
-      }
     } else if constexpr (EPI == EPI_FF_DOWN) {
       static_assert(BLOCK_N == 128, "the feed-forward epilogues use 128-column tiles");
       need(0);
@@ -788,66 +943,12 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           st_bf16x8(p.ff_out2 + (long long)row * p.ff_ld2 + col0 + i, v + i);
         }
       }
-    } else {   // EPI_FF_BWD: tile columns = hidden units [128 n_blk, +128)
-      static_assert(BLOCK_N == 128, "the feed-forward epilogues use 128-column tiles");
-      need(0);
-      float mean = 0.f, rstd = 0.f, am = 0.f, bm = 0.f;
-      if (row_ok) {
-        const float2 st = *reinterpret_cast<const float2*>(p.ff_stats + 2ll * row);
-        const float2 ab = *reinterpret_cast<const float2*>(p.ff_ab + 2ll * row);
-        mean = st.x; rstd = st.y; am = ab.x; bm = ab.y;
-      }
-      const f32x2 rstd2 = f2_splat(rstd), nmr = f2_splat(-mean * rstd), namr = f2_splat(-am * rstd),
-                  nbmr = f2_splat(-bm * rstd);
-      const bf16* urow = p.ff_u + (long long)(row_ok ? row : 0) * p.ff_ldu;
-      bf16* drow = reinterpret_cast<bf16*>(p.c) + (long long)(row_ok ? row : 0) * p.ldc;
-      // u of chunk c + 16 is loaded before chunk c is processed: one DRAM round trip in flight
-      // behind the GELU math instead of one per chunk
-      uint4 u_next[4] = {};
-      auto load_u = [&](int c) {
-        const int kq = n_blk * BLOCK_N + c;
-        u_next[0] = *reinterpret_cast<const uint4*>(urow + kq);
-        u_next[1] = *reinterpret_cast<const uint4*>(urow + kq + 8);
-        u_next[2] = *reinterpret_cast<const uint4*>(urow + p.ff_hidden + kq);
-        u_next[3] = *reinterpret_cast<const uint4*>(urow + p.ff_hidden + kq + 8);
-      };
-      if (row_ok) load_u(0);
-#pragma unroll 1
-      for (int c = 0; c < BLOCK_N; c += 16) {
-        if (!row_ok) break;
-        const int kq = n_blk * BLOCK_N + c;
-        uint4 u_cur[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) u_cur[i] = u_next[i];
-        if (c + 16 < BLOCK_N) load_u(c + 16);
-        float v[16];
-        acc_ld16(acc_row, acc_sw, c, v);
-#pragma unroll
-        for (int i = 0; i < 16; i += 8) {
-          const uint4 wv4 = u_cur[i / 8];
-          const uint4 wg4 = u_cur[2 + i / 8];
-          const uint32_t wv[4] = {wv4.x, wv4.y, wv4.z, wv4.w}, wgt[4] = {wg4.x, wg4.y, wg4.z, wg4.w};
-          uint32_t dvw[4], dgw[4];
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {                           // two columns per step
-            const float g0 = __uint_as_float(wgt[k] << 16), g1 = __uint_as_float(wgt[k] & 0xffff0000u);
-            const f32x2 gate = f2_pack(g0, g1), val = f2_from_bf16x2(wv[k]);
-            const GeluParts2 gp = gelu_parts2(g0, g1);
-            const f32x2 ge = f2_mul(gate, gp.cdf);                // gelu(gate)
-            const f32x2 gd = f2_fma(gate, gp.pdf, gp.cdf);        // gelu'(gate)
-            const f32x2 hn = f2_fma(f2_mul(val, ge), rstd2, nmr); // (val*ge - mean) rstd
-            f32x2 dhp = f2_fma(f2_pack(v[i + 2 * k], v[i + 2 * k + 1]), rstd2, namr);   // rstd (gdh - a)
-            dhp = f2_fma(hn, nbmr, dhp);                          //   - rstd b hn
-            dvw[k] = f2_to_bf16x2(f2_mul(dhp, ge));
-            dgw[k] = f2_to_bf16x2(f2_mul(f2_mul(dhp, val), gd));
-          }
-          *reinterpret_cast<uint4*>(drow + kq + i) = make_uint4(dvw[0], dvw[1], dvw[2], dvw[3]);
-          *reinterpret_cast<uint4*>(drow + p.ff_hidden + kq + i) = make_uint4(dgw[0], dgw[1], dgw[2], dgw[3]);
-        }
-      }
     }
     if constexpr (!kPingPong)
       while (staged < kPasses) stage_pass(false);      // keep the staging handshake in lock-step
+  }
+  if constexpr (S::kActTile) {
+    if (wt < 32 && XCLIP_ONE_LANE(lane)) bulk_wait_group<0>();   // the last tile's stores
   }
 }
 

@@ -67,7 +67,7 @@ static int launch_simreg(const CUtensorMap& tmA, const CUtensorMap& tmB, const G
     const int rc_attr = ensure_dynamic_smem(reinterpret_cast<const void*>(kern), S::kTotal);
     if (rc_attr) return rc_attr;
   }
-  kern<<<grid, kGemmThreads, S::kTotal, stream>>>(tmA, tmB, p);
+  kern<<<grid, kGemmThreads, S::kTotal, stream>>>(tmA, tmB, p, CUtensorMap{}, CUtensorMap{});
   XCLIP_LAUNCH_CHECK("gemm_bf16_kernel<simreg>");
   return XCLIP_OK;
 }
