@@ -10,8 +10,11 @@ Sequence length is not limited by the non-causal attention: image towers such as
 (576 patches) and long text towers run on the same kernels (streamed through shared memory above
 320 tokens).  The FILIP loss (`use_all_token_embeds=True`) takes any number of text and image
 tokens: cfg3's 77 x 196 (98 under patch dropout), 576-patch towers and grids smaller than 16 tokens
-run on the same segment-max kernels.  Feature combinations the kernels do not cover raise at construction (never a silent
-CPU or eager fallback): dim_head != 64, model dims not multiples of 256, a causal text tower longer than
+run on the same segment-max kernels.  Model and latent widths may be any multiple of 128 from 128 to
+1024 (ViT-S at 384, B/16-plus at 640 / 896, tiny 128-wide ablations), with any head count: the
+attention width heads * 64 need not equal the model width.  Feature combinations the kernels do not
+cover raise at construction (never a silent CPU or eager fallback): dim_head != 64, model or latent
+widths that are not 128 * {1..8}, a causal text tower longer than
 128 tokens, rotary + causal together (broken in the reference itself: n+1 angles for n tokens,
 x_clip.py:328), dropout > 0 and conv-downsampled image latents.  MLM, SimSiam / SimCLR and the
 multiview term run through the fast encoders (aux.py).  The similarity-regularisation term
@@ -101,7 +104,8 @@ class Transformer(nn.Module):
                  causal: bool = False, attn_dropout: float = 0., ff_dropout: float = 0.,
                  ff_mult: int = 4, checkpoint_during_training: bool = False):
         super().__init__()
-        _require(dim % 256 == 0 and dim <= 1024, f"model dim must be 256/512/768/1024, got {dim}")
+        _require(dim % 128 == 0 and 128 <= dim <= 1024,
+                 f"model dim must be a multiple of 128 from 128 to 1024, got {dim}")
         _require(depth >= 1, "depth must be >= 1")
         self.dim, self.depth, self.heads, self.causal = dim, depth, heads, causal
         # activation checkpointing only trades memory for recompute; accepted and ignored
@@ -330,7 +334,8 @@ class CLIP(nn.Module):
                      "sim_reg_loss_weight > 0 needs extra_latent_projection=True (the reference fails at x_clip.py:779 without it)")
             _require(not use_all_token_embeds,
                      "sim_reg_loss_weight > 0 with use_all_token_embeds (the reference's mask at x_clip.py:779 does not fit the token similarities)")
-        _require(dim_latent % 256 == 0 and dim_latent <= 1024, "dim_latent must be 256/512/768/1024")
+        _require(dim_latent % 128 == 0 and 128 <= dim_latent <= 1024,
+                 f"dim_latent must be a multiple of 128 from 128 to 1024, got {dim_latent}")
         _require(dim_text % 8 == 0 and dim_image % 8 == 0, "dim_text / dim_image must be multiples of 8")
 
         self.dim_text, self.dim_image, self.dim_latent = dim_text, dim_image, dim_latent

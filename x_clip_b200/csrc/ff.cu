@@ -93,7 +93,7 @@ using namespace xclip;
 extern "C" int xclip_ff_permute_cast(const float* w1, void* out, int d, xclip_stream_t stream) {
   int rc = xclip_init();
   if (rc) return rc;
-  XCLIP_REQUIRE(w1 && out && d > 0 && d % 256 == 0, "ff_permute_cast: d=%d must be a multiple of 256", d);
+  XCLIP_REQUIRE(w1 && out && d > 0 && d % 128 == 0, "ff_permute_cast: d=%d must be a multiple of 128", d);
   XCLIP_REQUIRE(FF_ALIGNED(w1) && FF_ALIGNED(out), "ff_permute_cast: misaligned pointer");
   ff_permute_cast_kernel<<<num_sms() * 8, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       w1, reinterpret_cast<bf16*>(out), d);
@@ -105,7 +105,7 @@ extern "C" int xclip_ff_scale_cast(const float* w2, const float* g, void* w2g, f
                                    xclip_stream_t stream) {
   int rc = xclip_init();
   if (rc) return rc;
-  XCLIP_REQUIRE(w2 && g && w2g && colvec && d > 0 && d % 256 == 0, "ff_scale_cast: bad arguments");
+  XCLIP_REQUIRE(w2 && g && w2g && colvec && d > 0 && d % 128 == 0, "ff_scale_cast: bad arguments");
   XCLIP_REQUIRE(FF_ALIGNED(w2) && FF_ALIGNED(g) && FF_ALIGNED(w2g), "ff_scale_cast: misaligned pointer");
   ff_scale_cast_kernel<<<d, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       w2, g, reinterpret_cast<bf16*>(w2g), colvec, d);
@@ -120,7 +120,7 @@ extern "C" int xclip_ff_up(const void* x, int64_t ldx, const void* w1p, void* u,
   XCLIP_REQUIRE(x && w1p && hp && rowsum, "ff_up: null pointer");
   const bool skip_u = (u == nullptr);      // forward-only sweeps: hp is all the down-projection needs
   if (skip_u) { u = hp; ldu = 8 * (int64_t)d; }   // (placeholder, never stored to)
-  XCLIP_REQUIRE(M > 0 && d > 0 && d % 256 == 0, "ff_up: M=%d d=%d (d %% 256)", M, d);
+  XCLIP_REQUIRE(M > 0 && d > 0 && d % 128 == 0, "ff_up: M=%d d=%d (d %% 128)", M, d);
   XCLIP_REQUIRE(ldx % 8 == 0 && ldx >= d && ldu % 8 == 0 && ldu >= 8 * d && ldhp % 8 == 0 && ldhp >= 4 * d,
                 "ff_up: bad leading dimensions");
   XCLIP_REQUIRE(FF_ALIGNED(x) && FF_ALIGNED(w1p) && FF_ALIGNED(u) && FF_ALIGNED(hp) && FF_ALIGNED(rowsum),
@@ -147,7 +147,7 @@ extern "C" int xclip_ff_down(const void* hp, int64_t ldhp, const void* w2g, cons
   int rc = xclip_init();
   if (rc) return rc;
   XCLIP_REQUIRE(hp && w2g && colvec && rowsum && out && acc_out && stats, "ff_down: null pointer");
-  XCLIP_REQUIRE(M > 0 && d > 0 && d % 256 == 0, "ff_down: M=%d d=%d (d %% 256)", M, d);
+  XCLIP_REQUIRE(M > 0 && d > 0 && d % 128 == 0, "ff_down: M=%d d=%d (d %% 128)", M, d);
   XCLIP_REQUIRE(ldhp % 8 == 0 && ldhp >= 4 * d && ldo % 8 == 0 && ldo >= d && ldacc % 8 == 0 && ldacc >= d &&
                     (!residual || (ldr % 8 == 0 && ldr >= d)),
                 "ff_down: bad leading dimensions");
@@ -174,7 +174,7 @@ extern "C" int xclip_ff_bwd(const void* dx, int64_t lddx, const void* w2g, const
   int rc = xclip_init();
   if (rc) return rc;
   XCLIP_REQUIRE(dx && w2g && u && stats && ab && du, "ff_bwd: null pointer");
-  XCLIP_REQUIRE(M > 0 && d > 0 && d % 256 == 0, "ff_bwd: M=%d d=%d (d %% 256)", M, d);
+  XCLIP_REQUIRE(M > 0 && d > 0 && d % 128 == 0, "ff_bwd: M=%d d=%d (d %% 128)", M, d);
   XCLIP_REQUIRE(lddx % 8 == 0 && lddx >= d && ldu % 8 == 0 && ldu >= 8 * d && lddu % 8 == 0 && lddu >= 8 * d,
                 "ff_bwd: bad leading dimensions");
   XCLIP_REQUIRE(FF_ALIGNED(dx) && FF_ALIGNED(w2g) && FF_ALIGNED(u) && FF_ALIGNED(du) && FF_ALIGNED8(stats) &&

@@ -6,9 +6,12 @@
 //
 // One warp owns one row; a lane owns 16-byte vectors (8 bf16) strided by 32 lanes so every
 // warp-wide access is a fully coalesced 512-byte segment.  Row statistics are reduced with
-// warp shuffles in fp32.  Column reductions (gain gradients) are accumulated per lane in
-// registers over the rows a warp visits, combined across the block in shared memory and
-// added to the fp32 output with one atomic per column per block.
+// warp shuffles in fp32.  A row of d = 256 NV + 128 HALF columns holds NV full vectors per lane;
+// with HALF, one more (half) vector covers the last 128 columns in lanes 0-15, and lanes 16-31 add
+// exact zeros to the warp sums (so d = 128 k for k = 1..8; HALF = false is the original code).
+// Column reductions (gain gradients) are accumulated per lane in registers over the rows a warp
+// visits, combined across the block in shared memory and added to the fp32 output with one atomic
+// per column per block.
 #include "common.cuh"
 #include "host.h"
 
@@ -16,6 +19,16 @@ namespace xclip {
 
 constexpr int kRowThreads = 256;
 constexpr int kRowWarps = kRowThreads / 32;
+
+// vectors per lane (the half vector counts as one: never a zero-length array) and row width
+template <int NV, bool HALF> constexpr int kRowVecs = NV + (HALF ? 1 : 0);
+template <int NV, bool HALF> constexpr int kRowD = NV * 256 + (HALF ? 128 : 0);
+
+// does vector j of this lane lie inside the row?  Always true (at compile time) for j < NV.
+template <int NV, bool HALF>
+__device__ __forceinline__ bool vec_live(int j, int lane) {
+  return j < NV || (HALF && lane < 16);
+}
 
 __device__ __forceinline__ void load8(const bf16* p, float (&f)[8]) {
   const uint4 u = *reinterpret_cast<const uint4*>(p);
@@ -53,64 +66,76 @@ __device__ __forceinline__ float bf16_round(float v) {
 }
 
 // Adds the per-lane column partials of all warps of the block and issues one atomicAdd per column.
-template <int NV>
-__device__ __forceinline__ void flush_column_partials(float (&acc)[NV][8], float* dst,
-                                                      float* smem /* [NV*256] */) {
+template <int NV, bool HALF>
+__device__ __forceinline__ void flush_column_partials(float (&acc)[kRowVecs<NV, HALF>][8], float* dst,
+                                                      float* smem /* [D] */) {
+  constexpr int D = kRowD<NV, HALF>;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int i = threadIdx.x; i < NV * 256; i += kRowThreads) smem[i] = 0.f;
+  for (int i = threadIdx.x; i < D; i += kRowThreads) smem[i] = 0.f;
   __syncthreads();
 #pragma unroll
-  for (int j = 0; j < NV; ++j)
+  for (int j = 0; j < kRowVecs<NV, HALF>; ++j)
+    if (vec_live<NV, HALF>(j, lane)) {
 #pragma unroll
-    for (int e = 0; e < 8; ++e) atomicAdd(&smem[(j * 32 + lane) * 8 + e], acc[j][e]);
+      for (int e = 0; e < 8; ++e) atomicAdd(&smem[(j * 32 + lane) * 8 + e], acc[j][e]);
+    }
   (void)warp;
   __syncthreads();
-  for (int i = threadIdx.x; i < NV * 256; i += kRowThreads) atomicAdd(dst + i, smem[i]);
+  for (int i = threadIdx.x; i < D; i += kRowThreads) atomicAdd(dst + i, smem[i]);
 }
 
 // ---------------------------------------------------------------------------
 // LayerNorm forward:  out = LN(x) * g (+ res);  optionally out2 = LN(bf16(out)) * g2
 // stats = (mean, rstd) per row of the FIRST norm, stats2 of the second.
 // ---------------------------------------------------------------------------
-template <int NV>
+template <int NV, bool HALF = false>
 __global__ void __launch_bounds__(kRowThreads)
 ln_fwd_kernel(const bf16* __restrict__ x, long long ldx, const float* __restrict__ g,
               const bf16* __restrict__ res, long long ldres, bf16* __restrict__ out,
               long long ldo, float* __restrict__ stats, const float* __restrict__ g2,
               bf16* __restrict__ out2, long long ldo2, float* __restrict__ stats2, int rows,
               float eps) {
-  constexpr int D = NV * 256;
+  constexpr int D = kRowD<NV, HALF>;
+  constexpr int NVT = kRowVecs<NV, HALF>;
   const int lane = threadIdx.x & 31;
   const int warp_global = blockIdx.x * kRowWarps + (threadIdx.x >> 5);
   const int warp_stride = gridDim.x * kRowWarps;
-  constexpr bool kPipelined = NV <= 3;   // next row's vectors in flight while this row is reduced
-  uint4 nx[NV];
+  // next row's vectors in flight while this row is reduced; 4 vectors a lane (d = 896, 1024) would
+  // cost occupancy, so those rows load just in time
+  constexpr bool kPipelined = NVT <= 3;
+  uint4 nx[NVT];
   if (kPipelined && warp_global < rows) {
 #pragma unroll
-    for (int j = 0; j < NV; ++j)
-      nx[j] = *reinterpret_cast<const uint4*>(x + warp_global * ldx + (j * 32 + lane) * 8);
+    for (int j = 0; j < NVT; ++j)
+      nx[j] = vec_live<NV, HALF>(j, lane)
+                  ? *reinterpret_cast<const uint4*>(x + warp_global * ldx + (j * 32 + lane) * 8)
+                  : make_uint4(0, 0, 0, 0);
   }
   for (int row = warp_global; row < rows; row += warp_stride) {
-    float v[NV][8];
+    float v[NVT][8];
     float s = 0.f;
 #pragma unroll
-    for (int j = 0; j < NV; ++j) {
+    for (int j = 0; j < NVT; ++j) {
       if (kPipelined) unpack8(nx[j], v[j]);
-      else load8(x + row * ldx + (j * 32 + lane) * 8, v[j]);
+      else if (vec_live<NV, HALF>(j, lane)) load8(x + row * ldx + (j * 32 + lane) * 8, v[j]);
+      else unpack8(make_uint4(0, 0, 0, 0), v[j]);
 #pragma unroll
       for (int e = 0; e < 8; ++e) s += v[j][e];
     }
     if (kPipelined && row + warp_stride < rows) {
 #pragma unroll
-      for (int j = 0; j < NV; ++j)
-        nx[j] = *reinterpret_cast<const uint4*>(x + (row + warp_stride) * ldx + (j * 32 + lane) * 8);
+      for (int j = 0; j < NVT; ++j)
+        if (vec_live<NV, HALF>(j, lane))
+          nx[j] = *reinterpret_cast<const uint4*>(x + (row + warp_stride) * ldx + (j * 32 + lane) * 8);
     }
     const float mean = warp_sum(s) * (1.f / D);
     float q = 0.f;
 #pragma unroll
-    for (int j = 0; j < NV; ++j)
+    for (int j = 0; j < NVT; ++j) {
+      if (!vec_live<NV, HALF>(j, lane)) continue;
 #pragma unroll
       for (int e = 0; e < 8; ++e) { const float c = v[j][e] - mean; q += c * c; }
+    }
     const float rstd = rsqrtf(warp_sum(q) * (1.f / D) + eps);
     if (lane == 0 && stats != nullptr) {
       stats[2 * (long long)row] = mean;
@@ -118,7 +143,8 @@ ln_fwd_kernel(const bf16* __restrict__ x, long long ldx, const float* __restrict
     }
     float s2 = 0.f;
 #pragma unroll
-    for (int j = 0; j < NV; ++j) {
+    for (int j = 0; j < NVT; ++j) {
+      if (!vec_live<NV, HALF>(j, lane)) continue;
       const int col = (j * 32 + lane) * 8;
       float gg[8];
       loadf8(g + col, gg);
@@ -136,16 +162,19 @@ ln_fwd_kernel(const bf16* __restrict__ x, long long ldx, const float* __restrict
       const float mean2 = warp_sum(s2) * (1.f / D);
       float q2 = 0.f;
 #pragma unroll
-      for (int j = 0; j < NV; ++j)
+      for (int j = 0; j < NVT; ++j) {
+        if (!vec_live<NV, HALF>(j, lane)) continue;
 #pragma unroll
         for (int e = 0; e < 8; ++e) { const float c = v[j][e] - mean2; q2 += c * c; }
+      }
       const float rstd2 = rsqrtf(warp_sum(q2) * (1.f / D) + eps);
       if (lane == 0 && stats2 != nullptr) {
         stats2[2 * (long long)row] = mean2;
         stats2[2 * (long long)row + 1] = rstd2;
       }
 #pragma unroll
-      for (int j = 0; j < NV; ++j) {
+      for (int j = 0; j < NVT; ++j) {
+        if (!vec_live<NV, HALF>(j, lane)) continue;
         const int col = (j * 32 + lane) * 8;
         float gg[8];
         loadf8(g2 + col, gg);
@@ -162,35 +191,38 @@ ln_fwd_kernel(const bf16* __restrict__ x, long long ldx, const float* __restrict
 // LayerNorm backward: dx = rstd * (g*dy - mean(g*dy) - xhat * mean(g*dy*xhat)) (+ add)
 //                     dg += sum_rows dy * xhat
 // ---------------------------------------------------------------------------
-template <int NV>
+template <int NV, bool HALF = false>
 __global__ void __launch_bounds__(kRowThreads)
 ln_bwd_kernel(const bf16* __restrict__ dy, long long lddy, const bf16* __restrict__ x,
               long long ldx, const float* __restrict__ stats, const float* __restrict__ g,
               const bf16* __restrict__ add, long long ldadd, bf16* __restrict__ dx,
               long long lddx, float* __restrict__ dg, int rows) {
-  constexpr int D = NV * 256;
-  __shared__ float red[NV * 256];
+  constexpr int D = kRowD<NV, HALF>;
+  constexpr int NVT = kRowVecs<NV, HALF>;
+  __shared__ float red[D];
   const int lane = threadIdx.x & 31;
   const int warp_global = blockIdx.x * kRowWarps + (threadIdx.x >> 5);
   const int warp_stride = gridDim.x * kRowWarps;
-  float dgacc[NV][8];
+  float dgacc[NVT][8];
 #pragma unroll
-  for (int j = 0; j < NV; ++j)
+  for (int j = 0; j < NVT; ++j)
 #pragma unroll
     for (int e = 0; e < 8; ++e) dgacc[j][e] = 0.f;
-  float gg[NV][8];
+  float gg[NVT][8];
 #pragma unroll
-  for (int j = 0; j < NV; ++j) loadf8(g + (j * 32 + lane) * 8, gg[j]);
+  for (int j = 0; j < NVT; ++j)
+    if (vec_live<NV, HALF>(j, lane)) loadf8(g + (j * 32 + lane) * 8, gg[j]);
 
   // software pipeline: x, dy (and the residual gradient) of the warp's NEXT row are in flight
   // while the current row is reduced
-  constexpr bool kPipelined = NV <= 2;   // wider rows would spill: they load just in time
-  uint4 nx[NV], nd[NV], na[NV];
+  constexpr bool kPipelined = NVT <= 2;  // wider rows would spill or lose occupancy: they load just in time
+  uint4 nx[NVT], nd[NVT], na[NVT];
   float nmean = 0.f, nrstd = 0.f;
   auto prefetch = [&](int r) {
     if (r < rows) {
 #pragma unroll
-      for (int j = 0; j < NV; ++j) {
+      for (int j = 0; j < NVT; ++j) {
+        if (!vec_live<NV, HALF>(j, lane)) continue;
         const int col = (j * 32 + lane) * 8;
         nx[j] = *reinterpret_cast<const uint4*>(x + r * ldx + col);
         nd[j] = *reinterpret_cast<const uint4*>(dy + r * lddy + col);
@@ -206,7 +238,8 @@ ln_bwd_kernel(const bf16* __restrict__ dy, long long lddy, const bf16* __restric
   auto prefetch_l2 = [&](long long r) {
     if (r < rows && (lane & 7) == 0) {
 #pragma unroll
-      for (int j = 0; j < NV; ++j) {
+      for (int j = 0; j < NVT; ++j) {
+        if (!vec_live<NV, HALF>(j, lane)) continue;
         const int col = (j * 32 + lane) * 8;
         asm volatile("prefetch.global.L2 [%0];" ::"l"(x + r * ldx + col));
         asm volatile("prefetch.global.L2 [%0];" ::"l"(dy + r * lddy + col));
@@ -221,11 +254,12 @@ ln_bwd_kernel(const bf16* __restrict__ dy, long long lddy, const bf16* __restric
       prefetch(row);
     }
     const float mean = nmean, rstd = nrstd;
-    float xh[NV][8], gd[NV][8];
-    uint4 ca[NV];
+    float xh[NVT][8], gd[NVT][8];
+    uint4 ca[NVT];
     float s1 = 0.f, s2 = 0.f;
 #pragma unroll
-    for (int j = 0; j < NV; ++j) {
+    for (int j = 0; j < NVT; ++j) {
+      if (!vec_live<NV, HALF>(j, lane)) continue;
       float d8[8];
       unpack8(nx[j], xh[j]);
       unpack8(nd[j], d8);
@@ -243,7 +277,8 @@ ln_bwd_kernel(const bf16* __restrict__ dy, long long lddy, const bf16* __restric
     s1 = warp_sum(s1) * (1.f / D);
     s2 = warp_sum(s2) * (1.f / D);
 #pragma unroll
-    for (int j = 0; j < NV; ++j) {
+    for (int j = 0; j < NVT; ++j) {
+      if (!vec_live<NV, HALF>(j, lane)) continue;
       const int col = (j * 32 + lane) * 8;
       float a8[8] = {0, 0, 0, 0, 0, 0, 0, 0};
       if (add != nullptr) {
@@ -256,7 +291,7 @@ ln_bwd_kernel(const bf16* __restrict__ dy, long long lddy, const bf16* __restric
       store8(dx + row * lddx + col, o);
     }
   }
-  if (dg != nullptr) flush_column_partials<NV>(dgacc, dg, red);
+  if (dg != nullptr) flush_column_partials<NV, HALF>(dgacc, dg, red);
 }
 
 // ---------------------------------------------------------------------------
@@ -399,7 +434,7 @@ geglu_ln_bwd_kernel(const bf16* __restrict__ dh, long long lddh, const bf16* __r
 //   inv = 1/max(||p||,eps)
 //   bwd: dp = inv * (dz - z * <z, dz>)   (bf16, operand of the projection dgrad/wgrad)
 // ---------------------------------------------------------------------------
-template <int NV>
+template <int NV, bool HALF = false>
 __global__ void __launch_bounds__(kRowThreads)
 l2norm_fwd_kernel(const float* __restrict__ p, long long ldp, float* __restrict__ z,
                   bf16* __restrict__ zrow, bf16* __restrict__ zcol, float* __restrict__ inv,
@@ -407,12 +442,14 @@ l2norm_fwd_kernel(const float* __restrict__ p, long long ldp, float* __restrict_
   const int lane = threadIdx.x & 31;
   const int warp_global = blockIdx.x * kRowWarps + (threadIdx.x >> 5);
   const int warp_stride = gridDim.x * kRowWarps;
-  constexpr int D = NV * 256;
+  constexpr int D = kRowD<NV, HALF>;
+  constexpr int NVT = kRowVecs<NV, HALF>;
   for (int row = warp_global; row < rows; row += warp_stride) {
-    float v[NV][8];
+    float v[NVT][8];
     float q = 0.f;
 #pragma unroll
-    for (int j = 0; j < NV; ++j) {
+    for (int j = 0; j < NVT; ++j) {
+      if (!vec_live<NV, HALF>(j, lane)) continue;
       loadf8(p + row * ldp + (j * 32 + lane) * 8, v[j]);
 #pragma unroll
       for (int e = 0; e < 8; ++e) q += v[j][e] * v[j][e];
@@ -420,7 +457,8 @@ l2norm_fwd_kernel(const float* __restrict__ p, long long ldp, float* __restrict_
     const float r = 1.f / fmaxf(sqrtf(warp_sum(q)), 1e-12f);
     if (lane == 0) inv[row] = r;
 #pragma unroll
-    for (int j = 0; j < NV; ++j) {
+    for (int j = 0; j < NVT; ++j) {
+      if (!vec_live<NV, HALF>(j, lane)) continue;
       const int col = (j * 32 + lane) * 8;
       float hi[8], lo[8];
 #pragma unroll
@@ -439,19 +477,21 @@ l2norm_fwd_kernel(const float* __restrict__ p, long long ldp, float* __restrict_
   }
 }
 
-template <int NV>
+template <int NV, bool HALF = false>
 __global__ void __launch_bounds__(kRowThreads)
 l2norm_bwd_kernel(const float* __restrict__ dz, const float* __restrict__ z,
                   const float* __restrict__ inv, bf16* __restrict__ dp, int rows) {
   const int lane = threadIdx.x & 31;
   const int warp_global = blockIdx.x * kRowWarps + (threadIdx.x >> 5);
   const int warp_stride = gridDim.x * kRowWarps;
-  constexpr int D = NV * 256;
+  constexpr int D = kRowD<NV, HALF>;
+  constexpr int NVT = kRowVecs<NV, HALF>;
   for (int row = warp_global; row < rows; row += warp_stride) {
-    float a[NV][8], b[NV][8];
+    float a[NVT][8], b[NVT][8];
     float dot = 0.f;
 #pragma unroll
-    for (int j = 0; j < NV; ++j) {
+    for (int j = 0; j < NVT; ++j) {
+      if (!vec_live<NV, HALF>(j, lane)) continue;
       const int col = (j * 32 + lane) * 8;
       loadf8(dz + (long long)row * D + col, a[j]);
       loadf8(z + (long long)row * D + col, b[j]);
@@ -461,7 +501,8 @@ l2norm_bwd_kernel(const float* __restrict__ dz, const float* __restrict__ z,
     dot = warp_sum(dot);
     const float r = inv[row];
 #pragma unroll
-    for (int j = 0; j < NV; ++j) {
+    for (int j = 0; j < NVT; ++j) {
+      if (!vec_live<NV, HALF>(j, lane)) continue;
       const int col = (j * 32 + lane) * 8;
       float o[8];
 #pragma unroll
@@ -480,19 +521,20 @@ l2norm_bwd_kernel(const float* __restrict__ dz, const float* __restrict__ z,
 //           = the two row means mean_k(gdh) and mean_k(gdh * hn) of the LayerNorm backward, because
 //             gdh = dx W2g and sum_k hn_k W2g_jk = (x2 - x1)_j = rstd (acc_j - mean colvec_j).
 // ---------------------------------------------------------------------------
-template <int NV>
+template <int NV, bool HALF = false>
 __global__ void __launch_bounds__(kRowThreads, 2)
 ff_bwd_prep_kernel(const bf16* __restrict__ dx, long long lddx, const float* __restrict__ stats,
                    const bf16* __restrict__ acc, long long ldacc, const float* __restrict__ colvec,
                    bf16* __restrict__ dxs, float* __restrict__ vsum, float* __restrict__ ab, int rows) {
-  __shared__ float red[NV * 256];
-  constexpr int D = NV * 256;
+  constexpr int D = kRowD<NV, HALF>;
+  constexpr int NVT = kRowVecs<NV, HALF>;
+  __shared__ float red[D];
   const int lane = threadIdx.x & 31;
   const int warp_global = blockIdx.x * kRowWarps + (threadIdx.x >> 5);
   const int warp_stride = gridDim.x * kRowWarps;
-  float vacc[NV][8];
+  float vacc[NVT][8];
 #pragma unroll
-  for (int j = 0; j < NV; ++j)
+  for (int j = 0; j < NVT; ++j)
 #pragma unroll
     for (int e = 0; e < 8; ++e) vacc[j][e] = 0.f;
   const float invD4 = 1.f / (4.f * D);
@@ -502,12 +544,13 @@ ff_bwd_prep_kernel(const bf16* __restrict__ dx, long long lddx, const float* __r
   // outstanding).  colvec is re-read from L1 instead of living in 8 NV registers.
   for (long long row0 = 2ll * warp_global; row0 < rows; row0 += 2ll * warp_stride) {
     const bool two = row0 + 1 < rows;
-    uint4 rdx[2][NV], rac[2][NV];
+    uint4 rdx[2][NVT], rac[2][NVT];
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
       const long long row = (r == 0 || two) ? row0 + r : row0;
 #pragma unroll
-      for (int j = 0; j < NV; ++j) {
+      for (int j = 0; j < NVT; ++j) {
+        if (!vec_live<NV, HALF>(j, lane)) continue;
         const int col = (j * 32 + lane) * 8;
         rdx[r][j] = *reinterpret_cast<const uint4*>(dx + row * lddx + col);
         if (ab != nullptr) rac[r][j] = *reinterpret_cast<const uint4*>(acc + row * ldacc + col);
@@ -525,7 +568,8 @@ ff_bwd_prep_kernel(const bf16* __restrict__ dx, long long lddx, const float* __r
     for (int r = 0; r < 2; ++r) {
       if (r == 1 && !two) break;
 #pragma unroll
-      for (int j = 0; j < NV; ++j) {
+      for (int j = 0; j < NVT; ++j) {
+        if (!vec_live<NV, HALF>(j, lane)) continue;
         const int col = (j * 32 + lane) * 8;
         float f[8];
         unpack8(rdx[r][j], f);
@@ -563,7 +607,7 @@ ff_bwd_prep_kernel(const bf16* __restrict__ dx, long long lddx, const float* __r
       }
     }
   }
-  flush_column_partials<NV>(vacc, vsum, red);
+  flush_column_partials<NV, HALF>(vacc, vsum, red);
 }
 
 // raw = dxs^T hp (f32 [d, 4d]).  In place: dW2[j,k] = g[k] (raw[j,k] - vsum[j]);  optionally
@@ -618,8 +662,9 @@ static int wide_grid(int rows, int dh) {
 
 using namespace xclip;
 
-#define LAUNCH_NV(KERNEL, NVAL, GRID, STREAM, ...) \
-  case NVAL: KERNEL<NVAL><<<GRID, kRowThreads, 0, STREAM>>>(__VA_ARGS__); break;
+// K = d / 128: NV = K / 2 full vectors per lane (256 columns a warp), plus the half vector when K is odd
+#define LAUNCH_ROW(KERNEL, K, GRID, STREAM, ...) \
+  case K: KERNEL<(K) / 2, (K) % 2 == 1><<<GRID, kRowThreads, 0, STREAM>>>(__VA_ARGS__); break;
 
 #define LAUNCH_WIDE(KERNEL, THREADS, GRID, STREAM, ...) \
   case THREADS: KERNEL<THREADS><<<GRID, THREADS, 0, STREAM>>>(__VA_ARGS__); break;
@@ -635,14 +680,19 @@ using namespace xclip;
       return fail(XCLIP_ERR_INVALID, "hidden width %d unsupported (1024*{1,2,3,4})", (D)); \
   }
 
+// row widths d = 128 k, k = 1..8 (callers check d % 128 == 0 first)
 #define DISPATCH_NARROW(KERNEL, D, GRID, STREAM, ...)                                     \
-  switch ((D) / 256) {                                                                    \
-    LAUNCH_NV(KERNEL, 1, GRID, STREAM, __VA_ARGS__)                                       \
-    LAUNCH_NV(KERNEL, 2, GRID, STREAM, __VA_ARGS__)                                       \
-    LAUNCH_NV(KERNEL, 3, GRID, STREAM, __VA_ARGS__)                                       \
-    LAUNCH_NV(KERNEL, 4, GRID, STREAM, __VA_ARGS__)                                       \
+  switch ((D) / 128) {                                                                    \
+    LAUNCH_ROW(KERNEL, 1, GRID, STREAM, __VA_ARGS__)                                      \
+    LAUNCH_ROW(KERNEL, 2, GRID, STREAM, __VA_ARGS__)                                      \
+    LAUNCH_ROW(KERNEL, 3, GRID, STREAM, __VA_ARGS__)                                      \
+    LAUNCH_ROW(KERNEL, 4, GRID, STREAM, __VA_ARGS__)                                      \
+    LAUNCH_ROW(KERNEL, 5, GRID, STREAM, __VA_ARGS__)                                      \
+    LAUNCH_ROW(KERNEL, 6, GRID, STREAM, __VA_ARGS__)                                      \
+    LAUNCH_ROW(KERNEL, 7, GRID, STREAM, __VA_ARGS__)                                      \
+    LAUNCH_ROW(KERNEL, 8, GRID, STREAM, __VA_ARGS__)                                      \
     default:                                                                              \
-      return fail(XCLIP_ERR_INVALID, "row width %d unsupported (256*{1,2,3,4})", (D));    \
+      return fail(XCLIP_ERR_INVALID, "row width %d unsupported (128*{1..8})", (D));       \
   }
 
 #define ALIGNED16(p) ((reinterpret_cast<uintptr_t>(p) & 15) == 0)
@@ -655,7 +705,7 @@ extern "C" int xclip_layernorm_fwd(const void* x, int64_t ldx, const float* g, c
   if (rc) return rc;
   XCLIP_REQUIRE(x && g && out, "layernorm_fwd: null pointer");
   XCLIP_REQUIRE(rows > 0, "layernorm_fwd: rows=%d", rows);
-  XCLIP_REQUIRE(d % 256 == 0, "layernorm_fwd: d=%d must be a multiple of 256", d);
+  XCLIP_REQUIRE(d > 0 && d % 128 == 0 && d <= 1024, "layernorm_fwd: d=%d must be 128*{1..8}", d);
   XCLIP_REQUIRE(ldx % 8 == 0 && ldo % 8 == 0 && (!res || ldres % 8 == 0) && (!g2 || ldo2 % 8 == 0),
                 "layernorm_fwd: leading dims must be multiples of 8");
   XCLIP_REQUIRE(ALIGNED16(x) && ALIGNED16(out) && ALIGNED16(g) && (!res || ALIGNED16(res)) &&
@@ -678,7 +728,8 @@ extern "C" int xclip_layernorm_bwd(const void* dy, int64_t lddy, const void* x, 
   int rc = xclip_init();
   if (rc) return rc;
   XCLIP_REQUIRE(dy && x && stats && g && dx, "layernorm_bwd: null pointer");
-  XCLIP_REQUIRE(rows > 0 && d % 256 == 0, "layernorm_bwd: rows=%d d=%d", rows, d);
+  XCLIP_REQUIRE(rows > 0 && d > 0 && d % 128 == 0 && d <= 1024, "layernorm_bwd: rows=%d d=%d (d = 128*{1..8})",
+                rows, d);
   XCLIP_REQUIRE(lddy % 8 == 0 && ldx % 8 == 0 && lddx % 8 == 0 && (!add || ldadd % 8 == 0),
                 "layernorm_bwd: leading dims must be multiples of 8");
   XCLIP_REQUIRE(ALIGNED16(dy) && ALIGNED16(x) && ALIGNED16(dx) && ALIGNED16(g) &&
@@ -732,7 +783,8 @@ extern "C" int xclip_l2norm_fwd(const float* p, int64_t ldp, float* z, void* zro
   int rc = xclip_init();
   if (rc) return rc;
   XCLIP_REQUIRE(p && z && zrow && zcol && inv, "l2norm_fwd: null pointer");
-  XCLIP_REQUIRE(rows > 0 && d % 256 == 0, "l2norm_fwd: rows=%d d=%d", rows, d);
+  XCLIP_REQUIRE(rows > 0 && d > 0 && d % 128 == 0 && d <= 1024, "l2norm_fwd: rows=%d d=%d (d = 128*{1..8})",
+                rows, d);
   XCLIP_REQUIRE(ldp % 4 == 0 && ALIGNED16(p) && ALIGNED16(z) && ALIGNED16(zrow) && ALIGNED16(zcol),
                 "l2norm_fwd: misaligned");
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
@@ -747,7 +799,8 @@ extern "C" int xclip_l2norm_bwd(const float* dz, const float* z, const float* in
   int rc = xclip_init();
   if (rc) return rc;
   XCLIP_REQUIRE(dz && z && inv && dp, "l2norm_bwd: null pointer");
-  XCLIP_REQUIRE(rows > 0 && d % 256 == 0, "l2norm_bwd: rows=%d d=%d", rows, d);
+  XCLIP_REQUIRE(rows > 0 && d > 0 && d % 128 == 0 && d <= 1024, "l2norm_bwd: rows=%d d=%d (d = 128*{1..8})",
+                rows, d);
   XCLIP_REQUIRE(ALIGNED16(dz) && ALIGNED16(z) && ALIGNED16(dp), "l2norm_bwd: misaligned");
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   DISPATCH_NARROW(l2norm_bwd_kernel, d, row_grid(rows), s, dz, z, inv, (bf16*)dp, rows)
@@ -842,7 +895,7 @@ extern "C" int xclip_ff_bwd_prep(const void* dx, int64_t lddx, const float* stat
   int rc = xclip_init();
   if (rc) return rc;
   XCLIP_REQUIRE(dx && stats && dxs && vsum && rows > 0, "ff_bwd_prep: bad arguments");
-  XCLIP_REQUIRE(d % 256 == 0, "ff_bwd_prep: d=%d must be a multiple of 256", d);
+  XCLIP_REQUIRE(d > 0 && d % 128 == 0 && d <= 1024, "ff_bwd_prep: d=%d must be 128*{1..8}", d);
   XCLIP_REQUIRE(ab == nullptr || (acc && colvec), "ff_bwd_prep: ab needs acc and colvec");
   XCLIP_REQUIRE(lddx % 8 == 0 && lddx >= d && ALIGNED16(dx) && ALIGNED16(dxs) &&
                     (!acc || (ALIGNED16(acc) && ldacc % 8 == 0 && ldacc >= d)) && (!colvec || ALIGNED16(colvec)),
@@ -860,7 +913,7 @@ extern "C" int xclip_ff_w2_grad_post(float* raw, const float* vsum, const float*
   using namespace xclip;
   int rc = xclip_init();
   if (rc) return rc;
-  XCLIP_REQUIRE(raw && vsum && g && d > 0 && d % 256 == 0, "ff_w2_grad_post: bad arguments");
+  XCLIP_REQUIRE(raw && vsum && g && d > 0 && d % 128 == 0, "ff_w2_grad_post: bad arguments");
   XCLIP_REQUIRE((dg == nullptr) == (w2 == nullptr), "ff_w2_grad_post: dg and w2 go together");
   const int rows_per_block = 8;      // 4d/256 x d/8 blocks: enough loads in flight for a 28 MB pass
   dim3 grid((4 * d + 255) / 256, (d + rows_per_block - 1) / rows_per_block);
