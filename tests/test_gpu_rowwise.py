@@ -196,7 +196,7 @@ def test_l2norm(cuda_device, rows, d):
 
 def test_cast(cuda_device):
     from x_clip_b200 import kernels as K
-    for n in (1, 7, 8, 1000003):
+    for n in (1, 7, 8, 1000003, 8 * 1024 * 1024):     # the last: an 8d x d weight at d = 1024, past the grid cap
         src = torch.randn(n, device=cuda_device)
         assert torch.equal(K.cast_bf16(src), src.bfloat16())
 
