@@ -290,10 +290,19 @@ int xclip_adamw_step(float* p, const float* g, float* m, float* v, int64_t n, fl
  * patchify_gather : img f32 [B,C,H,W] -> bf16 [B*k, patch*patch*C] rows in the reference's
  *                   (p1 p2 c) order for the patches keep[b, j] (int64 [B,k]; NULL = all k = n patches,
  *                   in order): only kept patches are read and embedded.
+ * patchify_scatter: the inverse (the image gradient): src f32 [B*k, patch*patch*C] (row stride lds, rows
+ *                   in the gather's order, (p1 p2 c) inside a row) -> img_grad f32 [B,C,H,W].  Every
+ *                   element is written: pixels of the patch keep[b, j] take row b*k + j, pixels of
+ *                   patches absent from keep[b, :] are 0 (allocate img_grad uninitialised).  The indices
+ *                   of one sample must be distinct (PatchDropout draws them with topk), so no pixel has
+ *                   two sources and no atomics are used; with duplicates the result is unspecified.
+ *                   src and img_grad 16-byte aligned, lds %% 4 == 0; the other refusals are the gather's.
  * scatter_add_rows: dst f32 [V,d] rows idx[r] (or r %% period) += src bf16 [rows,d]  (gradient of the
  *                   gathered position table);  colsum_rows: dst[d] += column sums (bias gradient). */
 int xclip_patchify_gather(const float* img, int B, int C, int H, int W, int patch, const int64_t* keep,
                           int k, void* out, xclip_stream_t stream);
+int xclip_patchify_scatter(const float* src, int64_t lds, int B, int C, int H, int W, int patch,
+                           const int64_t* keep, int k, float* img_grad, xclip_stream_t stream);
 int xclip_scatter_add_rows(const int32_t* idx, int period, const void* src, int64_t lds, float* dst,
                            int64_t rows, int d, int V, xclip_stream_t stream);
 int xclip_colsum_rows(const void* src, int64_t lds, float* dst, int64_t rows, int d,

@@ -241,7 +241,8 @@ class VisionTransformer(nn.Module):
     def forward(self, x, keep_all_patches: bool = False):
         """image f32 [b, c, H, W] -> [b, 1 + n_kept, dim] (CLS first).  Patchify, PatchDropout and the
         bf16 cast are ONE pass that reads only the kept patches (xclip_patchify_gather); the
-        patch-embedding GEMM adds bias and the gathered position rows in its epilogue."""
+        patch-embedding GEMM adds bias and the gathered position rows in its epilogue.  An image with
+        requires_grad gets its gradient (xclip_patchify_scatter; 0 on dropped patches)."""
         b = x.shape[0]
         _require(x.is_cuda, "inputs must live on a CUDA (sm_90) device")
         p = self.patch_size
@@ -256,8 +257,14 @@ class VisionTransformer(nn.Module):
         else:
             index = keep.reshape(-1).to(torch.int32)
             k = keep.shape[1]
-        patches = E.K.patchify_gather(x.float(), p, keep)
-        tok = E.PatchEmbedFn.apply(patches, index, lin.weight, lin.bias, self.pos_emb.weight)
+        x = x.float()
+        if x.requires_grad and torch.is_grad_enabled():
+            # d loss / d image (adversarial training, guidance, saliency): the backward scatters the
+            # patch gradients back to pixels; every other call keeps the launch sequence below
+            tok = E.PatchifyFn.apply(x, p, keep, index, lin.weight, lin.bias, self.pos_emb.weight)
+        else:
+            patches = E.K.patchify_gather(x, p, keep)
+            tok = E.PatchEmbedFn.apply(patches, index, lin.weight, lin.bias, self.pos_emb.weight)
         out = self.transformer(tok.view(b, k, -1))
         pooled = out.float().mean(dim=1).to(BF16)
         cls = E.LinearFn.apply(pooled, self.to_cls_tokens[1].weight, None, None)

@@ -256,6 +256,74 @@ patchify_gather_kernel(const float* __restrict__ img, int B, int C, int H, int W
   }
 }
 
+// Inverse of the gather (the image gradient): block (b, chunk) owns patches [lo, lo + ppc) of sample b
+// and writes every pixel of them, the src row of a kept patch or 0 for a dropped one.  The row of each
+// owned patch comes from an inverse map of keep[b, :] built in shared memory (indices of one sample are
+// distinct, so each slot has at most one writer).
+//   CT > 0 (C == CT, patch % 4 == 0): a thread owns 4 horizontally adjacent pixels of one patch row:
+//          CT 16-byte loads of the (p1 p2 c) row (4 pixels x CT channels, contiguous), transposed in
+//          registers, CT 16-byte stores, one per channel plane.  Consecutive threads walk along p2, so
+//          loads are contiguous across a warp and stores fill whole 32-byte sectors of an image row.
+//   CT == 0: any C / patch, one pixel x C channels per thread with scalar accesses.
+constexpr int kScatterMaxPatchesPerBlock = 1024;
+
+template <int CT>
+__global__ void __launch_bounds__(256)
+patchify_scatter_kernel(const float* __restrict__ src, long long lds, int B, int C, int H, int W, int P,
+                        const long long* __restrict__ keep, int k, int n_patches, int ppc,
+                        float* __restrict__ img) {
+  __shared__ int inv[kScatterMaxPatchesPerBlock];
+  const long long b = blockIdx.x;
+  const int lo = blockIdx.y * ppc;
+  const int cnt = min(ppc, n_patches - lo);
+  if (cnt <= 0) return;
+  if (keep != nullptr) {
+    for (int i = threadIdx.x; i < cnt; i += blockDim.x) inv[i] = -1;
+    __syncthreads();
+    for (int j = threadIdx.x; j < k; j += blockDim.x) {
+      const long long p = keep[b * k + j];
+      if (p < 0 || p >= n_patches) __trap();
+      if (p >= lo && p < lo + cnt) inv[p - lo] = j;
+    }
+    __syncthreads();
+  }
+  const int gw_n = W / P;
+  const int per_row = (CT > 0) ? P / 4 : P;          // work items per patch row
+  const int per_patch = P * per_row;
+  const int items = cnt * per_patch;       // < 2^31 for patch sizes up to 2048
+  for (int it = threadIdx.x; it < items; it += blockDim.x) {
+    const int pl = it / per_patch;
+    const int w = it - pl * per_patch;
+    const int p1 = w / per_row;
+    const int p2 = (w - p1 * per_row) * (CT > 0 ? 4 : 1);
+    const int pidx = lo + pl;
+    const int j = keep != nullptr ? inv[pl] : pidx;
+    const int gh = pidx / gw_n, gw = pidx - gh * gw_n;
+    const long long plane = (long long)H * W;
+    float* dst = img + (b * C) * plane + (long long)(gh * P + p1) * W + gw * P + p2;
+    const float* s = j >= 0 ? src + (b * k + j) * lds + (long long)(p1 * P + p2) * C : nullptr;
+    if constexpr (CT > 0) {
+      float v[4 * CT];
+      if (j >= 0) {
+#pragma unroll
+        for (int i = 0; i < CT; ++i) {
+          const float4 t = *reinterpret_cast<const float4*>(s + 4 * i);
+          v[4 * i] = t.x; v[4 * i + 1] = t.y; v[4 * i + 2] = t.z; v[4 * i + 3] = t.w;
+        }
+      } else {
+#pragma unroll
+        for (int i = 0; i < 4 * CT; ++i) v[i] = 0.f;
+      }
+#pragma unroll
+      for (int c = 0; c < CT; ++c)
+        *reinterpret_cast<float4*>(dst + c * plane) =
+            make_float4(v[c], v[CT + c], v[2 * CT + c], v[3 * CT + c]);
+    } else {
+      for (int c = 0; c < C; ++c) dst[c * plane] = j >= 0 ? s[c] : 0.f;
+    }
+  }
+}
+
 // dst[idx[r] or r %% period, :] += src[r, :]  (f32 += bf16): gradient of a gathered / periodic table
 __global__ void __launch_bounds__(256)
 scatter_add_rows_kernel(const int* __restrict__ idx, int period, const bf16* __restrict__ src,
@@ -315,6 +383,45 @@ extern "C" int xclip_patchify_gather(const float* img, int B, int C, int H, int 
       img, B, C, H, W, patch, reinterpret_cast<const long long*>(keep), k, n_patches,
       reinterpret_cast<bf16*>(out));
   XCLIP_LAUNCH_CHECK("patchify_gather_kernel");
+  return XCLIP_OK;
+}
+
+extern "C" int xclip_patchify_scatter(const float* src, int64_t lds, int B, int C, int H, int W, int patch,
+                                      const int64_t* keep, int k, float* img_grad, xclip_stream_t stream) {
+  using namespace xclip;
+  int rc = xclip_init();
+  if (rc) return rc;
+  XCLIP_REQUIRE(src && img_grad && B > 0 && C > 0 && patch > 0 && H % patch == 0 && W % patch == 0,
+                "patchify_scatter: bad arguments");
+  const int n_patches = (H / patch) * (W / patch);
+  const int patch_dim = patch * patch * C;
+  XCLIP_REQUIRE(patch_dim % 8 == 0, "patchify_scatter: channels*patch^2 must be a multiple of 8");
+  XCLIP_REQUIRE(k > 0 && k <= n_patches && (keep != nullptr || k == n_patches), "patchify_scatter: k=%d", k);
+  XCLIP_REQUIRE(lds >= patch_dim && lds % 4 == 0 && (reinterpret_cast<uintptr_t>(src) & 15) == 0 &&
+                    (reinterpret_cast<uintptr_t>(img_grad) & 15) == 0,
+                "patchify_scatter: src and img_grad must be 16-byte aligned with lds %% 4 == 0");
+  // about 8 blocks per SM in all, at most kScatterMaxPatchesPerBlock patches per block
+  const long long target = (long long)num_sms() * 8;
+  long long chunks = (target + B - 1) / B;
+  if (chunks > n_patches) chunks = n_patches;
+  int ppc = (int)((n_patches + chunks - 1) / chunks);
+  if (ppc > kScatterMaxPatchesPerBlock) ppc = kScatterMaxPatchesPerBlock;
+  chunks = (n_patches + ppc - 1) / ppc;
+  XCLIP_REQUIRE(chunks <= 65535, "patchify_scatter: %d patches per image", n_patches);
+  dim3 grid((unsigned)B, (unsigned)chunks);
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  const long long* kp = reinterpret_cast<const long long*>(keep);
+  if (patch % 4 == 0 && C <= 4) {
+    switch (C) {
+      case 1: patchify_scatter_kernel<1><<<grid, 256, 0, s>>>(src, lds, B, C, H, W, patch, kp, k, n_patches, ppc, img_grad); break;
+      case 2: patchify_scatter_kernel<2><<<grid, 256, 0, s>>>(src, lds, B, C, H, W, patch, kp, k, n_patches, ppc, img_grad); break;
+      case 3: patchify_scatter_kernel<3><<<grid, 256, 0, s>>>(src, lds, B, C, H, W, patch, kp, k, n_patches, ppc, img_grad); break;
+      default: patchify_scatter_kernel<4><<<grid, 256, 0, s>>>(src, lds, B, C, H, W, patch, kp, k, n_patches, ppc, img_grad); break;
+    }
+  } else {
+    patchify_scatter_kernel<0><<<grid, 256, 0, s>>>(src, lds, B, C, H, W, patch, kp, k, n_patches, ppc, img_grad);
+  }
+  XCLIP_LAUNCH_CHECK("patchify_scatter_kernel");
   return XCLIP_OK;
 }
 

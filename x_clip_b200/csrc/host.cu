@@ -87,12 +87,24 @@ int ensure_dynamic_smem(const void* kernel, int bytes) {
   return XCLIP_OK;
 }
 
+// cuTensorMapEncodeTiled needs a current context.  A thread whose first CUDA work is a GEMM of this
+// library (an autograd worker thread whose first backward op is a GEMM, for one) may have none bound
+// yet: cudaFree(nullptr) binds the primary context of the thread's current device, once per thread.
+static void bind_thread_context() {
+  static thread_local bool bound = false;
+  if (!bound) {
+    cudaFree(nullptr);
+    bound = true;
+  }
+}
+
 int encode_2d_bf16(CUtensorMap* out, const void* ptr, uint64_t inner, uint64_t outer,
                    uint64_t outer_stride_elems, uint32_t box_inner, uint32_t box_outer) {
   if (!g_inited) {
     int rc = do_init();
     if (rc) return rc;
   }
+  bind_thread_context();
   cuuint64_t dims[2] = {inner, outer};
   cuuint64_t strides[1] = {outer_stride_elems * 2};
   cuuint32_t box[2] = {box_inner, box_outer};
@@ -117,6 +129,7 @@ int encode_3d_bf16(CUtensorMap* out, const void* ptr, uint64_t inner, uint64_t m
     int rc = do_init();
     if (rc) return rc;
   }
+  bind_thread_context();
   cuuint64_t dims[3] = {inner, mid, outer};
   cuuint64_t strides[2] = {mid_stride_elems * 2, outer_stride_elems * 2};
   cuuint32_t box[3] = {box_inner, box_mid, 1};

@@ -15,6 +15,7 @@ from __future__ import annotations
 from typing import List, Optional
 
 import torch
+from torch.autograd.function import once_differentiable
 
 from . import kernels as K
 from . import distributed as D_
@@ -240,9 +241,16 @@ class TransformerFn(torch.autograd.Function):
 
         grads: List[Optional[torch.Tensor]] = [None] * len(weights)
         wg = _WgradStream(dev)
+        # parameters with requires_grad=False (a frozen tower: adversarial / guidance use) cost no
+        # weight-gradient work: their wgrad GEMMs and gain reductions are skipped and None returned.
+        # The data-gradient chain reads none of them, so dx is the same either way.
+        wneed = ctx.needs_input_grad[8:]
 
         def gain_grad(idx):
-            """fp32 accumulator for the gain gradient of weights[idx]: its .grad (in-place mode) or zeros"""
+            """fp32 accumulator for the gain gradient of weights[idx]: its .grad (in-place mode) or
+            zeros; (None, None) when the gain needs no gradient"""
+            if not wneed[idx]:
+                return None, None
             tgt = _grad_target(weights[idx])
             if tgt is not None:
                 return tgt, None
@@ -250,6 +258,8 @@ class TransformerFn(torch.autograd.Function):
             return z, z
 
         def weight_grad(idx, dy_, x_):
+            if not wneed[idx]:
+                return None
             tgt = _grad_target(weights[idx])
             if tgt is not None:
                 K.gemm(dy_, x_, a_major=1, b_major=1, out=tgt, accumulate=True)
@@ -271,13 +281,17 @@ class TransformerFn(torch.autograd.Function):
                 # LN + GEGLU backward inside the dgrad GEMM, dW2 / dg4 from dW2g = dxs^T hp - vsum
                 w2g, colvec, acc = ctx.ff_saved[L]
                 ctx.ff_saved[L] = None
-                dxs, vsum, ab = K.ff_bwd_prep(dx, st_v, acc, colvec)
+                dxs, vsum, ab = K.ff_bwd_prep(dx, st_v, acc, colvec)     # dxs / vsum: dW2 / dg4 only
                 du = K.ff_bwd(dx, w2g, u, st_v, ab)
-                dw2 = K.ff_w2_grad_post_(wg.wgrad(dxs, h), vsum, g4.detach(), w2.detach(), dg4)
-                tgt = _grad_target(w2)
-                if tgt is not None:
-                    tgt.add_(dw2)
-                    dw2 = None
+                dw2 = None
+                if wneed[base + 7] or wneed[base + 6]:     # dg4 comes out of dW2g as well
+                    dw2 = K.ff_w2_grad_post_(wg.wgrad(dxs, h), vsum, g4.detach(),
+                                             *((w2.detach(), dg4) if dg4 is not None else ()))
+                    tgt = _grad_target(w2) if wneed[base + 7] else None
+                    if tgt is not None:
+                        tgt.add_(dw2)
+                    if tgt is not None or not wneed[base + 7]:
+                        dw2 = None
                 grads[base + 7] = dw2
                 dh = None
             else:
@@ -354,12 +368,39 @@ class LinearFn(torch.autograd.Function):
         if dy.dtype != BF16:
             dy = dy.to(BF16)
         dx = K.gemm(dy, wb, b_major=1) if ctx.needs_input_grad[0] else None
-        dw = _wgrad(dy, x)
-        db = dy.float().sum(dim=0) if ctx.has_bias else None
+        dw = _wgrad(dy, x) if ctx.needs_input_grad[1] else None
+        db = dy.float().sum(dim=0) if ctx.has_bias and ctx.needs_input_grad[2] else None
         dt = None
-        if ctx.period is not None:
+        if ctx.period is not None and ctx.needs_input_grad[3]:
             dt = dy.float().view(-1, ctx.period, dy.shape[1]).sum(dim=0)
         return dx, dw, db, dt
+
+
+def _patch_embed_fwd(ctx, patches, index, weight, bias, table, keep_wb: bool):
+    wb = weight_bf16(weight)
+    tbl16 = K.cast_bf16(table.detach())
+    y = K.gemm(patches, wb, bias=bias.detach(), residual=tbl16, res_row_idx=index)
+    ctx.save_for_backward(patches, index)
+    ctx.wb = wb if keep_wb else None          # the dgrad operand, kept only when d patches is wanted
+    ctx.table_rows = table.shape[0]
+    return y
+
+
+def _patch_embed_bwd(ctx, dy, need_dp: bool, need_w: bool, need_b: bool, need_t: bool):
+    """(d patches f32, dW, d bias, d pos), each None unless asked for"""
+    patches, index = ctx.saved_tensors
+    dy = dy.contiguous()
+    if dy.dtype != BF16:
+        dy = dy.to(BF16)
+    dp = K.gemm(dy, ctx.wb, b_major=1, out_dtype=F32) if need_dp else None
+    dw = _wgrad(dy, patches) if need_w else None
+    db = K.colsum_rows_(torch.zeros(dy.shape[1], device=dy.device, dtype=F32), dy) if need_b else None
+    dt = None
+    if need_t:
+        dt = K.scatter_add_rows_(torch.zeros((ctx.table_rows, dy.shape[1]), device=dy.device, dtype=F32),
+                                 dy, idx=index)
+    ctx.wb = None
+    return dp, dw, db, dt
 
 
 class PatchEmbedFn(torch.autograd.Function):
@@ -368,29 +409,45 @@ class PatchEmbedFn(torch.autograd.Function):
 
     patches bf16 [B*k, patch_dim] come from K.patchify_gather (only the kept patches are read from
     the image); `index` int32 [B*k] is the patch index of every row = the row of the position table
-    the GEMM epilogue adds.  Backward: dW by the wgrad GEMM, d bias = column sums, d pos = rows of dy
-    scatter-added by `index`; the image needs no gradient."""
+    the GEMM epilogue adds.  Backward: d patches = dy @ W (f32 GEMM output; autograd hands it back in
+    the dtype of `patches`), dW by the wgrad GEMM, d bias = column sums, d pos = rows of dy
+    scatter-added by `index`; each only for inputs that need a gradient.  An image that wants a
+    gradient goes through PatchifyFn instead, which keeps d patches in f32 up to the pixels."""
 
     @staticmethod
     def forward(ctx, patches, index, weight, bias, table):
-        wb = weight_bf16(weight)
-        tbl16 = K.cast_bf16(table.detach())
-        y = K.gemm(patches, wb, bias=bias.detach(), residual=tbl16, res_row_idx=index)
-        ctx.save_for_backward(patches, index)
-        ctx.table_rows = table.shape[0]
-        return y
+        return _patch_embed_fwd(ctx, patches, index, weight, bias, table, ctx.needs_input_grad[0])
 
     @staticmethod
     def backward(ctx, dy):
-        patches, index = ctx.saved_tensors
-        dy = dy.contiguous()
-        if dy.dtype != BF16:
-            dy = dy.to(BF16)
-        dw = _wgrad(dy, patches)
-        db = K.colsum_rows_(torch.zeros(dy.shape[1], device=dy.device, dtype=F32), dy)
-        dt = K.scatter_add_rows_(torch.zeros((ctx.table_rows, dy.shape[1]), device=dy.device, dtype=F32),
-                                 dy, idx=index)
-        return None, None, dw, db, dt
+        n = ctx.needs_input_grad
+        dp, dw, db, dt = _patch_embed_bwd(ctx, dy, n[0], n[2], n[3], n[4])
+        return dp, None, dw, db, dt
+
+
+class PatchifyFn(torch.autograd.Function):
+    """tokens of an image that wants a gradient: patchify + PatchDropout selection (x_clip.py:356-359,
+    :134-151; forward K.patchify_gather) and the patch embedding of PatchEmbedFn in one Function.
+    Backward: d patches = dy @ W in f32, then K.patchify_scatter - the kept patches' rows go back to
+    their pixels, dropped patches get 0, as the reference's gather `x[batch_indices, keep]` gives.  One
+    Function, so that d patches reaches the scatter in f32 (autograd would round a gradient flowing
+    between two Functions to the bf16 of the patches).  once_differentiable: a double backward through
+    the image raises instead of returning zero curvature."""
+
+    @staticmethod
+    def forward(ctx, img, patch: int, keep, index, weight, bias, table):
+        patches = K.patchify_gather(img, patch, keep)
+        ctx.shape, ctx.patch, ctx.keep = tuple(img.shape), patch, keep
+        return _patch_embed_fwd(ctx, patches, index, weight, bias, table, ctx.needs_input_grad[0])
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dy):
+        n = ctx.needs_input_grad
+        dp, dw, db, dt = _patch_embed_bwd(ctx, dy, n[0], n[4], n[5], n[6])
+        dimg = K.patchify_scatter(dp, ctx.shape, ctx.patch, ctx.keep) if dp is not None else None
+        ctx.keep = None
+        return dimg, None, None, None, dw, db, dt
 
 
 class ProjectL2NormFn(torch.autograd.Function):
@@ -412,7 +469,7 @@ class ProjectL2NormFn(torch.autograd.Function):
         e, wb, z, inv = ctx.saved_tensors
         dp = K.l2norm_bwd(dz.contiguous().float(), z, inv)
         de = K.gemm(dp, wb, b_major=1) if ctx.needs_input_grad[0] else None
-        dw = _wgrad(dp, e)
+        dw = _wgrad(dp, e) if ctx.needs_input_grad[1] else None
         return de, dw
 
 
@@ -585,7 +642,10 @@ class ChunkedClipLossFn(torch.autograd.Function):
     the GPU's HBM holds (80 GB on an H100) (`retain`: "auto" measures the first chunk's footprint and plans against
     the free memory; an int fixes the count; 0 = none); only the remaining chunks are encoded
     without saving anything and re-encoded in step 3 (RNG replayed for PatchDropout).  Retained
-    chunks cost no extra flops; each re-encoded chunk costs one extra encoder forward."""
+    chunks cost no extra flops; each re-encoded chunk costs one extra encoder forward.
+    An image that wants a gradient enters every chunk's encoder as a detached per-chunk leaf; backward
+    collects the leaves' gradients into d loss / d image, so the outer graph (a generator, an
+    augmentation) is only ever entered by autograd itself, after this backward returns."""
 
     @staticmethod
     def forward(ctx, clip, text, image, text_mask, chunk, temperature, retain="auto"):
@@ -593,6 +653,14 @@ class ChunkedClipLossFn(torch.autograd.Function):
         dev = text.device
         bounds = [(s, min(s + chunk, B)) for s in range(0, B, chunk)]
         rng_states, zs, opss, kept = [], [], [], []
+        want_dimage = image.requires_grad
+        img_leaves = []                               # per retained chunk: its image leaf (or None)
+
+        def chunk_image(s, e):
+            if not want_dimage:
+                return image[s:e]
+            return image[s:e].detach().requires_grad_(True)
+
         foot = None                                   # bytes of one retained chunk's activations
         # "auto" plans ONCE per (batch, chunk size): the first step measures and decides, later steps
         # repeat its decision - the same tensors are then allocated in the same order every step, which
@@ -621,9 +689,10 @@ class ChunkedClipLossFn(torch.autograd.Function):
                 if keep_it:
                     before = torch.cuda.memory_allocated(dev)
                     z = ops = None
+                    img_k = chunk_image(s, e)
                     try:
                         with torch.enable_grad():
-                            z, ops = clip._encode_to_latents(text[s:e], image[s:e], text_mask[s:e])
+                            z, ops = clip._encode_to_latents(text[s:e], img_k, text_mask[s:e])
                     except torch.OutOfMemoryError:
                         # the plan was too optimistic (a fragmented cache, memory taken by someone else
                         # since the estimate): this chunk and all later ones are re-encoded in backward
@@ -635,19 +704,23 @@ class ChunkedClipLossFn(torch.autograd.Function):
                         torch.cuda.set_rng_state(rng_states[-1], dev)
                         z, ops = clip._encode_to_latents(text[s:e], image[s:e], text_mask[s:e])
                         kept.append(None)
+                        img_leaves.append(None)
                         zs.append(z)
                         opss.append(ops)
                         continue
                     kept.append(list(z))
+                    img_leaves.append(img_k if want_dimage else None)
                     if foot is None:
                         foot = max(torch.cuda.memory_allocated(dev) - before, 1)
                         if planned and len(bounds) > 1 and \
                                 _avail_bytes(dev) < foot * (1.0 + RETAIN_TRANSIENT_FRAC) + RETAIN_MARGIN_BYTES:
                             kept[-1] = None           # not even a second live chunk fits beside it: let it go
+                            img_leaves[-1] = None
                     z = [t.detach() for t in z]
                 else:
                     z, ops = clip._encode_to_latents(text[s:e], image[s:e], text_mask[s:e])
                     kept.append(None)
+                    img_leaves.append(None)
                 zs.append(z)
                 opss.append(ops)
         nsets = len(zs[0])
@@ -663,6 +736,7 @@ class ChunkedClipLossFn(torch.autograd.Function):
                 *((clip.sim_reg_loss_weight, 1.0) if clip.has_sim_reg_loss else ()))
         ctx.clip, ctx.inputs = clip, (text, image, text_mask)
         ctx.bounds, ctx.rng_states, ctx.kept = bounds, rng_states, kept
+        ctx.img_leaves = img_leaves if want_dimage else None
         ctx.graph = (loss, leaves, temp_leaf)
         ctx.weight_casts = wscope.cache
         n_kept = sum(z is not None for z in kept)
@@ -683,6 +757,7 @@ class ChunkedClipLossFn(torch.autograd.Function):
         dev = text.device
         keep_state = torch.cuda.get_rng_state(dev)
         kept = ctx.kept
+        dimage = torch.empty_like(image) if ctx.img_leaves is not None else None
         # retained chunks first: their backward releases HBM before any chunk is re-encoded
         order = [k for k in range(len(ctx.bounds)) if kept[k] is not None] + \
                 [k for k in range(len(ctx.bounds)) if kept[k] is None]
@@ -694,13 +769,25 @@ class ChunkedClipLossFn(torch.autograd.Function):
                 # the last one processed runs with the hooks deferred (the DDP no_sync convention)
                 with torch.enable_grad(), D_.defer_grad_sync(pos != len(order) - 1), \
                         _InPlaceGradAccumulation(INPLACE_GRAD_ACCUMULATION and pos != len(order) - 1):
+                    img_k = None
                     if kept[k] is not None:
                         z, kept[k] = kept[k], None
+                        if dimage is not None:
+                            img_k, ctx.img_leaves[k] = ctx.img_leaves[k], None
                     else:
                         torch.cuda.set_rng_state(ctx.rng_states[k], dev)
-                        z, _ = clip._encode_to_latents(text[s:e], image[s:e], text_mask[s:e])
+                        if dimage is not None:
+                            img_k = image[s:e].detach().requires_grad_(True)
+                        z, _ = clip._encode_to_latents(text[s:e], image[s:e] if img_k is None else img_k,
+                                                       text_mask[s:e])
                     torch.autograd.backward(list(z), [d[s:e] for d in dz])   # accumulates into .grad
                     del z
+                    if img_k is not None:
+                        if img_k.grad is None:
+                            dimage[s:e].zero_()
+                        else:
+                            dimage[s:e].copy_(img_k.grad)
+                        del img_k
         torch.cuda.set_rng_state(keep_state, dev)
-        ctx.graph = ctx.inputs = ctx.kept = ctx.weight_casts = None
-        return None, None, None, None, None, temp_leaf.grad, None
+        ctx.graph = ctx.inputs = ctx.kept = ctx.weight_casts = ctx.img_leaves = None
+        return None, None, dimage, None, None, temp_leaf.grad, None

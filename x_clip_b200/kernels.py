@@ -271,6 +271,27 @@ def patchify_gather(img, patch, keep=None):
     return out
 
 
+def patchify_scatter(src, image_shape, patch, keep=None):
+    """Inverse of patchify_gather (the image gradient): src f32 [B*k, patch*patch*C] rows in the
+    gather's order -> f32 [B,C,H,W]; pixels of patches not in keep[b, :] are 0.  The indices of one
+    sample must be distinct (xclip_patchify_scatter)."""
+    _need(src, F32, "src"); _rows2d(src, "src")
+    B, C, H, W = (int(s) for s in image_shape)
+    n = (H // patch) * (W // patch)
+    k = n if keep is None else keep.shape[1]
+    if keep is not None:
+        if keep.dtype != torch.int64 or keep.shape[0] != B or keep.device != src.device:
+            raise _lib.XClipB200Error("patchify_scatter: keep must be int64 [B, k] on src's device")
+        keep = keep.contiguous()
+    if src.shape[0] != B * k or src.shape[1] != patch * patch * C:
+        raise _lib.XClipB200Error(f"patchify_scatter: src must be [{B * k}, {patch * patch * C}], "
+                                  f"got {tuple(src.shape)}")
+    out = torch.empty((B, C, H, W), device=src.device, dtype=F32)
+    _call(src, "embed", 0.0, (B * k + B * n) * patch * patch * C * 4.0, "xclip_patchify_scatter",
+          src.data_ptr(), src.stride(0), B, C, H, W, int(patch), _ptr(keep), k, out.data_ptr())
+    return out
+
+
 def scatter_add_rows_(dst, src, idx=None, period=0):
     """dst f32 [V,d] rows idx[r] (int32) or r % period += src bf16 [rows,d]."""
     _need(src, BF16, "src"); _rows2d(src, "src"); _need(dst, F32, "dst")
