@@ -60,19 +60,29 @@ class ClipConfig:
 
 # --------------------------------------------------------------------------- blocks
 
+# The reference's precision rules: LayerNorm eps 1e-3 for any non-fp32 input (:118) and the attention
+# softmax in fp32 (:238).  tests/step_oracle.py pins them (PINNED_LN_EPS = 1e-5, SOFTMAX_FP32 = False)
+# to run these same functions as an fp64 reference of the fp32 step.  The defaults change nothing.
+PINNED_LN_EPS: Optional[float] = None
+SOFTMAX_FP32 = True
+
+
 def gain_layernorm(x: Tensor, g: Tensor) -> Tensor:
     """Gain-only LayerNorm, biased variance; eps 1e-5 for fp32 inputs (:112-121)."""
-    eps = 1e-5 if x.dtype == torch.float32 else 1e-3
+    if PINNED_LN_EPS is not None:
+        eps = PINNED_LN_EPS
+    else:
+        eps = 1e-5 if x.dtype == torch.float32 else 1e-3
     mu = x.mean(dim=-1, keepdim=True)
     var = ((x - mu) ** 2).mean(dim=-1, keepdim=True)
     return (x - mu) * torch.rsqrt(var + eps) * g
 
 
-def rotary_angles(n_pos: int, rot_dim: int) -> Tensor:
+def rotary_angles(n_pos: int, rot_dim: int, device=None) -> Tensor:
     """RotaryEmbedding(rot_dim)(n_pos) (:155-166): angle[pos, j] = pos / 10000^(2(j mod rot_dim/2)/rot_dim),
-    the half-table repeated twice along the feature axis -> [n_pos, rot_dim]."""
-    inv_freq = 1.0 / (10000 ** (torch.arange(0, rot_dim, 2).float() / rot_dim))
-    ang = torch.arange(n_pos).float()[:, None] * inv_freq[None, :]
+    the half-table repeated twice along the feature axis -> [n_pos, rot_dim] fp32 on `device`."""
+    inv_freq = 1.0 / (10000 ** (torch.arange(0, rot_dim, 2, device=device).float() / rot_dim))
+    ang = torch.arange(n_pos, device=device).float()[:, None] * inv_freq[None, :]
     return torch.cat([ang, ang], dim=-1)
 
 
@@ -106,7 +116,7 @@ def attention(x: Tensor, p: Params, prefix: str, heads: int, dim_head: int,
     if causal:
         future = torch.ones(n, n, dtype=torch.bool, device=x.device).triu(1)
         scores = scores.masked_fill(future, fill)
-    probs = torch.softmax(scores.float(), dim=-1).to(scores.dtype)
+    probs = torch.softmax(scores.float() if SOFTMAX_FP32 else scores, dim=-1).to(scores.dtype)
     ctx = (probs @ v).permute(0, 2, 1, 3).reshape(b, n, heads * dim_head)
     out = ctx @ p[prefix + "to_out.0.weight"].t()
     return gain_layernorm(out, p[prefix + "to_out.1.g"])
@@ -148,7 +158,7 @@ def encode_text(ids: Tensor, key_mask: Tensor, p: Params, cfg: ClipConfig) -> Te
     x = p["text_transformer.token_emb.weight"][ids]
     rotary = None
     if cfg.text_rotary_pos_emb:
-        rotary = rotary_angles(n + 1, min(cfg.text_dim_head, 32))
+        rotary = rotary_angles(n + 1, min(cfg.text_dim_head, 32), ids.device)
     else:
         x = x + p["text_transformer.abs_pos_emb.weight"][:n][None]
     mask = key_mask

@@ -79,6 +79,12 @@ def test_clip_matches_reference(cuda_device, case):
     gn = torch.sqrt(sum((g.double() ** 2).sum() for g in grads.values())).item()
     assert abs(gn - gold["grad_norm"]) <= 1e-2 * gold["grad_norm"], (gn, gold["grad_norm"])
 
+    # a gradient the GPU step never produces (or produces where the reference has none) is a failure
+    # of its own, before any per-parameter comparison below
+    def has_grad(g):
+        return g is not None and bool(g.ne(0).any())
+    assert {k for k, g in grads.items() if has_grad(g)} == {k for k, q in p.items() if has_grad(q.grad)}
+
     bad = []
     for k, g in grads.items():
         og = p[k].grad
