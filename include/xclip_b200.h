@@ -130,6 +130,22 @@ int xclip_attn_bwd(const void* qkv, int64_t ld_qkv, const uint8_t* key_mask, con
                    int64_t ldo, const void* d_o, int64_t lddo, const float* lse, float* delta,
                    void* dqkv, int64_t ld_dqkv, float* dq_workspace, int B, int n, int heads,
                    float scale, int causal, xclip_stream_t stream);
+/* The same attention with dropout on the softmax probabilities (x_clip.py:211, :241-243):
+ * P' = P M / (1 - p), o = P' v, and lse stays that of the undropped row.  Backward: dv = P'^T dO,
+ * dS = P (dO v^T M / (1 - p) - delta), delta = rowsum(dO o) as before.  Element (b, h, i, j) of
+ * `layer` is kept iff word j & 3 of Philox4x32-10 with counter (j >> 2, i, b * heads + h, layer) and
+ * key *seed (low word first) is below round((1 - p) 2^32).  The mask is a function of the element, so
+ * the backward given the same seed and layer sees the forward's mask, on either schedule.  seed is an
+ * 8-byte aligned device pointer (read by the kernels, no host sync); p in [0, 1] as fp32 (p = 1 gives
+ * o = 0 and zero gradients); layer >= 0.  Other arguments and refusals as xclip_attn_fwd / _bwd. */
+int xclip_attn_dropout_fwd(const void* qkv, int64_t ld_qkv, const uint8_t* key_mask, void* o,
+                           int64_t ldo, float* lse, int B, int n, int heads, float scale, int causal,
+                           float p, const uint64_t* seed, int layer, xclip_stream_t stream);
+int xclip_attn_dropout_bwd(const void* qkv, int64_t ld_qkv, const uint8_t* key_mask, const void* o,
+                           int64_t ldo, const void* d_o, int64_t lddo, const float* lse, float* delta,
+                           void* dqkv, int64_t ld_dqkv, int B, int n, int heads, float scale,
+                           int causal, float p, const uint64_t* seed, int layer,
+                           xclip_stream_t stream);
 
 /* ---- similarity + InfoNCE / DCL (wgmma, logits never materialised in forward) ------------
  * Replaces x_clip/x_clip.py:813-847 for one direction of the loss:

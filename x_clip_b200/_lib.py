@@ -58,6 +58,11 @@ SIGNATURES = {
     "xclip_attn_bwd": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_int64, c_void_p, c_int64,
                                c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_int, c_int,
                                c_int, c_float, c_int, c_void_p]),
+    "xclip_attn_dropout_fwd": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_int64, c_void_p, c_int,
+                                       c_int, c_int, c_float, c_int, c_float, c_void_p, c_int, c_void_p]),
+    "xclip_attn_dropout_bwd": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_int64, c_void_p, c_int64,
+                                       c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_float,
+                                       c_int, c_float, c_void_p, c_int, c_void_p]),
     "xclip_nce_num_col_blocks": (c_int, [c_int]),
     "xclip_nce_fwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int,
                               c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_void_p]),

@@ -16,8 +16,10 @@ attention width heads * 64 need not equal the model width.  Feature combinations
 cover raise at construction (never a silent CPU or eager fallback): dim_head != 64, model or latent
 widths that are not 128 * {1..8}, a causal text tower longer than
 128 tokens, rotary + causal together (broken in the reference itself: n+1 angles for n tokens,
-x_clip.py:328), dropout > 0 and conv-downsampled image latents.  MLM, SimSiam / SimCLR and the
-multiview term run through the fast encoders (aux.py).  The similarity-regularisation term
+x_clip.py:328) and conv-downsampled image latents.  Attention dropout (`attn_dropout`, 0 <= p <= 1)
+runs inside the attention kernels, with a counter-based mask that a re-encode regenerates exactly
+(engine.TransformerDropoutFn); `ff_dropout` is accepted and, as in the reference's Transformer
+(x_clip.py:268), not applied.  MLM, SimSiam / SimCLR and the multiview term run through the fast encoders (aux.py).  The similarity-regularisation term
 (`sim_reg_loss_weight > 0`) runs fused with the contrastive loss (engine.ContrastiveLossFn) where the
 reference itself runs it: with `extra_latent_projection=True`, without FILIP and with a single view;
 the other combinations fail inside the reference (x_clip.py:779) and raise `Unsupported` here.
@@ -73,13 +75,15 @@ class Attention(nn.Module):
                  dropout: float = 0.):
         super().__init__()
         _require(dim_head == 64, f"dim_head must be 64, got {dim_head}")
-        _require(dropout == 0., "attention dropout > 0 is not implemented")
         self.heads = heads
         self.causal = causal
         self.scale = dim_head ** -0.5
         inner = dim_head * heads
         self.to_qkv = nn.Linear(dim, inner * 3, bias=False)
         self.to_out = nn.Sequential(nn.Linear(inner, dim, bias=False), LayerNorm(dim))
+        # parameter-free, as in the reference (:211): holds p (range-checked by nn.Dropout) and follows
+        # train() / eval(); the dropout itself runs in the attention kernels
+        self.dropout = nn.Dropout(dropout)
 
 
 class FeedForward(nn.Module):
@@ -98,7 +102,13 @@ class FeedForward(nn.Module):
 
 
 class Transformer(nn.Module):
-    """norm_in -> depth x (attention, feed-forward) -> norm_out, executed by engine.TransformerFn."""
+    """norm_in -> depth x (attention, feed-forward) -> norm_out, executed by engine.TransformerFn.
+
+    Attention dropout is active, as nn.Dropout is, iff the layer's `dropout` module is in training mode
+    and its p > 0, under no_grad as well; it then runs engine.TransformerDropoutFn with one 64-bit seed
+    per call, drawn from the CUDA generator of the input's device (so torch.manual_seed governs the
+    masks).  `forced_dropout_seed` (an int) pins that seed for tests.  `ff_dropout` is accepted and not
+    applied: the reference's Transformer never hands it to its FeedForward (x_clip.py:268)."""
 
     def __init__(self, dim: int, *, depth: int, dim_head: int = 64, heads: int = 8,
                  causal: bool = False, attn_dropout: float = 0., ff_dropout: float = 0.,
@@ -114,11 +124,12 @@ class Transformer(nn.Module):
             nn.ModuleList([
                 PreNorm(dim, Attention(dim, dim_head=dim_head, heads=heads, causal=causal,
                                        dropout=attn_dropout)),
-                PreNorm(dim, FeedForward(dim, mult=ff_mult, dropout=ff_dropout)),
+                PreNorm(dim, FeedForward(dim, mult=ff_mult)),
             ]) for _ in range(depth)
         ])
         self.norm_in = LayerNorm(dim)
         self.norm_out = LayerNorm(dim)
+        self.forced_dropout_seed: Optional[int] = None
 
     def flat_weights(self):
         w = [self.norm_in.g, self.norm_out.g]
@@ -139,8 +150,20 @@ class Transformer(nn.Module):
                      f"rotary table must be [n, 32] (dim_head 64 -> rot dim 32), got {tuple(rotary_pos_emb.shape)}")
             ang = rotary_pos_emb[:, :16].to(device=x.device, dtype=torch.float32)
             cos, sin = ang.cos().contiguous(), ang.sin().contiguous()
+        ps = tuple(float(attn.fn.dropout.p) if attn.fn.dropout.training else 0.0 for attn, _ in self.layers)
+        if any(p > 0.0 for p in ps):
+            return E.TransformerDropoutFn.apply(x, mask, self.heads, self.depth, self.causal, cos, sin,
+                                                torch.is_grad_enabled(), (ps, self.dropout_seed(x.device)),
+                                                *self.flat_weights())
         return E.TransformerFn.apply(x, mask, self.heads, self.depth, self.causal, cos, sin,
                                      torch.is_grad_enabled(), *self.flat_weights())
+
+    def dropout_seed(self, device) -> torch.Tensor:
+        """int64 [1] on `device`: the Philox key of this call's attention-dropout masks, drawn from the
+        device's CUDA generator without a host sync, or `forced_dropout_seed`."""
+        if self.forced_dropout_seed is not None:
+            return torch.tensor([self.forced_dropout_seed], dtype=torch.int64, device=device)
+        return torch.randint(-2 ** 63, 2 ** 63 - 1, (1,), dtype=torch.int64, device=device)
 
 
 class PatchDropout(nn.Module):

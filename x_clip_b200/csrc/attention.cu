@@ -23,8 +23,12 @@
 // The backward kernels read such a row's lse as +inf, so the block bodies give it p = 0 everywhere
 // (on every other row a hidden score already has p = 0 exactly, hence ds = 0), and the dK / dV
 // kernels add its dO / n to dv after the key loop (attn_dv_empty_rows).
+// Every kernel is also instantiated with kDropout (xclip_attn_dropout_*): the block bodies then drop
+// probabilities with a Philox mask that is a function of the element alone (see AttnDrop); the
+// kDropout = false instantiations are the plain kernels.
 #include "common.cuh"
 #include "host.h"
+#include "philox.cuh"
 
 namespace xclip {
 
@@ -189,18 +193,137 @@ __device__ __forceinline__ void attn_dv_empty_rows(float (&dv)[8][4], const bf16
     }
 }
 
+// ---- attention dropout (DESIGN.md, Dropout) ------------------------------------------------------
+// Element (b, h, i, j) of layer L is kept iff word j & 3 of philox4x32_10((j >> 2, i, b H + h, L), seed)
+// is <= keep_le, so the mask is a function of the element alone: every schedule and block order
+// draws the same one.  A kept p is scaled by inv_keep = 1 / (1 - p) before it meets V or dP.
+struct AttnDrop {
+  const uint64_t* seed;   // the 64-bit Philox key, read on the device (low word first)
+  uint32_t keep_le;       // round((1 - p) 2^32) - 1, saturated at 2^32 - 1
+  float inv_keep;         // 1 / (1 - p); 0 at p = 1, which drops every element
+  uint32_t layer;
+};
+
+// what a thread of a dropout kernel needs: the kernel's AttnDrop (read from the parameter bank where
+// used, so that it holds no registers through the block loops), the counter's b H + h word and the
+// warp's 32-word staging area for one block's mask bits
+struct DropCtx {
+  const AttnDrop& d;
+  uint32_t bh;
+  uint32_t* bits;
+};
+
+template <bool kDropout>
+__device__ __forceinline__ DropCtx drop_ctx(const AttnDrop& d, long long bh) {
+  if constexpr (kDropout) {
+    __shared__ uint32_t bits[kAttnThreads];   // 512 B, in the dropout kernels only
+    return DropCtx{d, (uint32_t)bh, bits + (threadIdx.x & ~31)};
+  } else {
+    return DropCtx{d, 0u, nullptr};
+  }
+}
+
+// the Philox key: the seed, re-read (an L1 hit) by every block instead of held in registers
+__device__ __forceinline__ uint2 drop_key(const DropCtx& dc) {
+  const unsigned long long s = __ldg(reinterpret_cast<const unsigned long long*>(dc.d.seed));
+  return make_uint2((uint32_t)s, (uint32_t)(s >> 32));
+}
+
+__device__ __forceinline__ uint32_t drop_keep4(uint4 w, uint32_t le) {
+  return (uint32_t)(w.x <= le) | ((uint32_t)(w.y <= le) << 1) | ((uint32_t)(w.z <= le) << 2) |
+         ((uint32_t)(w.w <= le) << 3);
+}
+
+// Mask bits of the warp's 16 rows [i0, i0 + 16) x 64 keys [j0, j0 + 64) (forward and dQ blocks):
+// word 2 r + h holds keys j0 + 32 h + [0, 32) of row i0 + r.  8 Philox calls per lane, none wasted.
+__device__ __forceinline__ void drop_bits_rows(const DropCtx& dc, int i0, int j0) {
+  const int lane = threadIdx.x & 31;
+  const uint32_t jg = (uint32_t)(j0 + (lane & 1) * 32) >> 2, i = (uint32_t)(i0 + (lane >> 1));
+  const uint2 key = drop_key(dc);
+  uint32_t w = 0;
+#pragma unroll
+  for (int g = 0; g < 8; ++g)
+    w |= drop_keep4(philox4x32_10(make_uint4(jg + g, i, dc.bh, dc.d.layer), key), dc.d.keep_le) << (4 * g);
+  __syncwarp();   // every lane has read the previous block's bits
+  dc.bits[lane] = w;
+  __syncwarp();
+}
+// row hh (0: lane / 4, 1: lane / 4 + 8) of the warp's 16, key nt * 8 + 2 (lane & 3) + e1 of the block
+__device__ __forceinline__ float drop_mul_rows(const DropCtx& dc, int hh, int nt, int e1) {
+  const int lane = threadIdx.x & 31;
+  const uint32_t w = dc.bits[((lane >> 2) + 8 * hh) * 2 + (nt >> 2)];
+  return (w >> ((nt & 3) * 8 + 2 * (lane & 3) + e1)) & 1u ? dc.d.inv_keep : 0.f;
+}
+
+// Mask bits of the warp's 16 keys [j0, j0 + 16) x 64 rows [i0, i0 + 64) (dK / dV blocks): word m holds
+// row i0 + 2 m in bits 0..15 and row i0 + 2 m + 1 in bits 16..31, bit = key - j0.
+__device__ __forceinline__ void drop_bits_keys(const DropCtx& dc, int j0, int i0) {
+  const int lane = threadIdx.x & 31;
+  const uint32_t jg = (uint32_t)j0 >> 2;
+  const uint2 key = drop_key(dc);
+  uint32_t w = 0;
+#pragma unroll
+  for (int r = 0; r < 2; ++r)
+#pragma unroll
+    for (int g = 0; g < 4; ++g)
+      w |= drop_keep4(philox4x32_10(make_uint4(jg + g, (uint32_t)(i0 + 2 * lane + r), dc.bh, dc.d.layer), key),
+                      dc.d.keep_le) << (16 * r + 4 * g);
+  __syncwarp();
+  dc.bits[lane] = w;
+  __syncwarp();
+}
+// row nt * 8 + 2 (lane & 3) + e1 of the block, key hh (0: lane / 4, 1: lane / 4 + 8) of the warp's 16
+__device__ __forceinline__ float drop_mul_keys(const DropCtx& dc, int hh, int nt, int e1) {
+  const int lane = threadIdx.x & 31;
+  const uint32_t w = dc.bits[nt * 4 + (lane & 3)];
+  return (w >> (16 * e1 + (lane >> 2) + 8 * hh)) & 1u ? dc.d.inv_keep : 0.f;
+}
+
+// attn_dv_empty_rows under dropout: the uniform p = 1/n of a row with no visible key is dropped per
+// key like any other p, so row i adds M_ij inv_keep dO_i / n to the dv of key j (one Philox call per
+// row and key; such rows are the rare left padding of a causal caption or a wholly masked item).
+__device__ __forceinline__ void attn_dv_empty_rows_drop(float (&dv)[8][4], const bf16* dO, long long lddo,
+                                                        const float* lse_bh, int n, const int (&key)[2],
+                                                        const DropCtx& dc) {
+  const int lane = threadIdx.x & 31;
+  const float w = dc.d.inv_keep / (float)n;
+  const uint2 k = drop_key(dc);
+  for (int i = 0; i < n; ++i) {
+    if (lse_bh[i] != -FLT_MAX) continue;
+    float mk[2];
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const uint4 r = philox4x32_10(make_uint4((uint32_t)key[hh] >> 2, (uint32_t)i, dc.bh, dc.d.layer), k);
+      const int c = key[hh] & 3;
+      const uint32_t word = c == 0 ? r.x : c == 1 ? r.y : c == 2 ? r.z : r.w;
+      mk[hh] = word <= dc.d.keep_le ? w : 0.f;
+    }
+    const bf16* g = dO + (long long)i * lddo + 2 * (lane & 3);
+#pragma unroll
+    for (int nt = 0; nt < 8; ++nt) {
+      const float2 x = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(g + nt * 8));
+      dv[nt][0] += mk[0] * x.x;
+      dv[nt][1] += mk[0] * x.y;
+      dv[nt][2] += mk[1] * x.x;
+      dv[nt][3] += mk[1] * x.y;
+    }
+  }
+}
+
 // ---- per-block bodies, shared by the resident and the streaming kernels ---------------------------
 // Each processes one 64-row block of the streamed operand for the warp's 16 rows.  The block's tiles
 // sit at rows [c0, c0 + 64) of tK / tV (tQ / tdO); kb (qb) is the block's first global row and
 // flags[j] (lse_b[j], delta_b[j]) belong to global row kb + j (qb + j).
 
-// forward: s = q k^T, online-softmax update of (m, l, oacc), oacc += p v
-template <bool kCausal>
+// forward: s = q k^T, online-softmax update of (m, l, oacc), oacc += p v.  Under dropout l sums the
+// undropped p (the lse is that of the whole row) and oacc takes p M / (1 - p).
+template <bool kCausal, bool kDropout>
 __device__ __forceinline__ void attn_fwd_block(const uint32_t (&qf)[4][4], const uint8_t* tK, const uint8_t* tV,
                                                int c0, const uint8_t* flags, int kb, const int (&row)[2],
                                                float scale_log2, float (&m)[2], float (&l)[2],
-                                               float (&oacc)[8][4]) {
+                                               float (&oacc)[8][4], const DropCtx& dc) {
   const int lane = threadIdx.x & 31;
+  if constexpr (kDropout) drop_bits_rows(dc, row[0] - (lane >> 2), kb);
   float s[8][4];
   zero_acc(s);
   mma_abt(s, qf, tK, c0);
@@ -233,7 +356,11 @@ __device__ __forceinline__ void attn_fwd_block(const uint32_t (&qf)[4][4], const
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
       const float pv = exp2f(s[nt][e] - m[e >> 1]);
-      s[nt][e] = pv;
+      if constexpr (kDropout) {
+        s[nt][e] = pv * drop_mul_rows(dc, e >> 1, nt, e & 1);
+      } else {
+        s[nt][e] = pv;
+      }
       l[e >> 1] += pv;
     }
   uint32_t pf[4][4];
@@ -266,13 +393,16 @@ __device__ __forceinline__ void attn_fwd_finish(float (&oacc)[8][4], const float
 
 // dK / dV: the warp's accumulators are S^T / dP^T (keys x queries), so P^T and dS^T feed the next
 // MMAs straight from registers.  key[] are the thread's two global key rows, flag[] their flags.
-template <bool kCausal>
+// Under dropout dv takes (P M / (1 - p))^T dO and ds = p (dp M / (1 - p) - delta).
+template <bool kCausal, bool kDropout>
 __device__ __forceinline__ void attn_dkdv_block(const uint32_t (&kf)[4][4], const uint32_t (&vf)[4][4],
                                                 const uint8_t* tQ, const uint8_t* tdO, int c0,
                                                 const float* lse_b, const float* delta_b, int qb,
                                                 const int (&key)[2], const int (&flag)[2], int n,
-                                                float scale_log2, float (&dk)[8][4], float (&dv)[8][4]) {
+                                                float scale_log2, float (&dk)[8][4], float (&dv)[8][4],
+                                                const DropCtx& dc) {
   const int lane = threadIdx.x & 31;
+  if constexpr (kDropout) drop_bits_keys(dc, key[0] - (lane >> 2), qb);
   float st[8][4], dpt[8][4];
   zero_acc(st);
   zero_acc(dpt);
@@ -286,8 +416,14 @@ __device__ __forceinline__ void attn_dkdv_block(const uint32_t (&kf)[4][4], cons
       const int q = qb + j;
       const float t = q < n ? attn_t(st[nt][e], scale_log2, flag[e >> 1], kCausal && key[e >> 1] > q) : -INFINITY;
       const float pv = exp2f(t - lse_b[j]);
-      st[nt][e] = pv;
-      dpt[nt][e] = pv * (dpt[nt][e] - delta_b[j]);
+      if constexpr (kDropout) {
+        const float mul = drop_mul_keys(dc, e >> 1, nt, e & 1);
+        st[nt][e] = pv * mul;
+        dpt[nt][e] = pv * (dpt[nt][e] * mul - delta_b[j]);
+      } else {
+        st[nt][e] = pv;
+        dpt[nt][e] = pv * (dpt[nt][e] - delta_b[j]);
+      }
     }
   uint32_t pf[4][4], df[4][4];
   acc_to_a(st, pf);
@@ -296,14 +432,16 @@ __device__ __forceinline__ void attn_dkdv_block(const uint32_t (&kf)[4][4], cons
   mma_ab(dk, df, tQ, c0);
 }
 
-// dQ: ds = p (dp - delta) over one block of keys, dq += ds k (a hidden score has p = 0, so ds = 0)
-template <bool kCausal>
+// dQ: ds = p (dp - delta) over one block of keys, dq += ds k (a hidden score has p = 0, so ds = 0);
+// under dropout dp is scaled by M / (1 - p) first
+template <bool kCausal, bool kDropout>
 __device__ __forceinline__ void attn_dq_block(const uint32_t (&qf)[4][4], const uint32_t (&of)[4][4],
                                               const uint8_t* tK, const uint8_t* tV, int c0,
                                               const uint8_t* flags, int kb, const int (&row)[2], int n,
                                               const float (&lr)[2], const float (&dr)[2], float scale_log2,
-                                              float (&dq)[8][4]) {
+                                              float (&dq)[8][4], const DropCtx& dc) {
   const int lane = threadIdx.x & 31;
+  if constexpr (kDropout) drop_bits_rows(dc, row[0] - (lane >> 2), kb);
   float s[8][4], dp[8][4];
   zero_acc(s);
   zero_acc(dp);
@@ -316,7 +454,11 @@ __device__ __forceinline__ void attn_dq_block(const uint32_t (&qf)[4][4], const 
       const int j = nt * 8 + 2 * (lane & 3) + (e & 1);
       const float t = attn_t(s[nt][e], scale_log2, flags[j], kCausal && kb + j > row[e >> 1]);
       const float pv = row[e >> 1] < n ? exp2f(t - lr[e >> 1]) : 0.f;
-      s[nt][e] = pv * (dp[nt][e] - dr[e >> 1]);
+      if constexpr (kDropout) {
+        s[nt][e] = pv * (dp[nt][e] * drop_mul_rows(dc, e >> 1, nt, e & 1) - dr[e >> 1]);
+      } else {
+        s[nt][e] = pv * (dp[nt][e] - dr[e >> 1]);
+      }
     }
   uint32_t df[4][4];
   acc_to_a(s, df);
@@ -325,10 +467,10 @@ __device__ __forceinline__ void attn_dq_block(const uint32_t (&qf)[4][4], const 
 
 // ---- forward ------------------------------------------------------------------------------------
 // resident: the head's whole K, V and key flags in shared memory
-template <bool kCausal>
+template <bool kCausal, bool kDropout>
 __global__ void __launch_bounds__(kAttnThreads)
 attn_fwd_kernel(const bf16* __restrict__ qkv, long long ld, const uint8_t* __restrict__ mask,
-                bf16* __restrict__ o, long long ldo, float* __restrict__ lse, int n, int H, float scale_log2) {
+                bf16* __restrict__ o, long long ldo, float* __restrict__ lse, int n, int H, float scale_log2, AttnDrop drop) {
   extern __shared__ __align__(128) uint8_t sm[];
   const int NP = (n + 63) & ~63;
   uint8_t* sQ = sm;
@@ -348,6 +490,7 @@ attn_fwd_kernel(const bf16* __restrict__ qkv, long long ld, const uint8_t* __res
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int r0 = warp * 16;
+  const DropCtx dc = drop_ctx<kDropout>(drop, (long long)b * H + h);
   uint32_t qf[4][4];
   load_a_frags(sQ, r0, qf);
   const int row[2] = {q0 + r0 + (lane >> 2), q0 + r0 + (lane >> 2) + 8};
@@ -355,18 +498,18 @@ attn_fwd_kernel(const bf16* __restrict__ qkv, long long ld, const uint8_t* __res
   float oacc[8][4];
   zero_acc(oacc);
   for (int kb = 0; kb < NP; kb += 64)
-    attn_fwd_block<kCausal>(qf, sK, sV, kb, sFlag + kb, kb, row, scale_log2, m, l, oacc);
+    attn_fwd_block<kCausal, kDropout>(qf, sK, sV, kb, sFlag + kb, kb, row, scale_log2, m, l, oacc, dc);
   attn_fwd_finish(oacc, m, l, row, o + (long long)b * n * ldo + h * kAttnDh, ldo, q0 + r0,
                   lse + ((long long)b * H + h) * n, n);
 }
 
 // streaming: the CTA's Q block stays; K, V and key flags of 64-key block i + 1 are fetched into the
 // other ring stage while block i is computed (flags through a register, K and V by cp.async)
-template <bool kCausal>
+template <bool kCausal, bool kDropout>
 __global__ void __launch_bounds__(kAttnThreads)
 attn_fwd_stream_kernel(const bf16* __restrict__ qkv, long long ld, const uint8_t* __restrict__ mask,
                        bf16* __restrict__ o, long long ldo, float* __restrict__ lse, int n, int H,
-                       float scale_log2) {
+                       float scale_log2, AttnDrop drop) {
   extern __shared__ __align__(128) uint8_t sm[];
   uint8_t* sQ = sm;
   uint8_t* ring = sQ + kAttnTile;            // stage s: K tile at ring + 2 s kAttnTile, V tile after it
@@ -386,6 +529,7 @@ attn_fwd_stream_kernel(const bf16* __restrict__ qkv, long long ld, const uint8_t
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int r0 = warp * 16;
+  const DropCtx dc = drop_ctx<kDropout>(drop, (long long)b * H + h);
   uint32_t qf[4][4];
   load_a_frags(sQ, r0, qf);
   const int row[2] = {q0 + r0 + (lane >> 2), q0 + r0 + (lane >> 2) + 8};
@@ -402,8 +546,8 @@ attn_fwd_stream_kernel(const bf16* __restrict__ qkv, long long ld, const uint8_t
       if (threadIdx.x < kAttnRows) next_flag = key_flag(mask, b, n, kb + kAttnRows + threadIdx.x);
     }
     const uint8_t* cur = ring + (i & 1) * 2 * kAttnTile;
-    attn_fwd_block<kCausal>(qf, cur, cur + kAttnTile, 0, sFlag + (i & 1) * kAttnRows, kb, row, scale_log2,
-                            m, l, oacc);
+    attn_fwd_block<kCausal, kDropout>(qf, cur, cur + kAttnTile, 0, sFlag + (i & 1) * kAttnRows, kb, row, scale_log2,
+                            m, l, oacc, dc);
     if (more && threadIdx.x < kAttnRows) sFlag[nxt * kAttnRows + threadIdx.x] = next_flag;
     cp_async_wait_all();   // block i + 1 landed, and no thread reads stage i & 1 any more
     __syncthreads();
@@ -450,12 +594,12 @@ attn_delta_kernel(const bf16* __restrict__ o, long long ldo, const bf16* __restr
 // ---- backward -----------------------------------------------------------------------------------
 // dK, dV of the 64 keys [k0, k0 + 64) of one (batch, head): loops over all queries.
 // resident: the head's whole Q, dO, lse and delta in shared memory
-template <bool kCausal>
+template <bool kCausal, bool kDropout>
 __global__ void __launch_bounds__(kAttnThreads)
 attn_bwd_dkdv_kernel(const bf16* __restrict__ qkv, long long ld, const uint8_t* __restrict__ mask,
                      const bf16* __restrict__ d_o, long long lddo, const float* __restrict__ lse,
                      const float* __restrict__ delta, bf16* __restrict__ dqkv, long long ldd, int n, int H,
-                     float scale, float scale_log2) {
+                     float scale, float scale_log2, AttnDrop drop) {
   extern __shared__ __align__(128) uint8_t sm[];
   const int NP = (n + 63) & ~63;
   uint8_t* sK = sm;
@@ -487,6 +631,7 @@ attn_bwd_dkdv_kernel(const bf16* __restrict__ qkv, long long ld, const uint8_t* 
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int r0 = warp * 16;
+  const DropCtx dc = drop_ctx<kDropout>(drop, (long long)b * H + h);
   uint32_t kf[4][4], vf[4][4];
   load_a_frags(sK, r0, kf);
   load_a_frags(sV, r0, vf);
@@ -497,10 +642,14 @@ attn_bwd_dkdv_kernel(const bf16* __restrict__ qkv, long long ld, const uint8_t* 
   zero_acc(dk);
   zero_acc(dv);
   for (int qb = 0; qb < NP; qb += 64)
-    attn_dkdv_block<kCausal>(kf, vf, sQ, sdO, qb, sLse + qb, sDelta + qb, qb, key, flag, n, scale_log2, dk, dv);
-  if (any_empty)
-    attn_dv_empty_rows(dv, d_o + (long long)b * n * lddo + h * kAttnDh, lddo, lse + bh * n, n,
-                       reinterpret_cast<float*>(sK));
+    attn_dkdv_block<kCausal, kDropout>(kf, vf, sQ, sdO, qb, sLse + qb, sDelta + qb, qb, key, flag, n, scale_log2, dk, dv, dc);
+  if (any_empty) {
+    if constexpr (kDropout)
+      attn_dv_empty_rows_drop(dv, d_o + (long long)b * n * lddo + h * kAttnDh, lddo, lse + bh * n, n, key, dc);
+    else
+      attn_dv_empty_rows(dv, d_o + (long long)b * n * lddo + h * kAttnDh, lddo, lse + bh * n, n,
+                         reinterpret_cast<float*>(sK));
+  }
   bf16* out = dqkv + (long long)b * n * ldd;
   store_rows(out + (H + h) * kAttnDh, ldd, k0 + r0, n, dk, scale);
   store_rows(out + (2 * H + h) * kAttnDh, ldd, k0 + r0, n, dv, 1.f);
@@ -508,12 +657,12 @@ attn_bwd_dkdv_kernel(const bf16* __restrict__ qkv, long long ld, const uint8_t* 
 
 // streaming: the CTA's K, V block stays; Q, dO (cp.async) and the 64 lse / delta values (through a
 // register) of query block i + 1 are fetched into the other ring stage while block i is computed
-template <bool kCausal>
+template <bool kCausal, bool kDropout>
 __global__ void __launch_bounds__(kAttnThreads)
 attn_bwd_dkdv_stream_kernel(const bf16* __restrict__ qkv, long long ld, const uint8_t* __restrict__ mask,
                             const bf16* __restrict__ d_o, long long lddo, const float* __restrict__ lse,
                             const float* __restrict__ delta, bf16* __restrict__ dqkv, long long ldd, int n,
-                            int H, float scale, float scale_log2) {
+                            int H, float scale, float scale_log2, AttnDrop drop) {
   extern __shared__ __align__(128) uint8_t sm[];
   uint8_t* sK = sm;
   uint8_t* sV = sK + kAttnTile;
@@ -544,6 +693,7 @@ attn_bwd_dkdv_stream_kernel(const bf16* __restrict__ qkv, long long ld, const ui
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int r0 = warp * 16;
+  const DropCtx dc = drop_ctx<kDropout>(drop, (long long)b * H + h);
   uint32_t kf[4][4], vf[4][4];
   load_a_frags(sK, r0, kf);
   load_a_frags(sV, r0, vf);
@@ -569,14 +719,18 @@ attn_bwd_dkdv_stream_kernel(const bf16* __restrict__ qkv, long long ld, const ui
     }
     const uint8_t* cur = ring + (i & 1) * 2 * kAttnTile;
     const float* st = sStat + (i & 1) * 2 * kAttnRows;
-    attn_dkdv_block<kCausal>(kf, vf, cur, cur + kAttnTile, 0, st, st + kAttnRows, qb, key, flag, n, scale_log2,
-                             dk, dv);
+    attn_dkdv_block<kCausal, kDropout>(kf, vf, cur, cur + kAttnTile, 0, st, st + kAttnRows, qb, key, flag, n, scale_log2,
+                             dk, dv, dc);
     if (more) sStat[nxt * 2 * kAttnRows + threadIdx.x] = next_stat;
     cp_async_wait_all();   // block i + 1 landed, and no thread reads stage i & 1 any more
     __syncthreads();
   }
-  if (__syncthreads_or(empty))
-    attn_dv_empty_rows(dv, gdO, lddo, lse + bh * n, n, reinterpret_cast<float*>(sK));
+  if (__syncthreads_or(empty)) {
+    if constexpr (kDropout)
+      attn_dv_empty_rows_drop(dv, gdO, lddo, lse + bh * n, n, key, dc);
+    else
+      attn_dv_empty_rows(dv, gdO, lddo, lse + bh * n, n, reinterpret_cast<float*>(sK));
+  }
   bf16* out = dqkv + (long long)b * n * ldd;
   store_rows(out + (H + h) * kAttnDh, ldd, k0 + r0, n, dk, scale);
   store_rows(out + (2 * H + h) * kAttnDh, ldd, k0 + r0, n, dv, 1.f);
@@ -584,12 +738,12 @@ attn_bwd_dkdv_stream_kernel(const bf16* __restrict__ qkv, long long ld, const ui
 
 // dQ of the 64 queries [q0, q0 + 64) of one (batch, head): loops over all keys.
 // resident: the head's whole K, V and key flags in shared memory
-template <bool kCausal>
+template <bool kCausal, bool kDropout>
 __global__ void __launch_bounds__(kAttnThreads)
 attn_bwd_dq_kernel(const bf16* __restrict__ qkv, long long ld, const uint8_t* __restrict__ mask,
                    const bf16* __restrict__ d_o, long long lddo, const float* __restrict__ lse,
                    const float* __restrict__ delta, bf16* __restrict__ dqkv, long long ldd, int n, int H,
-                   float scale, float scale_log2) {
+                   float scale, float scale_log2, AttnDrop drop) {
   extern __shared__ __align__(128) uint8_t sm[];
   const int NP = (n + 63) & ~63;
   uint8_t* sQ = sm;
@@ -611,6 +765,7 @@ attn_bwd_dq_kernel(const bf16* __restrict__ qkv, long long ld, const uint8_t* __
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int r0 = warp * 16;
+  const DropCtx dc = drop_ctx<kDropout>(drop, (long long)b * H + h);
   uint32_t qf[4][4], of[4][4];
   load_a_frags(sQ, r0, qf);
   load_a_frags(sdO, r0, of);
@@ -625,18 +780,18 @@ attn_bwd_dq_kernel(const bf16* __restrict__ qkv, long long ld, const uint8_t* __
   float dq[8][4];
   zero_acc(dq);
   for (int kb = 0; kb < NP; kb += 64)
-    attn_dq_block<kCausal>(qf, of, sK, sV, kb, sFlag + kb, kb, row, n, lr, dr, scale_log2, dq);
+    attn_dq_block<kCausal, kDropout>(qf, of, sK, sV, kb, sFlag + kb, kb, row, n, lr, dr, scale_log2, dq, dc);
   store_rows(dqkv + (long long)b * n * ldd + h * kAttnDh, ldd, q0 + r0, n, dq, scale);
 }
 
 // streaming: the CTA's Q, dO block stays; K, V and key flags of 64-key block i + 1 are fetched into
 // the other ring stage while block i is computed
-template <bool kCausal>
+template <bool kCausal, bool kDropout>
 __global__ void __launch_bounds__(kAttnThreads)
 attn_bwd_dq_stream_kernel(const bf16* __restrict__ qkv, long long ld, const uint8_t* __restrict__ mask,
                           const bf16* __restrict__ d_o, long long lddo, const float* __restrict__ lse,
                           const float* __restrict__ delta, bf16* __restrict__ dqkv, long long ldd, int n,
-                          int H, float scale, float scale_log2) {
+                          int H, float scale, float scale_log2, AttnDrop drop) {
   extern __shared__ __align__(128) uint8_t sm[];
   uint8_t* sQ = sm;
   uint8_t* sdO = sQ + kAttnTile;
@@ -658,6 +813,7 @@ attn_bwd_dq_stream_kernel(const bf16* __restrict__ qkv, long long ld, const uint
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int r0 = warp * 16;
+  const DropCtx dc = drop_ctx<kDropout>(drop, (long long)b * H + h);
   uint32_t qf[4][4], of[4][4];
   load_a_frags(sQ, r0, qf);
   load_a_frags(sdO, r0, of);
@@ -681,8 +837,8 @@ attn_bwd_dq_stream_kernel(const bf16* __restrict__ qkv, long long ld, const uint
       if (threadIdx.x < kAttnRows) next_flag = key_flag(mask, b, n, kb + kAttnRows + threadIdx.x);
     }
     const uint8_t* cur = ring + (i & 1) * 2 * kAttnTile;
-    attn_dq_block<kCausal>(qf, of, cur, cur + kAttnTile, 0, sFlag + (i & 1) * kAttnRows, kb, row, n, lr, dr,
-                           scale_log2, dq);
+    attn_dq_block<kCausal, kDropout>(qf, of, cur, cur + kAttnTile, 0, sFlag + (i & 1) * kAttnRows, kb, row, n, lr, dr,
+                           scale_log2, dq, dc);
     if (more && threadIdx.x < kAttnRows) sFlag[nxt * kAttnRows + threadIdx.x] = next_flag;
     cp_async_wait_all();   // block i + 1 landed, and no thread reads stage i & 1 any more
     __syncthreads();
@@ -694,9 +850,12 @@ attn_bwd_dq_stream_kernel(const bf16* __restrict__ qkv, long long ld, const uint
 
 using namespace xclip;
 
-extern "C" int xclip_attn_fwd(const void* qkv, int64_t ld_qkv, const uint8_t* key_mask, void* o,
-                              int64_t ldo, float* lse, int B, int n, int heads, float scale,
-                              int causal, xclip_stream_t stream) {
+namespace {
+
+// launches of the plain (kDropout = false) and the dropout kernels; the callers have checked `drop`
+template <bool kDropout>
+int attn_fwd_run(const void* qkv, int64_t ld_qkv, const uint8_t* key_mask, void* o, int64_t ldo, float* lse,
+                 int B, int n, int heads, float scale, int causal, AttnDrop drop, xclip_stream_t stream) {
   int rc = xclip_init();
   if (rc) return rc;
   XCLIP_REQUIRE(qkv && o && lse, "attn_fwd: null pointer");
@@ -715,23 +874,21 @@ extern "C" int xclip_attn_fwd(const void* qkv, int64_t ld_qkv, const uint8_t* ke
   const long long blocks = (long long)(NP / kAttnRows) * B * heads;
   XCLIP_REQUIRE(blocks <= 0x7fffffffLL, "attn: B=%d x heads=%d is too large", B, heads);
   const dim3 grid((unsigned)blocks);
-  auto kern = streaming ? (causal ? attn_fwd_stream_kernel<true> : attn_fwd_stream_kernel<false>)
-                        : (causal ? attn_fwd_kernel<true> : attn_fwd_kernel<false>);
+  auto kern = streaming ? (causal ? attn_fwd_stream_kernel<true, kDropout> : attn_fwd_stream_kernel<false, kDropout>)
+                        : (causal ? attn_fwd_kernel<true, kDropout> : attn_fwd_kernel<false, kDropout>);
   rc = ensure_dynamic_smem(reinterpret_cast<const void*>(kern), smem);
   if (rc) return rc;
   kern<<<grid, kAttnThreads, smem, s>>>(reinterpret_cast<const bf16*>(qkv), ld_qkv, key_mask,
                                         reinterpret_cast<bf16*>(o), ldo, lse, n, heads,
-                                        scale * kLog2e);
+                                        scale * kLog2e, drop);
   XCLIP_LAUNCH_CHECK(streaming ? "attn_fwd_stream_kernel" : "attn_fwd_kernel");
   return XCLIP_OK;
 }
 
-extern "C" int xclip_attn_bwd(const void* qkv, int64_t ld_qkv, const uint8_t* key_mask,
-                              const void* o, int64_t ldo, const void* d_o, int64_t lddo,
-                              const float* lse, float* delta, void* dqkv, int64_t ld_dqkv,
-                              float* dq_workspace, int B, int n, int heads, float scale,
-                              int causal, xclip_stream_t stream) {
-  (void)dq_workspace;
+template <bool kDropout>
+int attn_bwd_run(const void* qkv, int64_t ld_qkv, const uint8_t* key_mask, const void* o, int64_t ldo,
+                 const void* d_o, int64_t lddo, const float* lse, float* delta, void* dqkv, int64_t ld_dqkv, int B,
+                 int n, int heads, float scale, int causal, AttnDrop drop, xclip_stream_t stream) {
   int rc = xclip_init();
   if (rc) return rc;
   XCLIP_REQUIRE(qkv && o && d_o && lse && delta && dqkv, "attn_bwd: null pointer");
@@ -767,24 +924,84 @@ extern "C" int xclip_attn_bwd(const void* qkv, int64_t ld_qkv, const uint8_t* ke
     // (Q, dO, 64 lse, 64 delta); both + the block's 64 key flags
     const int smem = streaming ? 6 * kAttnTile + 4 * kAttnRows * 4 + kAttnRows
                                : 2 * kAttnTile + 2 * NP * 128 + 2 * NP * 4 + kAttnRows;
-    auto kern = streaming ? (causal ? attn_bwd_dkdv_stream_kernel<true> : attn_bwd_dkdv_stream_kernel<false>)
-                          : (causal ? attn_bwd_dkdv_kernel<true> : attn_bwd_dkdv_kernel<false>);
+    auto kern = streaming ? (causal ? attn_bwd_dkdv_stream_kernel<true, kDropout>
+                                    : attn_bwd_dkdv_stream_kernel<false, kDropout>)
+                          : (causal ? attn_bwd_dkdv_kernel<true, kDropout> : attn_bwd_dkdv_kernel<false, kDropout>);
     rc = ensure_dynamic_smem(reinterpret_cast<const void*>(kern), smem);
     if (rc) return rc;
     kern<<<grid, kAttnThreads, smem, s>>>(q, ld_qkv, key_mask, g, lddo, lse, delta, d, ld_dqkv, n, heads,
-                                          scale, sl2);
+                                          scale, sl2, drop);
     XCLIP_LAUNCH_CHECK(streaming ? "attn_bwd_dkdv_stream_kernel" : "attn_bwd_dkdv_kernel");
   }
   {
     // resident: Q, dO block + the head's K, V and flags; streaming: Q, dO block + 2 stages of (K, V, 64 flags)
     const int smem = streaming ? 6 * kAttnTile + 2 * kAttnRows : 2 * kAttnTile + 2 * NP * 128 + NP;
-    auto kern = streaming ? (causal ? attn_bwd_dq_stream_kernel<true> : attn_bwd_dq_stream_kernel<false>)
-                          : (causal ? attn_bwd_dq_kernel<true> : attn_bwd_dq_kernel<false>);
+    auto kern = streaming ? (causal ? attn_bwd_dq_stream_kernel<true, kDropout>
+                                    : attn_bwd_dq_stream_kernel<false, kDropout>)
+                          : (causal ? attn_bwd_dq_kernel<true, kDropout> : attn_bwd_dq_kernel<false, kDropout>);
     rc = ensure_dynamic_smem(reinterpret_cast<const void*>(kern), smem);
     if (rc) return rc;
     kern<<<grid, kAttnThreads, smem, s>>>(q, ld_qkv, key_mask, g, lddo, lse, delta, d, ld_dqkv, n, heads,
-                                          scale, sl2);
+                                          scale, sl2, drop);
     XCLIP_LAUNCH_CHECK(streaming ? "attn_bwd_dq_stream_kernel" : "attn_bwd_dq_kernel");
   }
   return XCLIP_OK;
+}
+
+// p in [0, 1] -> the kernels' keep threshold and scale; refuses a bad p, seed or layer
+int attn_drop_args(const char* what, float p, const uint64_t* seed, int layer, AttnDrop* d) {
+  XCLIP_REQUIRE(p >= 0.f && p <= 1.f, "%s: dropout p=%g must lie in [0, 1]", what, (double)p);
+  XCLIP_REQUIRE(seed != nullptr && (reinterpret_cast<uintptr_t>(seed) & 7) == 0, "%s: seed must be an aligned "
+                "device pointer", what);
+  XCLIP_REQUIRE(layer >= 0, "%s: layer must be >= 0", what);
+  // keep iff the Philox word < round((1 - p) 2^32); p below 2^-33 keeps every element
+  const double thr = nearbyint((1.0 - (double)p) * 4294967296.0);
+  d->seed = seed;
+  d->keep_le = thr >= 4294967296.0 ? 0xffffffffu : thr >= 1.0 ? (uint32_t)(thr - 1.0) : 0u;
+  d->inv_keep = p == 1.f ? 0.f : 1.f / (1.f - p);
+  d->layer = (uint32_t)layer;
+  return XCLIP_OK;
+}
+
+}  // namespace
+
+extern "C" int xclip_attn_fwd(const void* qkv, int64_t ld_qkv, const uint8_t* key_mask, void* o,
+                              int64_t ldo, float* lse, int B, int n, int heads, float scale,
+                              int causal, xclip_stream_t stream) {
+  return attn_fwd_run<false>(qkv, ld_qkv, key_mask, o, ldo, lse, B, n, heads, scale, causal, AttnDrop{}, stream);
+}
+
+extern "C" int xclip_attn_bwd(const void* qkv, int64_t ld_qkv, const uint8_t* key_mask,
+                              const void* o, int64_t ldo, const void* d_o, int64_t lddo,
+                              const float* lse, float* delta, void* dqkv, int64_t ld_dqkv,
+                              float* dq_workspace, int B, int n, int heads, float scale,
+                              int causal, xclip_stream_t stream) {
+  (void)dq_workspace;
+  return attn_bwd_run<false>(qkv, ld_qkv, key_mask, o, ldo, d_o, lddo, lse, delta, dqkv, ld_dqkv, B, n, heads,
+                             scale, causal, AttnDrop{}, stream);
+}
+
+extern "C" int xclip_attn_dropout_fwd(const void* qkv, int64_t ld_qkv, const uint8_t* key_mask, void* o,
+                                      int64_t ldo, float* lse, int B, int n, int heads, float scale, int causal,
+                                      float p, const uint64_t* seed, int layer, xclip_stream_t stream) {
+  int rc = xclip_init();
+  if (rc) return rc;
+  AttnDrop d;
+  rc = attn_drop_args("attn_dropout_fwd", p, seed, layer, &d);
+  if (rc) return rc;
+  return attn_fwd_run<true>(qkv, ld_qkv, key_mask, o, ldo, lse, B, n, heads, scale, causal, d, stream);
+}
+
+extern "C" int xclip_attn_dropout_bwd(const void* qkv, int64_t ld_qkv, const uint8_t* key_mask,
+                                      const void* o, int64_t ldo, const void* d_o, int64_t lddo,
+                                      const float* lse, float* delta, void* dqkv, int64_t ld_dqkv, int B, int n,
+                                      int heads, float scale, int causal, float p, const uint64_t* seed,
+                                      int layer, xclip_stream_t stream) {
+  int rc = xclip_init();
+  if (rc) return rc;
+  AttnDrop d;
+  rc = attn_drop_args("attn_dropout_bwd", p, seed, layer, &d);
+  if (rc) return rc;
+  return attn_bwd_run<true>(qkv, ld_qkv, key_mask, o, ldo, d_o, lddo, lse, delta, dqkv, ld_dqkv, B, n, heads,
+                            scale, causal, d, stream);
 }

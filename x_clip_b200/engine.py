@@ -158,11 +158,20 @@ class TransformerFn(torch.autograd.Function):
     flat weights = [norm_in.g, norm_out.g] + depth * [g1, wqkv, wo, go, g2, w1, g4, w2].
     causal: the reference's causal mask (x_clip.py:233-236); rot_cos / rot_sin: f32 [n, 16] tables of
     the rotary embedding applied to q, k and v (x_clip.py:221-223) or None.
+    TransformerDropoutFn is the same encoder with attention dropout.
     """
 
     @staticmethod
     def forward(ctx, x, mask, heads: int, depth: int, causal: bool, rot_cos, rot_sin, need_bwd: bool,
                 *weights):
+        return TransformerFn._forward(ctx, x, mask, heads, depth, causal, rot_cos, rot_sin, need_bwd, None, weights)
+
+    @staticmethod
+    def backward(ctx, dout):
+        return TransformerFn._backward(ctx, dout, 8)
+
+    @staticmethod
+    def _forward(ctx, x, mask, heads, depth, causal, rot_cos, rot_sin, need_bwd, drop, weights):
         B, n, d = x.shape
         M = B * n
         scale = 64 ** -0.5
@@ -187,7 +196,7 @@ class TransformerFn(torch.autograd.Function):
             qkv = K.gemm(xn, bqkv)
             if rot_cos is not None:
                 K.rotary_(qkv, n, 3 * heads, rot_cos, rot_sin)
-            o, lse = K.attn_fwd(qkv, mask_c, B, n, heads, scale, causal)
+            o, lse = K.attn_fwd(qkv, mask_c, B, n, heads, scale, causal, dropout=_attn_dropout(drop, L))
             y = K.gemm(o, bo)
             # x1 = LN(y)*go + x ; xn2 = LN(x1)*g2   (attention tail + feed-forward pre-norm)
             x1, st_y, xn2, st_x1 = K.layernorm_fwd(y, go, res=xcur, g2=g2, eps=LN_EPS)
@@ -222,10 +231,12 @@ class TransformerFn(torch.autograd.Function):
         ctx.ff_saved = ff_saved
         ctx.weights = weights
         ctx.wb = wb
+        ctx.drop = drop
         return out.view(B, n, d)
 
     @staticmethod
-    def backward(ctx, dout):
+    def _backward(ctx, dout, n_args: int):
+        """-> gradients of the n_args leading arguments (dx and Nones) + the weights' gradients"""
         B, n, d, heads, depth, scale, causal = ctx.dims
         rot_cos, rot_sin = ctx.rot
         M = B * n
@@ -244,7 +255,7 @@ class TransformerFn(torch.autograd.Function):
         # parameters with requires_grad=False (a frozen tower: adversarial / guidance use) cost no
         # weight-gradient work: their wgrad GEMMs and gain reductions are skipped and None returned.
         # The data-gradient chain reads none of them, so dx is the same either way.
-        wneed = ctx.needs_input_grad[8:]
+        wneed = ctx.needs_input_grad[n_args:]
 
         def gain_grad(idx):
             """fp32 accumulator for the gain gradient of weights[idx]: its .grad (in-place mode) or
@@ -309,7 +320,8 @@ class TransformerFn(torch.autograd.Function):
             dy = K.layernorm_bwd(dx1, y, st_y, go, dg=dgo)
             d_o = K.gemm(dy, bo, b_major=1)
             grads[base + 2] = weight_grad(base + 2, dy, o)
-            dqkv = K.attn_bwd(qkv, ctx.mask, o, d_o, lse, B, n, heads, scale, causal)
+            dqkv = K.attn_bwd(qkv, ctx.mask, o, d_o, lse, B, n, heads, scale, causal,
+                              dropout=_attn_dropout(ctx.drop, L))
             if rot_cos is not None:      # back through the rotation (its transpose)
                 K.rotary_(dqkv, n, 3 * heads, rot_cos, rot_sin, inverse=True)
             dxn = K.gemm(dqkv, bqkv, b_major=1)
@@ -319,8 +331,34 @@ class TransformerFn(torch.autograd.Function):
         dg_in, grads[0] = gain_grad(0)
         dx_in = K.layernorm_bwd(dx, x_in, st_in, g_in, dg=dg_in)
         wg.join()
-        ctx.saved = ctx.wb = None
-        return (dx_in.view(B, n, d), None, None, None, None, None, None, None, *grads)
+        ctx.saved = ctx.wb = ctx.drop = None
+        return (dx_in.view(B, n, d),) + (None,) * (n_args - 1) + tuple(grads)
+
+
+def _attn_dropout(drop, L: int):
+    """The (p, seed, layer) argument of K.attn_fwd / attn_bwd for layer L, or None (no dropout)."""
+    if drop is None or drop[0][L] == 0.0:
+        return None
+    return drop[0][L], drop[1], L
+
+
+class TransformerDropoutFn(torch.autograd.Function):
+    """TransformerFn with dropout on the attention probabilities (x_clip.py:211, :241-243).
+
+    drop = (p per layer, seed): seed is an int64 [1] device tensor, the Philox key of every layer's
+    mask (xclip_attn_dropout_fwd; layer L draws with counter word L).  The backward reuses the seed
+    kept in ctx, so it sees the forward's masks; a second forward with the same seed (the re-encode of
+    a micro-batched step, or a forward-only sweep) draws the same masks as well.  A layer with p = 0
+    runs the plain kernels."""
+
+    @staticmethod
+    def forward(ctx, x, mask, heads: int, depth: int, causal: bool, rot_cos, rot_sin, need_bwd: bool, drop,
+                *weights):
+        return TransformerFn._forward(ctx, x, mask, heads, depth, causal, rot_cos, rot_sin, need_bwd, drop, weights)
+
+    @staticmethod
+    def backward(ctx, dout):
+        return TransformerFn._backward(ctx, dout, 9)
 
 
 class TextEmbedFn(torch.autograd.Function):

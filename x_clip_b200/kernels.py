@@ -226,30 +226,53 @@ def l2norm_bwd(dz, z, inv):
     return dp
 
 
-def attn_fwd(qkv, key_mask, B, n, heads, scale, causal=False):
-    """qkv bf16 [B*n, 3*heads*64] -> (o bf16 [B*n, heads*64], lse f32 [B, heads, n])."""
+def _attn_key_mask(key_mask, B, n, what):
+    if key_mask is not None:
+        if key_mask.dtype != torch.bool or tuple(key_mask.shape) != (B, n) or not key_mask.is_contiguous():
+            raise _lib.XClipB200Error(f"{what}: key_mask must be a contiguous bool [B, n]")
+
+
+def _attn_seed(seed, qkv):
+    if seed.dtype != torch.int64 or seed.numel() != 1 or seed.device != qkv.device:
+        raise _lib.XClipB200Error("attention dropout: seed must be one int64 on the operands' device")
+
+
+def attn_fwd(qkv, key_mask, B, n, heads, scale, causal=False, dropout=None):
+    """qkv bf16 [B*n, 3*heads*64] -> (o bf16 [B*n, heads*64], lse f32 [B, heads, n]).
+    dropout = (p, seed int64 [1] on the device, layer) runs xclip_attn_dropout_fwd."""
     _need(qkv, BF16, "qkv"); _rows2d(qkv, "qkv")
     o = torch.empty((B * n, heads * 64), device=qkv.device, dtype=BF16)
     lse = torch.empty((B, heads, n), device=qkv.device, dtype=F32)
-    if key_mask is not None:
-        if key_mask.dtype != torch.bool or tuple(key_mask.shape) != (B, n) or not key_mask.is_contiguous():
-            raise _lib.XClipB200Error("attn_fwd: key_mask must be a contiguous bool [B, n]")
-    _call(qkv, "attn_fwd", 4.0 * B * heads * n * n * 64, 2.0 * B * n * heads * 64 * 4, "xclip_attn_fwd", qkv.data_ptr(), qkv.stride(0), _ptr(key_mask), o.data_ptr(),
-              o.stride(0), lse.data_ptr(), B, n, heads, float(scale), 1 if causal else 0)
+    _attn_key_mask(key_mask, B, n, "attn_fwd")
+    args = (qkv.data_ptr(), qkv.stride(0), _ptr(key_mask), o.data_ptr(), o.stride(0), lse.data_ptr(), B, n, heads,
+            float(scale), 1 if causal else 0)
+    flops, nbytes = 4.0 * B * heads * n * n * 64, 2.0 * B * n * heads * 64 * 4
+    if dropout is None:
+        _call(qkv, "attn_fwd", flops, nbytes, "xclip_attn_fwd", *args)
+    else:
+        p, seed, layer = dropout
+        _attn_seed(seed, qkv)
+        _call(qkv, "attn_fwd", flops, nbytes, "xclip_attn_dropout_fwd", *args, float(p), seed.data_ptr(), int(layer))
     return o, lse
 
 
-def attn_bwd(qkv, key_mask, o, d_o, lse, B, n, heads, scale, causal=False):
+def attn_bwd(qkv, key_mask, o, d_o, lse, B, n, heads, scale, causal=False, dropout=None):
+    """-> dqkv bf16 like qkv.  dropout = the forward's (p, seed, layer): xclip_attn_dropout_bwd."""
     _need(d_o, BF16, "d_o"); _rows2d(d_o, "d_o")
-    if key_mask is not None:
-        if key_mask.dtype != torch.bool or tuple(key_mask.shape) != (B, n) or not key_mask.is_contiguous():
-            raise _lib.XClipB200Error("attn_bwd: key_mask must be a contiguous bool [B, n]")
+    _attn_key_mask(key_mask, B, n, "attn_bwd")
     dqkv = torch.empty_like(qkv)
     delta = torch.empty((B, heads, n), device=qkv.device, dtype=F32)
-    _call(qkv, "attn_bwd", 10.0 * B * heads * n * n * 64, 2.0 * B * n * heads * 64 * 8, "xclip_attn_bwd", qkv.data_ptr(), qkv.stride(0), _ptr(key_mask), o.data_ptr(),
-              o.stride(0), d_o.data_ptr(), d_o.stride(0), lse.data_ptr(), delta.data_ptr(),
-              dqkv.data_ptr(), dqkv.stride(0), None, B, n, heads, float(scale),
-              1 if causal else 0)
+    head = (qkv.data_ptr(), qkv.stride(0), _ptr(key_mask), o.data_ptr(), o.stride(0), d_o.data_ptr(), d_o.stride(0),
+            lse.data_ptr(), delta.data_ptr(), dqkv.data_ptr(), dqkv.stride(0))
+    tail = (B, n, heads, float(scale), 1 if causal else 0)
+    flops, nbytes = 10.0 * B * heads * n * n * 64, 2.0 * B * n * heads * 64 * 8
+    if dropout is None:
+        _call(qkv, "attn_bwd", flops, nbytes, "xclip_attn_bwd", *head, None, *tail)
+    else:
+        p, seed, layer = dropout
+        _attn_seed(seed, qkv)
+        _call(qkv, "attn_bwd", flops, nbytes, "xclip_attn_dropout_bwd", *head, *tail, float(p), seed.data_ptr(),
+              int(layer))
     return dqkv
 
 
