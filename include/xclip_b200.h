@@ -243,6 +243,23 @@ int xclip_filip_expand(const int* seg_arg, const float* seg_max, const float* wm
                        const float* rowscale, const float* temp_exp, int row0, int rows,
                        int rows_per_sample, int seg_len, int nseg, void* g, int64_t ldg,
                        float* dtemp, xclip_stream_t stream);
+/* Compact argmax, for the saved state of a row-chunked FILIP loss (2 bytes per (row, sample)
+ * instead of 8):
+ * segmax_arg16 : xclip_filip_segmax_any, writing seg_max (f32) and / or a 16-bit seg_arg; either
+ *          may be null, not both.  Refused without a launch: seg_len > 65535, both outputs null,
+ *          seg_max not 4-byte or seg_arg not 2-byte aligned, and every refusal of segmax_any.
+ * expand16 : xclip_filip_expand on a 16-bit seg_arg that holds rows [row0, row0 + rows) only
+ *          (row r of G reads seg_arg[(r - row0) * nseg + y]; wmat and rowscale are still indexed
+ *          by the global row).  No seg_max and no dtemp: d loss / d log temperature is
+ *          sum(d t2i * t2i) + sum(d i2t * i2t) over the [B,B] matrices.  Writes the same G bits
+ *          as xclip_filip_expand.  seg_len <= 65535, seg_arg 2-byte aligned, otherwise as expand. */
+int xclip_filip_segmax_arg16(const void* a, const void* b, int R, int C, int D,
+                             const float* temp_exp, int seg_len, const float* col_mul,
+                             const float* col_add, float* seg_max, uint16_t* seg_arg, void* keys,
+                             xclip_stream_t stream);
+int xclip_filip_expand16(const uint16_t* seg_arg, const float* wmat, const float* rowscale,
+                         const float* temp_exp, int row0, int rows, int rows_per_sample,
+                         int seg_len, int nseg, void* g, int64_t ldg, xclip_stream_t stream);
 
 /* ---- text embedding (x_clip/x_clip.py:320-332) ---------------------------------------------
  * fwd: out bf16 [B, n+1, d]: out[b,0] = cls, out[b,1+t] = tok[ids[b,t]] + pos[t]  (fp32 tables,

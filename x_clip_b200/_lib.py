@@ -103,6 +103,10 @@ SIGNATURES = {
                                     c_void_p, c_void_p]),
     "xclip_filip_expand": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
                                    c_int, c_int, c_int, c_void_p, c_int64, c_void_p, c_void_p]),
+    "xclip_filip_segmax_arg16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int,
+                                         c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "xclip_filip_expand16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
+                                     c_int, c_void_p, c_int64, c_void_p]),
 }
 
 

@@ -457,14 +457,19 @@ class CLIP(nn.Module):
         return torch.gather(enc_text, 1, order[:, :, None].expand(-1, -1, d))
 
     def _encode_to_latents(self, text, image, text_mask):
-        """encoders -> CLS select -> projections (CLS mode).  Returns ([zt, zi(, zt_x, zi_x)], ops)."""
+        """encoders -> CLS select (FILIP: every token but the CLS) -> projections.
+        Returns ([zt, zi(, zt_x, zi_x)], ops): latents [b, D], or [b, tokens, D] in FILIP mode."""
         text_args = (text,) if self.text_encode_without_mask else (text, text_mask)
         enc_text = self.text_transformer(*text_args)
         if self.text_causal_mask:
             enc_text = self._eos_to_front(enc_text, text)
         enc_image = self.visual_transformer(image)
-        te = enc_text[:, 0] if enc_text.ndim == 3 else enc_text
-        ie = enc_image[:, 0] if enc_image.ndim == 3 else enc_image
+        if self.use_all_token_embeds:
+            te = enc_text[:, 1:] if self.text_has_cls_token else enc_text
+            ie = enc_image[:, 1:] if self.visual_has_cls_token else enc_image
+        else:
+            te = enc_text[:, 0] if enc_text.ndim == 3 else enc_text
+            ie = enc_image[:, 0] if enc_image.ndim == 3 else enc_image
         zt, ops_t = self._project(te, self.to_text_latent)
         zi, ops_i = self._project(ie, self.to_visual_latent)
         zs, ops = [zt, zi], [ops_t, ops_i]
@@ -534,7 +539,7 @@ class CLIP(nn.Module):
 
         has_aux = is_multiview or self.use_mlm or self.use_visual_ssl
         if (return_loss and self.microbatch and text.shape[0] > self.microbatch and not has_aux
-                and not self.use_all_token_embeds and not (freeze_image_encoder or freeze_text_encoder)):
+                and not (freeze_image_encoder or freeze_text_encoder)):
             return E.ChunkedClipLossFn.apply(self, text, image, text_mask, int(self.microbatch),
                                              self.temperature, self.microbatch_retain)
         text_args = (text,) if self.text_encode_without_mask else (text, text_mask)

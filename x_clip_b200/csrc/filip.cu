@@ -92,12 +92,16 @@ filip_nce_bwd_kernel(const float* __restrict__ s, const float* __restrict__ lse,
 
 // G[r, c] (bf16) for rows [row0, row0+rows): alpha * wmat[sample(r), seg(c)] * rowscale[r] at the
 // argmax column of each segment, zero elsewhere.  dtemp += sum_r,seg w * segmax (w without alpha).
+// Idx = int: seg_arg / seg_max are indexed by the global row r.  Idx = unsigned short (the compact
+// form): seg_arg holds rows [row0, row0 + rows) only, and there is no seg_max and no dtemp.
+template <typename Idx>
 __global__ void __launch_bounds__(256)
-filip_expand_kernel(const int* __restrict__ seg_arg, const float* __restrict__ seg_max,
+filip_expand_kernel(const Idx* __restrict__ seg_arg, const float* __restrict__ seg_max,
                     const float* __restrict__ wmat, const float* __restrict__ rowscale,
                     const float* __restrict__ alpha_dev, int row0, int rows, int rows_per_sample,
                     int seg_len, int nseg, bf16* __restrict__ g, long long ldg,
                     float* __restrict__ dtemp) {
+  constexpr bool kCompact = sizeof(Idx) == 2;
   const float alpha = __ldg(alpha_dev);
   const int vec_per_row = nseg * seg_len / 8;
   float tsum = 0.f;
@@ -108,12 +112,12 @@ filip_expand_kernel(const int* __restrict__ seg_arg, const float* __restrict__ s
     const long long r = row0 + lr;
     const int seg = c0 / seg_len;
     const int in_seg = c0 - seg * seg_len;
-    const int a = seg_arg[r * nseg + seg];
+    const int a = seg_arg[(kCompact ? lr : r) * nseg + seg];
     uint4 o = make_uint4(0, 0, 0, 0);
     if (a >= in_seg && a < in_seg + 8) {
       const float w = wmat[(r / rows_per_sample) * nseg + seg] * rowscale[r];
       if (w != 0.f) {
-        tsum += w * seg_max[r * nseg + seg];
+        if constexpr (!kCompact) tsum += w * seg_max[r * nseg + seg];
         bf16 vals[8];
 #pragma unroll
         for (int k = 0; k < 8; ++k) vals[k] = __float2bfloat16_rn(0.f);
@@ -123,7 +127,7 @@ filip_expand_kernel(const int* __restrict__ seg_arg, const float* __restrict__ s
     }
     *reinterpret_cast<uint4*>(g + lr * ldg + c0) = o;
   }
-  if (dtemp != nullptr) {
+  if (!kCompact && dtemp != nullptr) {
     tsum = warp_sum(tsum);
     if ((threadIdx.x & 31) == 0 && tsum != 0.f) atomicAdd(dtemp, tsum);
   }
@@ -132,12 +136,14 @@ filip_expand_kernel(const int* __restrict__ seg_arg, const float* __restrict__ s
 // filip_expand_kernel for seg_len % 8 != 0: an 8-column vector may hold the end of one segment and
 // the start of the next (several when seg_len < 8), so every column steps its own (segment,
 // position).  Columns [nseg * seg_len, roundup8) of the last vector are written as zeros.
+template <typename Idx>
 __global__ void __launch_bounds__(256)
-filip_expand_any_kernel(const int* __restrict__ seg_arg, const float* __restrict__ seg_max,
+filip_expand_any_kernel(const Idx* __restrict__ seg_arg, const float* __restrict__ seg_max,
                         const float* __restrict__ wmat, const float* __restrict__ rowscale,
                         const float* __restrict__ alpha_dev, int row0, int rows, int rows_per_sample,
                         int seg_len, int nseg, bf16* __restrict__ g, long long ldg,
                         float* __restrict__ dtemp) {
+  constexpr bool kCompact = sizeof(Idx) == 2;
   const float alpha = __ldg(alpha_dev);
   const int C = nseg * seg_len;
   const int vec_per_row = (C + 7) / 8;
@@ -147,7 +153,7 @@ filip_expand_any_kernel(const int* __restrict__ seg_arg, const float* __restrict
     const int lr = (int)(v / vec_per_row);
     const int c0 = (int)(v % vec_per_row) * 8;
     const long long r = row0 + lr;
-    const int* arg_row = seg_arg + r * nseg;
+    const Idx* arg_row = seg_arg + (kCompact ? lr : r) * nseg;
     const float* w_row = wmat + (r / rows_per_sample) * nseg;
     int seg = c0 / seg_len;
     int pos = c0 - seg * seg_len;
@@ -160,7 +166,7 @@ filip_expand_any_kernel(const int* __restrict__ seg_arg, const float* __restrict
         if (pos == a) {
           const float w = w_row[seg] * rowscale[r];
           if (w != 0.f) {
-            tsum += w * seg_max[r * nseg + seg];
+            if constexpr (!kCompact) tsum += w * seg_max[r * nseg + seg];
             vals[k] = __float2bfloat16_rn(w * alpha);
           }
         }
@@ -172,7 +178,7 @@ filip_expand_any_kernel(const int* __restrict__ seg_arg, const float* __restrict
     }
     *reinterpret_cast<uint4*>(g + lr * ldg + c0) = *reinterpret_cast<const uint4*>(vals);
   }
-  if (dtemp != nullptr) {
+  if (!kCompact && dtemp != nullptr) {
     tsum = warp_sum(tsum);
     if ((threadIdx.x & 31) == 0 && tsum != 0.f) atomicAdd(dtemp, tsum);
   }
@@ -190,33 +196,44 @@ filip_unpack_keys_kernel(const unsigned long long* __restrict__ keys, long long 
   }
 }
 
+// keys of EPI_SEGMAX -> seg_max (f32, optional) and a 16-bit seg_arg (optional): the compact
+// argmax a saved chunk keeps for its backward (seg_len <= 65535)
+__global__ void __launch_bounds__(256)
+filip_unpack_keys16_kernel(const unsigned long long* __restrict__ keys, long long n,
+                           float* __restrict__ seg_max, unsigned short* __restrict__ seg_arg) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n;
+       i += (long long)gridDim.x * blockDim.x) {
+    const unsigned long long k = keys[i];
+    if (seg_max != nullptr) seg_max[i] = segmax_key_value(k);
+    if (seg_arg != nullptr) seg_arg[i] = (unsigned short)segmax_key_index(k);
+  }
+}
+
 }  // namespace xclip
 
 using namespace xclip;
 
-extern "C" int xclip_filip_segmax_any(const void* a, const void* b, int R, int C, int D,
-                                      const float* temp_exp, int seg_len, const float* col_mul,
-                                      const float* col_add, float* seg_max, int* seg_arg, void* keys,
-                                      xclip_stream_t stream) {
-  int rc = xclip_init();
-  if (rc) return rc;
-  XCLIP_REQUIRE(a && b && temp_exp && seg_max && seg_arg && keys, "filip_segmax_any: null pointer");
-  XCLIP_REQUIRE(R > 0 && C > 0 && D > 0 && D % 8 == 0, "filip_segmax_any: bad sizes");
+// The segment-max GEMM shared by both unpack forms: checks its arguments, zeroes the keys and
+// launches EPI_SEGMAX.  Returns non-zero (nothing launched) when an argument is refused.
+static int filip_segmax_keys(const char* who, const void* a, const void* b, int R, int C, int D,
+                             const float* temp_exp, int seg_len, const float* col_mul,
+                             const float* col_add, void* keys, cudaStream_t st) {
+  XCLIP_REQUIRE(a && b && temp_exp && keys, "%s: null pointer", who);
+  XCLIP_REQUIRE(R > 0 && C > 0 && D > 0 && D % 8 == 0, "%s: bad sizes", who);
   XCLIP_REQUIRE(seg_len >= 1 && C % seg_len == 0,
-                "filip_segmax_any: C (%d) must be a whole number of segments of seg_len (%d) >= 1 tokens",
+                "%s: C (%d) must be a whole number of segments of seg_len (%d) >= 1 tokens", who,
                 C, seg_len);
-  XCLIP_REQUIRE((col_mul == nullptr) == (col_add == nullptr), "filip_segmax_any: mask tables mismatch");
+  XCLIP_REQUIRE((col_mul == nullptr) == (col_add == nullptr), "%s: mask tables mismatch", who);
   XCLIP_REQUIRE(((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b)) & 15) == 0,
-                "filip_segmax_any: misaligned latents");
-  XCLIP_REQUIRE(((reinterpret_cast<uintptr_t>(temp_exp) | reinterpret_cast<uintptr_t>(seg_max) |
-                  reinterpret_cast<uintptr_t>(seg_arg) | reinterpret_cast<uintptr_t>(col_mul) |
+                "%s: misaligned latents", who);
+  XCLIP_REQUIRE(((reinterpret_cast<uintptr_t>(temp_exp) | reinterpret_cast<uintptr_t>(col_mul) |
                   reinterpret_cast<uintptr_t>(col_add)) & 3) == 0,
-                "filip_segmax_any: misaligned fp32 / int32 pointer");
-  XCLIP_REQUIRE((reinterpret_cast<uintptr_t>(keys) & 7) == 0, "filip_segmax_any: misaligned keys");
+                "%s: misaligned fp32 pointer", who);
+  XCLIP_REQUIRE((reinterpret_cast<uintptr_t>(keys) & 7) == 0, "%s: misaligned keys", who);
   const int nseg = C / seg_len;
   const long long nkeys = (long long)R * nseg;
   CUtensorMap tmA, tmB;
-  rc = encode_2d_bf16(&tmA, a, (uint64_t)D, (uint64_t)R, (uint64_t)D, 64, kGemmBlockM);
+  int rc = encode_2d_bf16(&tmA, a, (uint64_t)D, (uint64_t)R, (uint64_t)D, 64, kGemmBlockM);
   if (rc) return rc;
   rc = encode_2d_bf16(&tmB, b, (uint64_t)D, (uint64_t)C, (uint64_t)D, 64, 256);
   if (rc) return rc;
@@ -236,15 +253,56 @@ extern "C" int xclip_filip_segmax_any(const void* a, const void* b, int R, int C
     const int rc_attr = ensure_dynamic_smem(reinterpret_cast<const void*>(kern), S::kTotal);
     if (rc_attr) return rc_attr;
   }
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   XCLIP_CUDA(cudaMemsetAsync(keys, 0, (size_t)nkeys * 8, st));
   kern<<<grid, kGemmThreads, S::kTotal, st>>>(tmA, tmB, p, CUtensorMap{}, CUtensorMap{});
   XCLIP_LAUNCH_CHECK("gemm_bf16_kernel<segmax>");
+  return XCLIP_OK;
+}
+
+static int unpack_blocks(long long nkeys) {
   long long blocks = (nkeys + 255) / 256;
   if (blocks > (long long)num_sms() * 16) blocks = (long long)num_sms() * 16;
-  filip_unpack_keys_kernel<<<(int)blocks, 256, 0, st>>>(
+  return (int)blocks;
+}
+
+extern "C" int xclip_filip_segmax_any(const void* a, const void* b, int R, int C, int D,
+                                      const float* temp_exp, int seg_len, const float* col_mul,
+                                      const float* col_add, float* seg_max, int* seg_arg, void* keys,
+                                      xclip_stream_t stream) {
+  int rc = xclip_init();
+  if (rc) return rc;
+  XCLIP_REQUIRE(seg_max && seg_arg, "filip_segmax_any: null pointer");
+  XCLIP_REQUIRE(((reinterpret_cast<uintptr_t>(seg_max) | reinterpret_cast<uintptr_t>(seg_arg)) & 3) == 0,
+                "filip_segmax_any: misaligned fp32 / int32 pointer");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  rc = filip_segmax_keys("filip_segmax_any", a, b, R, C, D, temp_exp, seg_len, col_mul, col_add, keys, st);
+  if (rc) return rc;
+  const long long nkeys = (long long)R * (C / seg_len);
+  filip_unpack_keys_kernel<<<unpack_blocks(nkeys), 256, 0, st>>>(
       reinterpret_cast<const unsigned long long*>(keys), nkeys, seg_max, seg_arg);
   XCLIP_LAUNCH_CHECK("filip_unpack_keys_kernel");
+  return XCLIP_OK;
+}
+
+extern "C" int xclip_filip_segmax_arg16(const void* a, const void* b, int R, int C, int D,
+                                        const float* temp_exp, int seg_len, const float* col_mul,
+                                        const float* col_add, float* seg_max, uint16_t* seg_arg,
+                                        void* keys, xclip_stream_t stream) {
+  int rc = xclip_init();
+  if (rc) return rc;
+  XCLIP_REQUIRE(seg_max || seg_arg, "filip_segmax_arg16: neither seg_max nor seg_arg requested");
+  XCLIP_REQUIRE(seg_len <= 65535, "filip_segmax_arg16: seg_len %d does not fit a 16-bit argmax (<= 65535)",
+                seg_len);
+  XCLIP_REQUIRE(((reinterpret_cast<uintptr_t>(seg_max) & 3) | (reinterpret_cast<uintptr_t>(seg_arg) & 1)) == 0,
+                "filip_segmax_arg16: misaligned seg_max / seg_arg");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  rc = filip_segmax_keys("filip_segmax_arg16", a, b, R, C, D, temp_exp, seg_len, col_mul, col_add, keys, st);
+  if (rc) return rc;
+  const long long nkeys = (long long)R * (C / seg_len);
+  filip_unpack_keys16_kernel<<<unpack_blocks(nkeys), 256, 0, st>>>(
+      reinterpret_cast<const unsigned long long*>(keys), nkeys, seg_max,
+      reinterpret_cast<unsigned short*>(seg_arg));
+  XCLIP_LAUNCH_CHECK("filip_unpack_keys16_kernel");
   return XCLIP_OK;
 }
 
@@ -302,15 +360,44 @@ extern "C" int xclip_filip_expand(const int* seg_arg, const float* seg_max, cons
   long long blocks = (vecs + 255) / 256;
   if (blocks > (long long)num_sms() * 16) blocks = (long long)num_sms() * 16;
   if (seg_len % 8 == 0) {
-    filip_expand_kernel<<<(int)blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+    filip_expand_kernel<int><<<(int)blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
         seg_arg, seg_max, wmat, rowscale, temp_exp, row0, rows, rows_per_sample, seg_len, nseg,
         reinterpret_cast<bf16*>(g), ldg, dtemp);
     XCLIP_LAUNCH_CHECK("filip_expand_kernel");
   } else {
-    filip_expand_any_kernel<<<(int)blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+    filip_expand_any_kernel<int><<<(int)blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
         seg_arg, seg_max, wmat, rowscale, temp_exp, row0, rows, rows_per_sample, seg_len, nseg,
         reinterpret_cast<bf16*>(g), ldg, dtemp);
     XCLIP_LAUNCH_CHECK("filip_expand_any_kernel");
+  }
+  return XCLIP_OK;
+}
+
+extern "C" int xclip_filip_expand16(const uint16_t* seg_arg, const float* wmat, const float* rowscale,
+                                    const float* temp_exp, int row0, int rows, int rows_per_sample,
+                                    int seg_len, int nseg, void* g, int64_t ldg, xclip_stream_t stream) {
+  int rc = xclip_init();
+  if (rc) return rc;
+  XCLIP_REQUIRE(seg_arg && wmat && rowscale && temp_exp && g, "filip_expand16: null pointer");
+  XCLIP_REQUIRE(row0 >= 0 && rows > 0 && rows_per_sample > 0 && seg_len >= 1 && seg_len <= 65535 &&
+                    nseg > 0 && ldg >= (int64_t)nseg * seg_len && ldg % 8 == 0,
+                "filip_expand16: bad sizes");
+  XCLIP_REQUIRE((reinterpret_cast<uintptr_t>(g) & 15) == 0, "filip_expand16: misaligned g");
+  XCLIP_REQUIRE((reinterpret_cast<uintptr_t>(seg_arg) & 1) == 0, "filip_expand16: misaligned seg_arg");
+  const long long vecs = (long long)rows * ((nseg * seg_len + 7) / 8);
+  long long blocks = (vecs + 255) / 256;
+  if (blocks > (long long)num_sms() * 16) blocks = (long long)num_sms() * 16;
+  const unsigned short* arg = reinterpret_cast<const unsigned short*>(seg_arg);
+  if (seg_len % 8 == 0) {
+    filip_expand_kernel<unsigned short><<<(int)blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+        arg, nullptr, wmat, rowscale, temp_exp, row0, rows, rows_per_sample, seg_len, nseg,
+        reinterpret_cast<bf16*>(g), ldg, nullptr);
+    XCLIP_LAUNCH_CHECK("filip_expand_kernel<u16>");
+  } else {
+    filip_expand_any_kernel<unsigned short><<<(int)blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+        arg, nullptr, wmat, rowscale, temp_exp, row0, rows, rows_per_sample, seg_len, nseg,
+        reinterpret_cast<bf16*>(g), ldg, nullptr);
+    XCLIP_LAUNCH_CHECK("filip_expand_any_kernel<u16>");
   }
   return XCLIP_OK;
 }

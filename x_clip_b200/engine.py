@@ -673,7 +673,9 @@ class ChunkedClipLossFn(torch.autograd.Function):
     here the same need (4096 pairs per GPU for a 32768 global batch) is met by a GradCache-style
     schedule that is mathematically identical to the single-pass step:
       1. encode every chunk -> latents of the whole local batch
-      2. one contrastive loss over ALL latents (with the usual cross-rank all-gather)
+      2. one contrastive loss over ALL latents (with the usual cross-rank all-gather); with
+         `use_all_token_embeds` the FILIP loss (filip.FilipLossFn) over all token latents, which
+         works in row chunks of its own and is left `filip.step_reserve_bytes` of HBM by the plan
       3. in backward: d loss / d latents, then back-propagate the matching slice of the latent
          gradient through every chunk's encoders.
     Memory plan: a chunk's saved activations are KEPT from step 1 for as many chunks as
@@ -700,6 +702,8 @@ class ChunkedClipLossFn(torch.autograd.Function):
             return image[s:e].detach().requires_grad_(True)
 
         foot = None                                   # bytes of one retained chunk's activations
+        reserve = 0                                   # HBM left to the loss (FILIP: filip.step_reserve_bytes)
+        filip = clip.use_all_token_embeds
         # "auto" plans ONCE per (batch, chunk size): the first step measures and decides, later steps
         # repeat its decision - the same tensors are then allocated in the same order every step, which
         # is what keeps torch's caching allocator free of fragmentation this close to the HBM limit
@@ -720,7 +724,7 @@ class ChunkedClipLossFn(torch.autograd.Function):
                     if foot is None:                  # first chunk: keep it, measure it
                         keep_it = True
                     else:
-                        need = foot * scale * (1.0 + RETAIN_TRANSIENT_FRAC) + RETAIN_MARGIN_BYTES
+                        need = foot * scale * (1.0 + RETAIN_TRANSIENT_FRAC) + RETAIN_MARGIN_BYTES + reserve
                         keep_it = _avail_bytes(dev) >= need
                 else:
                     keep_it = k < int(retain)
@@ -750,8 +754,13 @@ class ChunkedClipLossFn(torch.autograd.Function):
                     img_leaves.append(img_k if want_dimage else None)
                     if foot is None:
                         foot = max(torch.cuda.memory_allocated(dev) - before, 1)
-                        if planned and len(bounds) > 1 and \
-                                _avail_bytes(dev) < foot * (1.0 + RETAIN_TRANSIENT_FRAC) + RETAIN_MARGIN_BYTES:
+                        if filip:
+                            from .filip import step_reserve_bytes
+                            world = D_.world()[1] if clip.requires_all_gather else 1
+                            reserve = step_reserve_bytes(B, world * B, z[0].shape[1], z[1].shape[1],
+                                                         z[0].shape[2], len(z) == 4)
+                        if planned and len(bounds) > 1 and _avail_bytes(dev) < \
+                                foot * (1.0 + RETAIN_TRANSIENT_FRAC) + RETAIN_MARGIN_BYTES + reserve:
                             kept[-1] = None           # not even a second live chunk fits beside it: let it go
                             img_leaves[-1] = None
                     z = [t.detach() for t in z]
@@ -765,13 +774,22 @@ class ChunkedClipLossFn(torch.autograd.Function):
         leaves = [torch.cat([z[j] for z in zs]).detach().requires_grad_(True) for j in range(nsets)]
         ops_all = tuple((torch.cat([o[j][0] for o in opss]), torch.cat([o[j][1] for o in opss]))
                         for j in range(nsets))
+        del zs, opss
         temp_leaf = temperature.detach().requires_grad_(True)
+        filip_stats = {} if filip else None
         with torch.enable_grad():
-            loss = ContrastiveLossFn.apply(
-                leaves[0], leaves[1], leaves[2] if nsets == 4 else None,
-                leaves[3] if nsets == 4 else None, temp_leaf, ops_all,
-                clip.decoupled_contrastive_learning, clip.requires_all_gather,
-                *((clip.sim_reg_loss_weight, 1.0) if clip.has_sim_reg_loss else ()))
+            if filip:
+                from .filip import FilipLossFn
+                loss = FilipLossFn.apply(
+                    leaves[0], leaves[1], leaves[2] if nsets == 4 else None,
+                    leaves[3] if nsets == 4 else None, temp_leaf, ops_all, text_mask.contiguous(),
+                    clip.decoupled_contrastive_learning, clip.requires_all_gather, filip_stats)
+            else:
+                loss = ContrastiveLossFn.apply(
+                    leaves[0], leaves[1], leaves[2] if nsets == 4 else None,
+                    leaves[3] if nsets == 4 else None, temp_leaf, ops_all,
+                    clip.decoupled_contrastive_learning, clip.requires_all_gather,
+                    *((clip.sim_reg_loss_weight, 1.0) if clip.has_sim_reg_loss else ()))
         ctx.clip, ctx.inputs = clip, (text, image, text_mask)
         ctx.bounds, ctx.rng_states, ctx.kept = bounds, rng_states, kept
         ctx.img_leaves = img_leaves if want_dimage else None
@@ -782,6 +800,9 @@ class ChunkedClipLossFn(torch.autograd.Function):
             plans[plan_key] = [z is not None for z in kept]    # WHICH chunks stay resident
         clip.last_step_plan = dict(chunks=len(bounds), retained=n_kept, chunk_activation_bytes=foot,
                                    oom_fallbacks=oom_fallbacks)
+        if filip:
+            # rows of both FILIP passes whose argmax was saved / will be recomputed in backward
+            clip.last_step_plan.update(filip=filip_stats, loss_reserve_bytes=reserve)
         return loss.detach()
 
     @staticmethod

@@ -577,6 +577,55 @@ def filip_expand(seg_arg, seg_max, wmat, rowscale, temp_exp, row0, rows, rows_pe
     return g[:, :C]
 
 
+ARG16_MAX_SEG_LEN = 65535
+
+
+def check_arg16_seg_len(seg_len):
+    """A 16-bit argmax indexes at most 65535 tokens per sample; larger counts are refused before
+    anything is allocated or launched."""
+    if not 1 <= int(seg_len) <= ARG16_MAX_SEG_LEN:
+        raise _lib.XClipB200Error(f"filip 16-bit argmax: seg_len {seg_len} is outside [1, {ARG16_MAX_SEG_LEN}]")
+
+
+def filip_segmax16(a, b, temp_exp, seg_len, col_mul, col_add, want_max=True, seg_arg=None):
+    """filip_segmax with the compact argmax: -> (seg_max f32 [R, nseg] or None, seg_arg int16 [R, nseg]
+    holding the unsigned 16-bit index, or None).  seg_arg may be a preallocated contiguous int16
+    [R, nseg] (a slice of a saved buffer); pass seg_arg=False for seg_max only."""
+    check_arg16_seg_len(seg_len)
+    _need(a, BF16, "a"); _need(b, BF16, "b")
+    R, D = a.shape
+    C = b.shape[0]
+    nseg = C // seg_len
+    seg_max = torch.empty((R, nseg), device=a.device, dtype=F32) if want_max else None
+    if seg_arg is None:
+        seg_arg = torch.empty((R, nseg), device=a.device, dtype=torch.int16)
+    elif seg_arg is False:
+        seg_arg = None
+    elif seg_arg.dtype != torch.int16 or seg_arg.shape != (R, nseg) or not seg_arg.is_contiguous():
+        raise _lib.XClipB200Error(f"filip_segmax16: seg_arg must be a contiguous int16 [{R}, {nseg}]")
+    keys = torch.empty((R, nseg), device=a.device, dtype=torch.int64)
+    _call(a, "filip_segmax", 2.0 * R * C * D,
+          2.0 * (R + C) * D + (16.0 + (4.0 if want_max else 0.0) + (2.0 if seg_arg is not None else 0.0)) * R * nseg,
+          "xclip_filip_segmax_arg16", a.data_ptr(), b.data_ptr(), R, C, D, temp_exp.data_ptr(), int(seg_len),
+          _ptr(col_mul), _ptr(col_add), _ptr(seg_max), _ptr(seg_arg), keys.data_ptr())
+    return seg_max, seg_arg
+
+
+def filip_expand16(seg_arg, wmat, rowscale, temp_exp, row0, rows_per_sample, seg_len, nseg):
+    """filip_expand on a compact int16 argmax holding rows [row0, row0 + seg_arg.shape[0]) only; no
+    d temperature.  Same G bits and layout as filip_expand."""
+    check_arg16_seg_len(seg_len)
+    if seg_arg.dtype != torch.int16 or seg_arg.dim() != 2 or seg_arg.shape[1] != nseg or not seg_arg.is_contiguous():
+        raise _lib.XClipB200Error(f"filip_expand16: seg_arg must be a contiguous int16 [rows, {nseg}]")
+    rows = seg_arg.shape[0]
+    C = nseg * seg_len
+    g = torch.empty((rows, (C + 7) // 8 * 8), device=seg_arg.device, dtype=BF16)
+    _call(seg_arg, "filip_expand", 0.0, 2.0 * g.numel(), "xclip_filip_expand16", seg_arg.data_ptr(),
+          wmat.data_ptr(), rowscale.data_ptr(), temp_exp.data_ptr(), int(row0), int(rows),
+          int(rows_per_sample), int(seg_len), int(nseg), g.data_ptr(), g.stride(0))
+    return g[:, :C]
+
+
 def text_embed_fwd(ids, tok, pos, cls):
     """ids int64 [B,n] -> bf16 [B, n+1, d] = [cls | tok[ids] + pos]."""
     if ids.dtype != torch.int64 or not ids.is_cuda:
