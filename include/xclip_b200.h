@@ -175,6 +175,28 @@ int xclip_nce_bwd(const void* a, const void* b, int R, int C, int D, const float
                   float w_row, float w_col, float w_diag, const float* gscale, void* g,
                   int64_t ldg, float* dtemp, xclip_stream_t stream);
 
+/* ---- vocabulary cross-entropy of the MLM head (x_clip/mlm.py:96-107) on the same kernels ----------
+ * l[r,v] = <x_r, w_v> + bias[v] for x bf16 [R,D] (the selected token encodings), w bf16 [V,D] (the
+ * bf16 cast of to_logits.weight), bias f32 [V] or NULL; labels int64 [R] hold each row's target in
+ * [0, V) (the caller checks the range: a label outside it gives an undefined loss and gradient, never
+ * an out-of-bounds access).  Any V >= 1: the columns past V are masked inside the kernel.
+ * fwd:  lse[r] = log sum_v exp(l[r,v]), pos[r] = l[r, labels[r]], both f32 [R], with an online
+ *       maximum; *loss_accum += loss_scale * sum_r (lse[r] - pos[r]) (loss_accum may be NULL).
+ *       part_ws: f32 scratch [2 * xclip_nce_num_col_blocks(V) * R], 8-byte aligned.  The [R, V]
+ *       logits are never written.
+ * bwd:  g[r,v] = bf16(*gscale * (exp(l[r,v] - lse[r]) - [v == labels[r]])) (gscale: DEVICE scalar),
+ *       written as [R, ldg], ldg % 8 == 0, ldg >= roundup8(V), zero in the columns [V, ldg).
+ *       dx = g[:, :V] w, dW = g[:, :V]^T x and dbias = column sums then run on xclip_gemm_bf16 and
+ *       xclip_colsum_rows; the caller bounds R (a window of rows) to bound g.
+ * x, w, g 16-byte aligned, bias 16-byte aligned, labels 8-byte aligned, D % 8 == 0; otherwise
+ * both calls return XCLIP_ERR_INVALID without launching. */
+int xclip_vocab_ce_fwd(const void* x, const void* w, const float* bias, const int64_t* labels, int R,
+                       int V, int D, float* part_ws, float* pos, float* lse, float* loss_accum,
+                       float loss_scale, xclip_stream_t stream);
+int xclip_vocab_ce_bwd(const void* x, const void* w, const float* bias, const int64_t* labels, int R,
+                       int V, int D, const float* lse, const float* gscale, void* g, int64_t ldg,
+                       xclip_stream_t stream);
+
 /* ---- similarity regularisation (arXiv 2309.08773; x_clip/x_clip.py:771-784, :870-873) ----------
  * E[r,c] = <t_r, t_c> - <v_r, v_c> for LOCAL rows r and ALL columns c of the global batch, formed in
  * the fp32 accumulator as one contraction a . b^T of the concatenated operands

@@ -5,10 +5,11 @@ language modelling on the text transformer), `SimSiam` / `SimCLR` (x_clip/visual
 BYOL-style wrapper around the vision transformer) and mixes their losses into the contrastive
 loss (x_clip/x_clip.py:611-621, :851-868).  Here the same objectives are written against the
 H100 encoders of this package: the expensive part - every encoder pass - runs on the CUDA kernels
-(engine.TransformerFn), the vocabulary projection of the MLM head runs on the wgmma GEMM over the
-MASKED positions only (engine.LinearFn), and the small heads (cross entropy over the selected
-rows, BatchNorm MLPs, cosine / NT-Xent losses, torchvision augmentations) stay ordinary torch
-modules, exactly as in the reference - they are not on the north-star path.
+(engine.TransformerFn), the MLM head's vocabulary projection and its cross entropy run as one
+wgmma GEMM with the softmax in its epilogue over the MASKED positions only
+(engine.VocabCrossEntropyFn: no [n_sel, V] logits, any vocabulary size), and the small heads
+(BatchNorm MLPs, cosine / NT-Xent losses, torchvision augmentations) stay ordinary torch modules,
+exactly as in the reference - they are not on the north-star path.
 
 Parameter names follow the reference (`mlm.to_logits.*`, `visual_ssl.online_encoder.*`) where the
 reference has parameters; masks and augmentations are random in both implementations, so parity is
@@ -24,8 +25,6 @@ import torch.nn.functional as F
 from torch import nn
 
 from . import engine as E
-
-BF16 = torch.bfloat16
 
 
 # ----------------------------------------------------------------------------- MLM
@@ -83,12 +82,9 @@ class MLM(nn.Module):
         rows = enc[sel]                                                       # [n_sel, dim] bf16
         if rows.shape[0] == 0:
             return enc.sum() * 0.
-        if rows.is_cuda and rows.dtype == BF16 and self.num_tokens % 8 == 0:
-            logits = E.LinearFn.apply(rows.contiguous(), self.to_logits.weight, self.to_logits.bias, None)
-        else:                           # vocabulary not a multiple of 8 (e.g. 10000 + [MASK]): torch matmul
-            logits = F.linear(rows.float(), self.to_logits.weight, self.to_logits.bias)
-        # mean over the selected positions == F.cross_entropy(..., ignore_index=pad) of the reference
-        return F.cross_entropy(logits.float(), labels[sel])
+        # mean over the selected positions == F.cross_entropy(..., ignore_index=pad) of the reference,
+        # fused into the vocabulary GEMM for any vocabulary size: no [n_sel, V] logits are written
+        return E.VocabCrossEntropyFn.apply(rows, self.to_logits.weight, self.to_logits.bias, labels[sel])
 
     def forward(self, seq: torch.Tensor, **kwargs) -> torch.Tensor:
         masked, labels = self.corrupt(seq)
@@ -136,10 +132,13 @@ class _Projected(nn.Module):
         self.net = net
         self.projector = _mlp(rep_dim, projection_size, hidden)
 
-    def forward(self, x):
+    def rep(self, x):
         rep = self.net(x)
         rep = rep[:, 0] if rep.ndim == 3 else rep
-        rep = rep.float()
+        return rep.float()
+
+    def forward(self, x):
+        rep = self.rep(x)
         return self.projector(rep), rep
 
 
@@ -165,13 +164,23 @@ class SimSiam(nn.Module):
         assert not (self.training and x.shape[0] == 1), \
             'you must have greater than 1 sample when training, due to the batchnorm in the projection layer'
         one, two = self.augment1(x), self.augment2(x)
-        p1, _ = self.online_encoder(one)
-        p2, _ = self.online_encoder(two)
+        enc = self.online_encoder
+        r1, r2 = enc.rep(one), enc.rep(two)
+        with torch.no_grad():
+            t1, t2 = enc.rep(one), enc.rep(two)
+        return self.loss_from_reps(r1, r2, t1, t2)
+
+    def loss_from_reps(self, r1, r2, t1, t2):
+        """The head on the encoders' CLS representations: r1 / r2 of the two views (with gradient),
+        t1 / t2 the same views encoded again without gradient (their own patch-dropout draws).  The
+        BatchNorm layers run in the order of the reference's forward: projector on r1, r2, predictor on
+        both, projector on t1, t2 - so their running statistics end as they would there."""
+        proj = self.online_encoder.projector
+        p1, p2 = proj(r1), proj(r2)
         q1, q2 = self.online_predictor(p1), self.online_predictor(p2)
         with torch.no_grad():
-            t1, _ = self.online_encoder(one)
-            t2, _ = self.online_encoder(two)
-        return (self._neg_cos(q1, t2.detach()) + self._neg_cos(q2, t1.detach())).mean()
+            z1, z2 = proj(t1), proj(t2)
+        return (self._neg_cos(q1, z2.detach()) + self._neg_cos(q2, z1.detach())).mean()
 
 
 class SimCLR(nn.Module):
@@ -189,11 +198,14 @@ class SimCLR(nn.Module):
         self.augment2 = augment_fn2 if augment_fn2 is not None else self.augment1
 
     def forward(self, x):
-        b = x.shape[0]
-        q, _ = self.net(self.augment1(x))
-        k, _ = self.net(self.augment2(x))
+        return self.loss_from_reps(self.net.rep(self.augment1(x)), self.net.rep(self.augment2(x)))
+
+    def loss_from_reps(self, r1, r2):
+        """NT-Xent on the encoders' CLS representations of the two views."""
+        b = r1.shape[0]
+        q, k = self.net.projector(r1), self.net.projector(r2)
         z = torch.cat((q, k), dim=0)                 # (not normalised, as in the reference's nt_xent_loss)
         logits = z @ z.t() / self.temperature
-        logits = logits.masked_fill(torch.eye(2 * b, dtype=torch.bool, device=x.device), -torch.finfo(logits.dtype).max)
-        target = torch.cat((torch.arange(b, 2 * b), torch.arange(0, b))).to(x.device)
+        logits = logits.masked_fill(torch.eye(2 * b, dtype=torch.bool, device=z.device), -torch.finfo(logits.dtype).max)
+        target = torch.cat((torch.arange(b, 2 * b), torch.arange(0, b))).to(z.device)
         return F.cross_entropy(logits, target)

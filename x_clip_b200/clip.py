@@ -480,6 +480,30 @@ class CLIP(nn.Module):
             ops += [ops_tx, ops_ix]
         return zs, ops
 
+    def _chunkable_ssl(self) -> bool:
+        """visual SSL the micro-batched step can split into encoder passes and a head"""
+        from .aux import SimCLR, SimSiam
+        return isinstance(self.visual_ssl, (SimSiam, SimCLR))
+
+    def _aux_inputs(self, text, image) -> dict:
+        """The random parts of the auxiliary losses for the whole batch, drawn once before any chunk
+        and in the single pass's order: the MLM corruption, then both augmentations (the reference's
+        augmentations draw one decision per call, so per-chunk augmentation would be another function)."""
+        aux = dict(mlm=None, ssl=None, ssl_encoder=None, ssl_targets=False)
+        if self.use_mlm:
+            masked, labels = self.mlm.corrupt(text)
+            sel = labels != self.mlm.pad_token_id
+            aux["mlm"] = (masked, sel, labels[sel])
+        if self.use_visual_ssl:
+            ssl = self.visual_ssl
+            assert image.shape[0] > 1, \
+                'you must have greater than 1 sample when training, due to the batchnorm in the projection layer'
+            aux["ssl"] = (ssl.augment1(image), ssl.augment2(image))
+            from .aux import SimSiam
+            aux["ssl_targets"] = isinstance(ssl, SimSiam)
+            aux["ssl_encoder"] = ssl.online_encoder if aux["ssl_targets"] else ssl.net
+        return aux
+
     def _project(self, embeds: torch.Tensor, linear: nn.Linear):
         """embeds [..., d] (any float dtype) -> (z fp32 [..., D], (zrow, zcol) bf16 [rows, 3D])."""
         lead = embeds.shape[:-1]
@@ -510,6 +534,18 @@ class CLIP(nn.Module):
 
         text_mask = text != self.text_pad_id
 
+        # large batches: the micro-batched step, auxiliary losses included (engine.ChunkedClipLossFn).
+        # Multiview, frozen towers, a custom visual_ssl module, and visual SSL on an image that wants a
+        # gradient run the single pass below.
+        if (return_loss and self.microbatch and text.shape[0] > self.microbatch
+                and aug_text is None and aug_image is None
+                and not (freeze_image_encoder or freeze_text_encoder)
+                and (not self.use_visual_ssl or (self._chunkable_ssl() and not image.requires_grad))):
+            assert self.training, 'loss cannot be used if not training'
+            aux = self._aux_inputs(text, image) if (self.use_mlm or self.use_visual_ssl) else None
+            return E.ChunkedClipLossFn.apply(self, text, image, text_mask, int(self.microbatch),
+                                             self.temperature, self.microbatch_retain, aux)
+
         # auxiliary losses on the un-augmented batch (reference :616-621)
         text_ssl_loss = image_ssl_loss = 0
         if return_loss:
@@ -538,10 +574,6 @@ class CLIP(nn.Module):
                  "multiview with use_all_token_embeds is not implemented")
 
         has_aux = is_multiview or self.use_mlm or self.use_visual_ssl
-        if (return_loss and self.microbatch and text.shape[0] > self.microbatch and not has_aux
-                and not (freeze_image_encoder or freeze_text_encoder)):
-            return E.ChunkedClipLossFn.apply(self, text, image, text_mask, int(self.microbatch),
-                                             self.temperature, self.microbatch_retain)
         text_args = (text,) if self.text_encode_without_mask else (text, text_mask)
         enc_text = _encode(self.text_transformer, text_args, freeze_text_encoder)
         if self.text_causal_mask:
@@ -583,7 +615,13 @@ class CLIP(nn.Module):
 
         if self.use_all_token_embeds:
             from .filip import filip_loss
-            return filip_loss(self, zt, zi, zt_x, zi_x, ops, text_mask)
+            loss = filip_loss(self, zt, zi, zt_x, zi_x, ops, text_mask)
+            if not has_aux:
+                return loss
+            # weighted with the auxiliary terms as the reference does (:851-865); multiview was refused
+            cl_w = 1 - (self.text_ssl_loss_weight + self.image_ssl_loss_weight)
+            return loss * cl_w + text_ssl_loss * self.text_ssl_loss_weight \
+                + image_ssl_loss * self.image_ssl_loss_weight
 
         def cl(tsl, isl, *sim_reg):
             """contrastive loss of text view rows `tsl` against image view rows `isl`; sim_reg =

@@ -71,6 +71,7 @@ struct GemmParams {
   float* dtemp;          // BWD: scalar accumulator of sum(g * s) or null
   const float* alpha_dev;  // NCE: exp(temperature) read from device memory (no host sync)
   const float* gscale_dev; // BWD: upstream scalar gradient / (2*B_global), multiplies the weights
+  const long long* labels; // EPI_VCE_*: [M] column of each row's target (the positive)
   // ---- FILIP segment-max epilogue (EPI_SEGMAX): columns are grouped in segments of seg_len
   // tokens (one segment = one sample of the other modality); the result goes to one packed key
   // per (row, segment) (segmax_key), zeroed before the launch
@@ -126,6 +127,13 @@ constexpr int EPI_FF_BWD = 6;
 //   EPI_SIMREG_BWD  C = bf16(*gscale_dev * E), zero on the excluded columns up to ldc
 constexpr int EPI_SIMREG_FWD = 7;
 constexpr int EPI_SIMREG_BWD = 8;
+// Vocabulary cross-entropy (nce.cu): logits l = acc + bias[c] over the N = V columns, the target
+// of row r is column labels[r]; columns >= N are masked here, so any V >= 1 works.
+//   EPI_VCE_FWD  nce_part[n_blk * M + row] = (max, sum of 2^(x - max)) over the block, x = l log2(e);
+//                nce_pos[row] = l[row, labels[row]]
+//   EPI_VCE_BWD  C = bf16(*gscale_dev * (exp(l - lse_row[row]) - [c == labels[row]])), zero in [N, ldc)
+constexpr int EPI_VCE_FWD = 9;
+constexpr int EPI_VCE_BWD = 10;
 
 constexpr int kGemmBlockM = 128;
 constexpr int kGemmBlockK = 64;
@@ -221,6 +229,22 @@ __device__ __forceinline__ float segmax_key_value(unsigned long long k) {
 }
 __device__ __forceinline__ int segmax_key_index(unsigned long long k) {
   return static_cast<int>(0xFFFFFFFFu - static_cast<uint32_t>(k));
+}
+
+// EPI_VCE_*: v[i] += bias[col0 + i] over the columns < N (bias 16-byte aligned, or null)
+__device__ __forceinline__ void vce_add_bias(const GemmParams& p, int col0, float (&v)[32]) {
+  if (p.bias == nullptr) return;
+  if (col0 + 32 <= p.N) {
+#pragma unroll
+    for (int i = 0; i < 32; i += 4) {
+      const float4 b4 = __ldg(reinterpret_cast<const float4*>(p.bias + col0 + i));
+      v[i] += b4.x; v[i + 1] += b4.y; v[i + 2] += b4.z; v[i + 3] += b4.w;
+    }
+  } else {
+#pragma unroll
+    for (int i = 0; i < 32; ++i)
+      if (col0 + i < p.N) v[i] += __ldg(p.bias + col0 + i);
+  }
 }
 
 // Epilogue of one 128 x BLOCK_N tile for EPI_STORE; `stage(c)` makes column c of the tile readable.
@@ -879,6 +903,74 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         for (int i = 0; i < 32; ++i) s4[i & 3] = fmaf(v[i], v[i], s4[i & 3]);
       }
       if (row_ok) p.nce_part[(long long)n_blk * p.M + row] = (s4[0] + s4[1]) + (s4[2] + s4[3]);
+    } else if constexpr (EPI == EPI_VCE_FWD) {
+      // EPI_NCE_FWD's online (max, sum) per 32-column chunk, on l = acc + bias
+      constexpr float kLog2e = 1.4426950408889634f;
+      const long long label = row_ok ? p.labels[row] : -1;
+      float run_m = -INFINITY, run_s = 0.f;
+#pragma unroll 1
+      for (int c = 0; c < BLOCK_N / 32; ++c) {
+        need(c * 32);
+        const int col0 = n_blk * BLOCK_N + c * 32;
+        if (col0 >= p.N) continue;
+        float v[32];
+        acc_ld32(acc_row, acc_sw, c * 32, v);
+        vce_add_bias(p, col0, v);
+        if (label >= col0 && label < col0 + 32) {
+#pragma unroll
+          for (int i = 0; i < 32; ++i)
+            if (col0 + i == label) p.nce_pos[row] = v[i];
+        }
+        float cm = -INFINITY;
+        if (col0 + 32 <= p.N) {
+#pragma unroll
+          for (int i = 0; i < 32; ++i) cm = fmaxf(cm, v[i]);
+        } else {
+#pragma unroll
+          for (int i = 0; i < 32; ++i) {
+            if (col0 + i >= p.N) v[i] = -INFINITY;        // not in the sum
+            cm = fmaxf(cm, v[i]);
+          }
+        }
+        cm *= kLog2e;
+        if (cm > run_m) { run_s *= exp2f(run_m - cm); run_m = cm; }
+#pragma unroll
+        for (int i = 0; i < 32; ++i) run_s += exp2f(fmaf(v[i], kLog2e, -run_m));
+      }
+      if (row_ok) {
+        float2* dst = reinterpret_cast<float2*>(p.nce_part) + ((long long)n_blk * p.M + row);
+        *dst = make_float2(run_m, run_s);
+      }
+    } else if constexpr (EPI == EPI_VCE_BWD) {
+      constexpr float kLog2e = 1.4426950408889634f;
+      const float gs = __ldg(p.gscale_dev);
+      const long long label = row_ok ? p.labels[row] : -1;
+      const float lr2 = row_ok ? p.lse_row[row] * kLog2e : 0.f;
+#pragma unroll 1
+      for (int c = 0; c < BLOCK_N / 32; ++c) {
+        need(c * 32);
+        const int col0 = n_blk * BLOCK_N + c * 32;
+        if (!row_ok || col0 >= (int)p.ldc) continue;   // pad columns [N, ldc) get zeros
+        float v[32];
+        acc_ld32(acc_row, acc_sw, c * 32, v);
+        vce_add_bias(p, col0, v);
+#pragma unroll
+        for (int i = 0; i < 32; ++i) v[i] = gs * nce_ex2(fmaf(v[i], kLog2e, -lr2));
+        if (col0 + 32 > p.N) {
+#pragma unroll
+          for (int i = 0; i < 32; ++i)
+            if (col0 + i >= p.N) v[i] = 0.f;
+        }
+        if (label >= col0 && label < col0 + 32) {
+#pragma unroll
+          for (int i = 0; i < 32; ++i)
+            if (col0 + i == label) v[i] -= gs;
+        }
+        bf16* grow = reinterpret_cast<bf16*>(p.c) + (long long)row * p.ldc + col0;
+#pragma unroll
+        for (int i = 0; i < 32; i += 8)
+          if (col0 + i < (int)p.ldc) st_bf16x8(grow + i, v + i);
+      }
     } else if constexpr (EPI == EPI_SIMREG_BWD) {
       const float gs = __ldg(p.gscale_dev);
       const int diag_col = row + p.diag_offset;

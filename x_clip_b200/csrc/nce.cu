@@ -13,6 +13,9 @@
 // Rows are the LOCAL samples of one modality, columns ALL samples of the other one, so under
 // data parallelism each rank evaluates only its B_g/W row block (SURVEY.md 8e) instead of the
 // reference's redundant full matrix.
+//
+// The MLM head's cross-entropy over the vocabulary (xclip_vocab_ce_*, end of file) is the same
+// softmax with a bias, a label column as the positive and no temperature.
 #include "gemm.cuh"
 #include "host.h"
 
@@ -145,4 +148,65 @@ extern "C" int xclip_nce_bwd(const void* a, const void* b, int R, int C, int D,
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   return block_n == 256 ? launch_nce<256, EPI_NCE_BWD>(tmA, tmB, p, grid, s)
                         : launch_nce<128, EPI_NCE_BWD>(tmA, tmB, p, grid, s);
+}
+
+// ---- vocabulary cross-entropy: the MLM head's F.cross_entropy(x W^T + b, labels) on the same
+// mainloop.  Rows are the selected token encodings, columns the V vocabulary rows of W; the
+// positive of row r is column labels[r] instead of a diagonal.  The forward reuses the InfoNCE
+// partials and finalize, so the [R, V] logits are never written.
+
+static int vce_check(const float* bias, const int64_t* labels, const char* what) {
+  XCLIP_REQUIRE(labels, "%s: null labels", what);
+  XCLIP_REQUIRE(bias == nullptr || (reinterpret_cast<uintptr_t>(bias) & 15) == 0,
+                "%s: bias must be 16-byte aligned (it is read as float4)", what);
+  XCLIP_REQUIRE((reinterpret_cast<uintptr_t>(labels) & 7) == 0, "%s: misaligned labels", what);
+  return XCLIP_OK;
+}
+
+extern "C" int xclip_vocab_ce_fwd(const void* x, const void* w, const float* bias, const int64_t* labels,
+                                  int R, int V, int D, float* part_ws, float* pos, float* lse,
+                                  float* loss_accum, float loss_scale, xclip_stream_t stream) {
+  GemmParams p;
+  CUtensorMap tmA, tmB;
+  int block_n = 0, grid = 0;
+  int rc = nce_common(x, w, R, V, D, &p, &tmA, &tmB, &block_n, &grid);
+  if (rc) return rc;
+  rc = vce_check(bias, labels, "vocab_ce_fwd");
+  if (rc) return rc;
+  XCLIP_REQUIRE(part_ws && pos && lse, "vocab_ce_fwd: null workspace/output");
+  XCLIP_REQUIRE((reinterpret_cast<uintptr_t>(part_ws) & 7) == 0,
+                "vocab_ce_fwd: part_ws must be 8-byte aligned (float2 partials)");
+  p.bias = bias; p.labels = reinterpret_cast<const long long*>(labels);
+  p.nce_part = part_ws; p.nce_pos = pos;
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  rc = block_n == 256 ? launch_nce<256, EPI_VCE_FWD>(tmA, tmB, p, grid, s)
+                      : launch_nce<128, EPI_VCE_FWD>(tmA, tmB, p, grid, s);
+  if (rc) return rc;
+  const int nblk = xclip_nce_num_col_blocks(V);
+  int fgrid = (R + 1023) / 1024;
+  if (fgrid > num_sms()) fgrid = num_sms();
+  nce_finalize_kernel<<<fgrid, 1024, 0, s>>>(part_ws, nblk, pos, R, nullptr, lse, loss_accum, loss_scale);
+  XCLIP_LAUNCH_CHECK("nce_finalize_kernel");
+  return XCLIP_OK;
+}
+
+extern "C" int xclip_vocab_ce_bwd(const void* x, const void* w, const float* bias, const int64_t* labels,
+                                  int R, int V, int D, const float* lse, const float* gscale, void* g,
+                                  int64_t ldg, xclip_stream_t stream) {
+  GemmParams p;
+  CUtensorMap tmA, tmB;
+  int block_n = 0, grid = 0;
+  int rc = nce_common(x, w, R, V, D, &p, &tmA, &tmB, &block_n, &grid);
+  if (rc) return rc;
+  rc = vce_check(bias, labels, "vocab_ce_bwd");
+  if (rc) return rc;
+  XCLIP_REQUIRE(g && ldg % 8 == 0 && ldg >= (V + 7) / 8 * 8, "vocab_ce_bwd: g needs ld >= roundup8(V)");
+  XCLIP_REQUIRE((reinterpret_cast<uintptr_t>(g) & 15) == 0, "vocab_ce_bwd: misaligned g");
+  XCLIP_REQUIRE(lse && gscale, "vocab_ce_bwd: lse / gscale required");
+  p.bias = bias; p.labels = reinterpret_cast<const long long*>(labels);
+  p.lse_row = lse; p.gscale_dev = gscale;
+  p.c = g; p.ldc = ldg;
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  return block_n == 256 ? launch_nce<256, EPI_VCE_BWD>(tmA, tmB, p, grid, s)
+                        : launch_nce<128, EPI_VCE_BWD>(tmA, tmB, p, grid, s);
 }

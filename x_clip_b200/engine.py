@@ -623,6 +623,87 @@ class ContrastiveLossFn(torch.autograd.Function):
         return grads + (None,) * (len(ctx.needs_input_grad) - len(grads))
 
 
+# bytes of one backward window of the vocabulary cross-entropy's g [rows, roundup8(V)] bf16: at the
+# CLIP BPE vocabulary (V = 49408) that is 10752 rows, against 2.4 G logits for 49 k selected rows
+VOCAB_CE_WINDOW_BYTES = 1 << 30
+
+
+def vocab_window_rows(n: int, V: int, budget: int = None) -> int:
+    """Rows of one backward window of g [rows, roundup8(V)] bf16 within `budget` bytes: all n rows
+    when they fit, else a multiple of 128 rows where that many fit, else at least 1."""
+    budget = VOCAB_CE_WINDOW_BYTES if budget is None else budget
+    rows = budget // (2 * ((V + 7) // 8 * 8))
+    if rows >= n:
+        return n
+    return rows // 128 * 128 if rows >= 128 else max(rows, 1)
+
+
+def check_labels(labels: torch.Tensor, V: int) -> None:
+    """Raise, as F.cross_entropy does, on a target outside [0, V).  The comparison stays on the
+    device: for CUDA labels the error is a device-side assert, reported by the next synchronising
+    call, and no host synchronisation is added to the step; for CPU labels it raises here."""
+    torch._assert_async(((labels >= 0) & (labels < V)).all(), "x_clip_b200: cross-entropy target out of bounds")
+
+
+class VocabCrossEntropyFn(torch.autograd.Function):
+    """F.cross_entropy(rows @ weight^T + bias, labels): the mean over the n rows of lse - target
+    logit (reference mlm.py:105-107 on the selected positions).
+
+    rows bf16 [n, d] (n >= 1), weight fp32 [V, d], bias fp32 [V] or None, labels int64 [n] in
+    [0, V) for any V >= 1.  Forward: xclip_vocab_ce_fwd, the softmax reduced inside the GEMM
+    epilogue, so no [n, V] logits exist.  Backward: g = gscale (softmax - onehot) in row windows
+    of VOCAB_CE_WINDOW_BYTES (xclip_vocab_ce_bwd recomputes the logits), then d rows = g W,
+    d weight = g^T rows and d bias = column sums of g - each only when its input needs a gradient.
+    A label outside [0, V) raises as in torch, through a device-side assert (no host sync)."""
+
+    @staticmethod
+    def forward(ctx, rows, weight, bias, labels):
+        rows = rows.contiguous()
+        if rows.dtype != BF16:
+            rows = rows.to(BF16)
+        labels = labels.contiguous()
+        n, V = rows.shape[0], weight.shape[0]
+        check_labels(labels, V)
+        wb = weight_bf16(weight)
+        b = None if bias is None else bias.detach().contiguous()
+        loss = torch.zeros(1, device=rows.device, dtype=F32)
+        lse, _ = K.vocab_ce_fwd(rows, wb, b, labels, loss, 1.0 / n)
+        # the bias as given: autograd's version check refuses a backward after an in-place update
+        # (wb is already this call's own copy of the weight)
+        ctx.save_for_backward(rows, wb, labels, lse, bias)
+        return loss.reshape(())
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gloss):
+        rows, wb, labels, lse, bias = ctx.saved_tensors
+        b = None if bias is None else bias.detach().contiguous()
+        need_x, need_w, need_b = ctx.needs_input_grad[:3]
+        n, d = rows.shape
+        V = wb.shape[0]
+        dev = rows.device
+        gscale = (gloss.detach().float() / n).reshape(1)
+        dx = torch.empty((n, d), device=dev, dtype=BF16) if need_x else None
+        dw = torch.zeros((V, d), device=dev, dtype=F32) if need_w else None
+        db = torch.zeros(((V + 7) // 8 * 8,), device=dev, dtype=F32) if need_b else None
+        if need_x or need_w or need_b:
+            win = vocab_window_rows(n, V)
+            gbuf = torch.empty((win, (V + 7) // 8 * 8), device=dev, dtype=BF16)
+            for r0 in range(0, n, win):
+                r1 = min(r0 + win, n)
+                x = rows[r0:r1]
+                g = K.vocab_ce_bwd(x, wb, b, labels[r0:r1], lse[r0:r1], gscale, out=gbuf[: r1 - r0])
+                gv = g[:, :V]
+                if need_x:
+                    K.gemm(gv, wb, b_major=1, out=dx[r0:r1])
+                if need_w:
+                    K.gemm(gv, x, a_major=1, b_major=1, out=dw, accumulate=True)
+                if need_b:
+                    K.colsum_rows_(db, g)                 # the pad columns of g are zero
+            del gbuf
+        return dx, dw, None if db is None else db[:V], None
+
+
 def _pad_rows(m: torch.Tensor, rows: int) -> torch.Tensor:
     """g has roundup8(C) columns; the matching operand needs that many rows (zeros beyond C)."""
     if m.shape[0] == rows:
@@ -666,6 +747,56 @@ class _InPlaceGradAccumulation:
         return False
 
 
+def _chunk_passes(clip, text, image, text_mask, aux, s: int, e: int, img_k=None):
+    """The gradient passes of chunk [s, e), in a fixed order: contrastive encoders, then the MLM text
+    pass on the corrupted rows, then the two augmented image views.  Each image pass draws its
+    patch-dropout keep from the RNG stream in that order, so a re-encode from the chunk's saved RNG
+    state draws the keeps of the forward.  -> (outputs, ops): the latents, then the encodings of the
+    chunk's MLM-selected positions [n_sel, d] and the CLS representations of both views [e - s, rep]."""
+    z, ops = clip._encode_to_latents(text[s:e], image[s:e] if img_k is None else img_k, text_mask[s:e])
+    outs = list(z)
+    if aux is not None:
+        if aux["mlm"] is not None:
+            masked, sel, _ = aux["mlm"]
+            enc = clip.mlm.transformer(masked[s:e], mask=text_mask[s:e])[:, 1:]
+            outs.append(enc[sel[s:e]])
+        if aux["ssl"] is not None:
+            one, two = aux["ssl"]
+            outs += [aux["ssl_encoder"].rep(one[s:e]), aux["ssl_encoder"].rep(two[s:e])]
+    return outs, ops
+
+
+def _chunk_targets(aux, s: int, e: int):
+    """SimSiam's target passes of chunk [s, e): both views encoded again without gradient (their own
+    patch-dropout draws, after the gradient passes), never kept for backward."""
+    one, two = aux["ssl"]
+    enc = aux["ssl_encoder"]
+    with torch.no_grad():
+        return enc.rep(one[s:e]), enc.rep(two[s:e])
+
+
+def _aux_losses(clip, aux, leaves, targets):
+    """(MLM loss, visual SSL loss) on the full-batch leaves, each None when off."""
+    mlm = ssl = None
+    i = 0
+    if aux["mlm"] is not None:
+        rows, labels = leaves[i], aux["mlm"][2]
+        i += 1
+        head = clip.mlm.to_logits
+        # no selected position: the single pass's enc.sum() * 0
+        mlm = VocabCrossEntropyFn.apply(rows, head.weight, head.bias, labels) if rows.shape[0] else \
+            rows.sum() * 0.
+    if aux["ssl"] is not None:
+        r1, r2 = leaves[i], leaves[i + 1]
+        if aux["ssl_targets"]:
+            t1 = torch.cat([t[0] for t in targets])
+            t2 = torch.cat([t[1] for t in targets])
+            ssl = clip.visual_ssl.loss_from_reps(r1, r2, t1, t2)
+        else:
+            ssl = clip.visual_ssl.loss_from_reps(r1, r2)
+    return mlm, ssl
+
+
 class ChunkedClipLossFn(torch.autograd.Function):
     """Full-batch contrastive loss with micro-batched encoders.
 
@@ -685,14 +816,23 @@ class ChunkedClipLossFn(torch.autograd.Function):
     chunks cost no extra flops; each re-encoded chunk costs one extra encoder forward.
     An image that wants a gradient enters every chunk's encoder as a detached per-chunk leaf; backward
     collects the leaves' gradients into d loss / d image, so the outer graph (a generator, an
-    augmentation) is only ever entered by autograd itself, after this backward returns."""
+    augmentation) is only ever entered by autograd itself, after this backward returns.
+
+    `aux` (CLIP._aux_inputs) adds the auxiliary losses: the corruption (MLM) and both augmented views
+    (SimSiam / SimCLR) of the whole batch, drawn once before any chunk.  Every chunk runs its gradient
+    passes in one fixed order (_chunk_passes); the MLM encodings of the selected positions and the
+    views' CLS representations become full-batch leaves like the latents, and the heads (vocabulary
+    cross-entropy, projector / predictor with BatchNorm over the whole batch, NT-Xent) run once on
+    them.  SimSiam's target passes run chunk by chunk without gradient and are never kept.  The step
+    returns cl_w * contrastive + w_t * MLM + w_i * SSL, as the single pass does.  Retention keeps or
+    re-encodes a chunk with all of its gradient passes."""
 
     @staticmethod
-    def forward(ctx, clip, text, image, text_mask, chunk, temperature, retain="auto"):
+    def forward(ctx, clip, text, image, text_mask, chunk, temperature, retain="auto", aux=None):
         B = text.shape[0]
         dev = text.device
         bounds = [(s, min(s + chunk, B)) for s in range(0, B, chunk)]
-        rng_states, zs, opss, kept = [], [], [], []
+        rng_states, zs, opss, kept, targets = [], [], [], [], []
         want_dimage = image.requires_grad
         img_leaves = []                               # per retained chunk: its image leaf (or None)
 
@@ -734,7 +874,7 @@ class ChunkedClipLossFn(torch.autograd.Function):
                     img_k = chunk_image(s, e)
                     try:
                         with torch.enable_grad():
-                            z, ops = clip._encode_to_latents(text[s:e], img_k, text_mask[s:e])
+                            z, ops = _chunk_passes(clip, text, image, text_mask, aux, s, e, img_k)
                     except torch.OutOfMemoryError:
                         # the plan was too optimistic (a fragmented cache, memory taken by someone else
                         # since the estimate): this chunk and all later ones are re-encoded in backward
@@ -744,11 +884,13 @@ class ChunkedClipLossFn(torch.autograd.Function):
                     if z is None:
                         torch.cuda.empty_cache()
                         torch.cuda.set_rng_state(rng_states[-1], dev)
-                        z, ops = clip._encode_to_latents(text[s:e], image[s:e], text_mask[s:e])
+                        z, ops = _chunk_passes(clip, text, image, text_mask, aux, s, e)
                         kept.append(None)
                         img_leaves.append(None)
                         zs.append(z)
                         opss.append(ops)
+                        if aux is not None and aux["ssl_targets"]:
+                            targets.append(_chunk_targets(aux, s, e))
                         continue
                     kept.append(list(z))
                     img_leaves.append(img_k if want_dimage else None)
@@ -765,17 +907,28 @@ class ChunkedClipLossFn(torch.autograd.Function):
                             img_leaves[-1] = None
                     z = [t.detach() for t in z]
                 else:
-                    z, ops = clip._encode_to_latents(text[s:e], image[s:e], text_mask[s:e])
+                    z, ops = _chunk_passes(clip, text, image, text_mask, aux, s, e)
                     kept.append(None)
                     img_leaves.append(None)
                 zs.append(z)
                 opss.append(ops)
-        nsets = len(zs[0])
-        leaves = [torch.cat([z[j] for z in zs]).detach().requires_grad_(True) for j in range(nsets)]
+                if aux is not None and aux["ssl_targets"]:
+                    targets.append(_chunk_targets(aux, s, e))
+        # rows [start, end) of every chunk in each full-batch leaf (the MLM leaf has n_sel rows)
+        row_bounds, offs = [], [0] * len(zs[0])
+        for z in zs:
+            row_bounds.append([(offs[j], offs[j] + t.shape[0]) for j, t in enumerate(z)])
+            offs = [b for _, b in row_bounds[-1]]
+        nleaves = len(zs[0])
+        nsets = len(opss[0])
+        leaves = [torch.cat([z[j] for z in zs]).detach().requires_grad_(True) for j in range(nleaves)]
         ops_all = tuple((torch.cat([o[j][0] for o in opss]), torch.cat([o[j][1] for o in opss]))
                         for j in range(nsets))
         del zs, opss
         temp_leaf = temperature.detach().requires_grad_(True)
+        cl_w = 1.0
+        if aux is not None:
+            cl_w = 1 - (clip.text_ssl_loss_weight + clip.image_ssl_loss_weight)
         filip_stats = {} if filip else None
         with torch.enable_grad():
             if filip:
@@ -789,17 +942,31 @@ class ChunkedClipLossFn(torch.autograd.Function):
                     leaves[0], leaves[1], leaves[2] if nsets == 4 else None,
                     leaves[3] if nsets == 4 else None, temp_leaf, ops_all,
                     clip.decoupled_contrastive_learning, clip.requires_all_gather,
-                    *((clip.sim_reg_loss_weight, 1.0) if clip.has_sim_reg_loss else ()))
+                    *((clip.sim_reg_loss_weight, cl_w) if clip.has_sim_reg_loss else ()))
+            if aux is not None:
+                if not (clip.has_sim_reg_loss and not filip):      # sim-reg weighs its contrastive term itself
+                    loss = loss * cl_w
+                mlm_loss, ssl_loss = _aux_losses(clip, aux, leaves[nsets:], targets)
+                if mlm_loss is not None:
+                    loss = loss + mlm_loss * clip.text_ssl_loss_weight
+                if ssl_loss is not None:
+                    loss = loss + ssl_loss * clip.image_ssl_loss_weight
+        del targets
         ctx.clip, ctx.inputs = clip, (text, image, text_mask)
         ctx.bounds, ctx.rng_states, ctx.kept = bounds, rng_states, kept
+        ctx.aux, ctx.row_bounds = aux, row_bounds
         ctx.img_leaves = img_leaves if want_dimage else None
         ctx.graph = (loss, leaves, temp_leaf)
         ctx.weight_casts = wscope.cache
         n_kept = sum(z is not None for z in kept)
         if planned or (oom_fallbacks and plan_key in plans):
             plans[plan_key] = [z is not None for z in kept]    # WHICH chunks stay resident
+        passes = ["contrastive"]
+        if aux is not None:
+            passes += (["mlm"] if aux["mlm"] is not None else []) + (["view1", "view2"] if aux["ssl"] is not None else [])
         clip.last_step_plan = dict(chunks=len(bounds), retained=n_kept, chunk_activation_bytes=foot,
-                                   oom_fallbacks=oom_fallbacks)
+                                   oom_fallbacks=oom_fallbacks, passes=passes,
+                                   retained_chunks=[k for k, z in enumerate(kept) if z is not None])
         if filip:
             # rows of both FILIP passes whose argmax was saved / will be recomputed in backward
             clip.last_step_plan.update(filip=filip_stats, loss_reserve_bytes=reserve)
@@ -837,10 +1004,13 @@ class ChunkedClipLossFn(torch.autograd.Function):
                         torch.cuda.set_rng_state(ctx.rng_states[k], dev)
                         if dimage is not None:
                             img_k = image[s:e].detach().requires_grad_(True)
-                        z, _ = clip._encode_to_latents(text[s:e], image[s:e] if img_k is None else img_k,
-                                                       text_mask[s:e])
-                    torch.autograd.backward(list(z), [d[s:e] for d in dz])   # accumulates into .grad
-                    del z
+                        z, _ = _chunk_passes(clip, text, image, text_mask, ctx.aux, s, e, img_k)
+                    # accumulates into .grad; an output with no gradient or no rows in this chunk is skipped
+                    pairs = [(t, dz[j][a:b]) for j, (t, (a, b)) in enumerate(zip(z, ctx.row_bounds[k]))
+                             if dz[j] is not None and b > a and t.requires_grad]
+                    if pairs:
+                        torch.autograd.backward([t for t, _ in pairs], [d for _, d in pairs])
+                    del z, pairs
                     if img_k is not None:
                         if img_k.grad is None:
                             dimage[s:e].zero_()
@@ -848,5 +1018,5 @@ class ChunkedClipLossFn(torch.autograd.Function):
                             dimage[s:e].copy_(img_k.grad)
                         del img_k
         torch.cuda.set_rng_state(keep_state, dev)
-        ctx.graph = ctx.inputs = ctx.kept = ctx.weight_casts = ctx.img_leaves = None
-        return None, None, dimage, None, None, temp_leaf.grad, None
+        ctx.graph = ctx.inputs = ctx.kept = ctx.weight_casts = ctx.img_leaves = ctx.aux = None
+        return None, None, dimage, None, None, temp_leaf.grad, None, None

@@ -472,6 +472,54 @@ def nce_bwd(a, b, temp_exp, diag_offset, dcl, lse_row, lse_col, w_row, w_col, w_
     return g
 
 
+def _vocab_ce_args(x, w, bias, labels):
+    _need(x, BF16, "x"); _need(w, BF16, "w"); _rows2d(x, "x")
+    if not w.is_contiguous() or w.dim() != 2 or w.shape[1] != x.shape[1]:
+        raise _lib.XClipB200Error("vocab_ce: w must be a contiguous [V, d] with the rows' width")
+    if bias is not None:
+        _need(bias, F32, "bias")
+        if not bias.is_contiguous() or bias.numel() != w.shape[0]:
+            raise _lib.XClipB200Error("vocab_ce: bias must be a contiguous f32 [V]")
+    if labels.dtype != torch.int64 or labels.numel() != x.shape[0] or not labels.is_contiguous() \
+            or labels.device != x.device:
+        raise _lib.XClipB200Error("vocab_ce: labels must be a contiguous int64 [n] on the rows' device")
+    if x.stride(0) != x.shape[1]:
+        raise _lib.XClipB200Error("vocab_ce: rows must be contiguous")
+    return x.shape[0], w.shape[0], x.shape[1]
+
+
+def vocab_ce_fwd(x, w, bias, labels, loss_accum=None, loss_scale=0.0):
+    """(lse [n], target logit [n]) of l = x @ w^T + bias; loss_accum += loss_scale * sum(lse - target).
+    See xclip_vocab_ce_fwd."""
+    R, V, D = _vocab_ce_args(x, w, bias, labels)
+    nblk = _lib.load().xclip_nce_num_col_blocks(V)
+    part = torch.empty((nblk, R, 2), device=x.device, dtype=F32)
+    pos = torch.empty((R,), device=x.device, dtype=F32)
+    lse = torch.empty((R,), device=x.device, dtype=F32)
+    if loss_accum is not None:
+        _need(loss_accum, F32, "loss_accum")
+    _call(x, "vocab_ce_fwd", 2.0 * R * V * D, 2.0 * (R + V) * D + 8.0 * R, "xclip_vocab_ce_fwd", x.data_ptr(),
+          w.data_ptr(), _ptr(bias), labels.data_ptr(), R, V, D, part.data_ptr(), pos.data_ptr(), lse.data_ptr(),
+          _ptr(loss_accum), float(loss_scale))
+    return lse, pos
+
+
+def vocab_ce_bwd(x, w, bias, labels, lse, gscale, out=None):
+    """bf16 g [n, roundup8(V)] = gscale * (softmax(l) - onehot(labels)), zero in the columns >= V;
+    `out` may be a preallocated contiguous buffer of that shape.  See xclip_vocab_ce_bwd."""
+    R, V, D = _vocab_ce_args(x, w, bias, labels)
+    _need(lse, F32, "lse"); _need(gscale, F32, "gscale")
+    ldg = (V + 7) // 8 * 8
+    if out is None:
+        out = torch.empty((R, ldg), device=x.device, dtype=BF16)
+    elif out.dtype != BF16 or tuple(out.shape) != (R, ldg) or not out.is_contiguous():
+        raise _lib.XClipB200Error(f"vocab_ce_bwd: out must be a contiguous bf16 [{R}, {ldg}]")
+    _call(x, "vocab_ce_bwd", 2.0 * R * V * D, 2.0 * (R + V) * D + 2.0 * R * ldg, "xclip_vocab_ce_bwd",
+          x.data_ptr(), w.data_ptr(), _ptr(bias), labels.data_ptr(), R, V, D, lse.data_ptr(), gscale.data_ptr(),
+          out.data_ptr(), ldg)
+    return out
+
+
 def simreg_pack(t, v, negate_v):
     """bf16 [rows, 2k] = [t | v] or [t | -v] (see xclip_simreg_pack)."""
     _need(t, BF16, "t"); _need(v, BF16, "v")
