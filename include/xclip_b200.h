@@ -87,13 +87,6 @@ int xclip_layernorm_bwd(const void* dy, int64_t lddy, const void* x, int64_t ldx
                         const float* stats, const float* g, const void* add, int64_t ldadd,
                         void* dx, int64_t lddx, float* dg, int rows, int d,
                         xclip_stream_t stream);
-/* GEGLU + LayerNorm of FeedForward (x_clip/x_clip.py:180-183,:193): u = [value | gate] bf16
- * [rows, 2*dh]; h = LN(value * gelu_erf(gate)) * g, bf16 [rows, dh]; dh in 1024*{1,2,3,4}. */
-int xclip_geglu_ln_fwd(const void* u, int64_t ldu, const float* g, void* h, int64_t ldh,
-                       float* stats, int rows, int dh, float eps, xclip_stream_t stream);
-int xclip_geglu_ln_bwd(const void* dh_grad, int64_t lddh, const void* u, int64_t ldu,
-                       const float* stats, const float* g, void* du, int64_t lddu, float* dg,
-                       int rows, int dh, xclip_stream_t stream);
 /* l2norm = F.normalize(dim=-1, eps=1e-12) (x_clip/x_clip.py:54-55, used at :715,:724).
  * p f32 [rows,d] -> z f32 [rows,d], inv = 1/max(|p|,eps), and the split-bf16 operands of the
  * logits contraction: zrow = [hi|lo|hi], zcol = [hi|hi|lo], bf16 [rows,3d], hi = bf16(z),
@@ -222,18 +215,19 @@ int xclip_simreg_bwd(const void* a, const void* b, int R, int C, int K, int diag
                      const float* gscale, void* g, int64_t ldg, xclip_stream_t stream);
 
 /* ---- FILIP fine-grained loss (x_clip/x_clip.py:799-811 + :821-847) -----------------------
- * segmax_any : a bf16 [R,D] token latents of one modality, b bf16 [C,D] token latents of the
- *          other, C = n_samples * seg_len (seg_len >= 1 tokens per sample).  For every row r and
- *          sample y: seg_max[r,y] = max_i s, seg_arg[r,y] = argmax_i s with
+ * segmax_arg16 : a bf16 [R,D] token latents of one modality, b bf16 [C,D] token latents of the
+ *          other, C = n_samples * seg_len (1 <= seg_len <= 65535 tokens per sample).  For every row
+ *          r and sample y: seg_max[r,y] = max_i s (f32), seg_arg[r,y] = argmax_i s (16-bit, 2 bytes
+ *          per (row, sample): the saved state of a row-chunked FILIP loss) with
  *          s = *temp_exp * <a_r, b_(y,i)> (optionally s*col_mul[c] + col_add[c]: padded text
  *          tokens get col_mul 0 / col_add -FLT_MAX, the reference's masked_fill at :810).
- *          Ties go to the lowest index; a segment whose columns are all masked gives -FLT_MAX at
- *          index 0.
+ *          Either output may be null, not both.  Ties go to the lowest index; a segment whose
+ *          columns are all masked gives -FLT_MAX at index 0.
  *          keys: caller-owned workspace of 8 * R * (C / seg_len) bytes, 8-byte aligned, no
  *          initialisation needed (the call zeroes it; it holds nothing of use afterwards).  a, b
- *          16-byte aligned; temp_exp, seg_max, seg_arg, col_mul, col_add 4-byte aligned.
- *          Refused without a launch: seg_len < 1, C not a whole number of segments, null or
- *          misaligned pointers, only one of col_mul / col_add.
+ *          16-byte aligned; temp_exp, seg_max, col_mul, col_add 4-byte aligned, seg_arg 2-byte
+ *          aligned.  Refused without a launch: seg_len < 1 or > 65535, C not a whole number of
+ *          segments, both outputs null, null or misaligned pointers, only one of col_mul / col_add.
  * reduce : out[a,b] = sum_k weights[a*len+k] * seg_max[(a*len+k), b]  ([samples, nseg] or
  *          transposed) - the masked mean over text tokens (:807) / mean over image tokens (:811).
  * nce_fwd/bwd : row-wise InfoNCE / DCL on an [R,C] fp32 similarity matrix (R local texts, C all
@@ -242,17 +236,21 @@ int xclip_simreg_bwd(const void* a, const void* b, int R, int C, int K, int diag
  *          row with row_valid[x] == 0 (the image-to-text row of a caption without valid tokens)
  *          adds no loss, gets g = 0 and lse = 0 - as in the reference, where that row is
  *          exp(-inf) = 0 in both the positive and the denominator.
- * expand : rows [row0,row0+rows) of the backward operand G[R,C] (bf16): at the argmax column
+ * expand16 : rows [row0,row0+rows) of the backward operand G[R,C] (bf16): at the argmax column
  *          of each (row, sample) the value *temp_exp * wmat[row/rows_per_sample, sample] *
- *          rowscale[row], zero elsewhere; *dtemp += sum w * seg_max.  d rows = G @ b and
- *          d cols += G^T @ a then run on xclip_gemm_bf16.  Any seg_len >= 1; g is [rows, ldg]
- *          with ldg % 8 == 0 and ldg >= nseg * seg_len, 16-byte aligned.  Columns
- *          [nseg * seg_len, roundup8(nseg * seg_len)) are written as zeros, the rest of the row is
- *          left alone; the gradient GEMMs take G[:, :nseg * seg_len] and never read past it. */
-int xclip_filip_segmax_any(const void* a, const void* b, int R, int C, int D,
-                           const float* temp_exp, int seg_len, const float* col_mul,
-                           const float* col_add, float* seg_max, int* seg_arg, void* keys,
-                           xclip_stream_t stream);
+ *          rowscale[row], zero elsewhere.  seg_arg (from segmax_arg16) holds rows
+ *          [row0, row0 + rows) only: row r of G reads seg_arg[(r - row0) * nseg + y], while wmat
+ *          and rowscale are indexed by the global row.  d rows = G @ b and d cols += G^T @ a then
+ *          run on xclip_gemm_bf16; d loss / d log temperature is sum(d t2i * t2i) +
+ *          sum(d i2t * i2t) over the [B,B] matrices.  1 <= seg_len <= 65535; g is [rows, ldg]
+ *          with ldg % 8 == 0 and ldg >= nseg * seg_len, 16-byte aligned; seg_arg 2-byte aligned;
+ *          row0 >= 0.  Columns [nseg * seg_len, roundup8(nseg * seg_len)) are written as zeros,
+ *          the rest of the row is left alone; the gradient GEMMs take G[:, :nseg * seg_len] and
+ *          never read past it. */
+int xclip_filip_segmax_arg16(const void* a, const void* b, int R, int C, int D,
+                             const float* temp_exp, int seg_len, const float* col_mul,
+                             const float* col_add, float* seg_max, uint16_t* seg_arg, void* keys,
+                             xclip_stream_t stream);
 int xclip_filip_reduce(const float* seg_max, const float* weights, int samples, int len, int nseg,
                        float* out, int transpose_out, xclip_stream_t stream);
 int xclip_filip_nce_fwd(const float* s, int R, int C, int diag_off, int dcl,
@@ -261,24 +259,6 @@ int xclip_filip_nce_fwd(const float* s, int R, int C, int diag_off, int dcl,
 int xclip_filip_nce_bwd(const float* s, const float* lse, int R, int C, int diag_off, int dcl,
                         const unsigned char* row_valid, const float* gscale, float* g,
                         xclip_stream_t stream);
-int xclip_filip_expand(const int* seg_arg, const float* seg_max, const float* wmat,
-                       const float* rowscale, const float* temp_exp, int row0, int rows,
-                       int rows_per_sample, int seg_len, int nseg, void* g, int64_t ldg,
-                       float* dtemp, xclip_stream_t stream);
-/* Compact argmax, for the saved state of a row-chunked FILIP loss (2 bytes per (row, sample)
- * instead of 8):
- * segmax_arg16 : xclip_filip_segmax_any, writing seg_max (f32) and / or a 16-bit seg_arg; either
- *          may be null, not both.  Refused without a launch: seg_len > 65535, both outputs null,
- *          seg_max not 4-byte or seg_arg not 2-byte aligned, and every refusal of segmax_any.
- * expand16 : xclip_filip_expand on a 16-bit seg_arg that holds rows [row0, row0 + rows) only
- *          (row r of G reads seg_arg[(r - row0) * nseg + y]; wmat and rowscale are still indexed
- *          by the global row).  No seg_max and no dtemp: d loss / d log temperature is
- *          sum(d t2i * t2i) + sum(d i2t * i2t) over the [B,B] matrices.  Writes the same G bits
- *          as xclip_filip_expand.  seg_len <= 65535, seg_arg 2-byte aligned, otherwise as expand. */
-int xclip_filip_segmax_arg16(const void* a, const void* b, int R, int C, int D,
-                             const float* temp_exp, int seg_len, const float* col_mul,
-                             const float* col_add, float* seg_max, uint16_t* seg_arg, void* keys,
-                             xclip_stream_t stream);
 int xclip_filip_expand16(const uint16_t* seg_arg, const float* wmat, const float* rowscale,
                          const float* temp_exp, int row0, int rows, int rows_per_sample,
                          int seg_len, int nseg, void* g, int64_t ldg, xclip_stream_t stream);
@@ -300,7 +280,7 @@ int xclip_text_embed_bwd(const int64_t* ids, const void* dx, float* dtok, float*
  *                     holds 64 value rows and the 64 MATCHING gate rows.
  *   ff_scale_cast   : w2g = bf16(net.4.weight [d, 4d] * net.2.g [4d]) and colvec[j] = sum_k w2g[j,k].
  *   ff_up           : u = [value | gate] bf16 [M, 8d] (reference layout, kept for the backward),
- *                     hp = value * gelu_erf(gate) bf16 [M, 4d], rowsum[r, box] = (sum hp, sum hp^2) of
+ *                     hp = value * gelu(gate) bf16 [M, 4d], rowsum[r, box] = (sum hp, sum hp^2) of
  *                     every 64-column box (rowsum f32 [M, 4d/64, 2], fully overwritten: no atomics,
  *                     bit-reproducible) - one GEMM, GEGLU in its epilogue.
  *                     u may be NULL (forward-only sweeps: two thirds of the output traffic saved).

@@ -27,11 +27,12 @@ def test_header_symbols_exported_and_bound():
         assert n in names, f"{n} bound in python but not declared in the header"
 
 
-def test_abi_version_2_and_error_string_without_gpu():
-    """ABI 2: xclip_filip_segmax_any is the only segment-max entry point."""
+def test_abi_version_and_error_string_without_gpu():
+    """ABI 3: the FILIP segment-max and expand entry points take the 16-bit argmax only, and the
+    un-fused GEGLU + LayerNorm kernels are gone."""
     from x_clip_b200 import _lib
     lib = _lib.load()
-    assert lib.xclip_abi_version() == 2
+    assert lib.xclip_abi_version() == 3
     assert isinstance(lib.xclip_last_error(), bytes)
     assert lib.xclip_nce_num_col_blocks(1024) == 4
     assert lib.xclip_nce_num_col_blocks(100) == 1

@@ -1,7 +1,7 @@
 """FILIP models at token counts that are not multiples of 16, or exceed 256: cfg3's towers (77 text
 tokens against 196 image tokens, 98 under patch dropout), 300 text tokens against 576 image tokens
 (384 px / patch 16) and 7 text tokens against 9 image tokens (48 px / patch 16) at batch 33.  The
-segment-max GEMMs then run xclip_filip_segmax_any.  Goldens: tests/golden/{vitb16_shaped_filip,
+segment-max GEMMs then run xclip_filip_segmax_arg16.  Goldens: tests/golden/{vitb16_shaped_filip,
 vitb16_shaped_filip_drop, vitb16_shaped_filip_dcl_extra, filip_t300_i576, filip_t7_i9}.json, written
 by tests/golden/make_golden_filip_any.py."""
 import json

@@ -1,5 +1,5 @@
 """FILIP at any token count: the segment max at lengths that are not multiples of 16 or exceed a
-256-column tile (segments cut by one or more tile edges, merged through 64-bit keys), filip_expand
+256-column tile (segments cut by one or more tile edges, merged through 64-bit keys), filip_expand16
 at segment lengths that are not multiples of 8, and FilipLossFn at cfg3's 77 x 98 / 77 x 196, at
 300 x 576 and at 7 x 9 tokens, against the fp64 references and gates of test_gpu_filip."""
 import math
@@ -149,12 +149,11 @@ def test_expand_pad_columns_are_never_read(cuda_device, seg_len):
     gen = _gen(dev, 21 + seg_len)
     samples, rows_per_sample, nseg, D = 6, 40, 5, 128
     R, C = samples * rows_per_sample, nseg * seg_len
-    seg_arg = torch.randint(0, seg_len, (R, nseg), generator=gen, device=dev, dtype=torch.int32)
-    seg_max = torch.randn((R, nseg), generator=gen, device=dev)
+    seg_arg = torch.randint(0, seg_len, (R, nseg), generator=gen, device=dev, dtype=torch.int16)
     wmat = torch.randn((samples, nseg), generator=gen, device=dev)
     rowscale = torch.rand((R,), generator=gen, device=dev) + 0.5
     alpha = torch.tensor([3.0], device=dev, dtype=F32)
-    g = K.filip_expand(seg_arg, seg_max, wmat, rowscale, alpha, 0, R, rows_per_sample, seg_len, nseg, None)
+    g = K.filip_expand16(seg_arg, wmat, rowscale, alpha, 0, rows_per_sample, seg_len, nseg)
     ld = g.stride(0)
     assert g.shape == (R, C) and ld % 8 == 0 and ld >= C and ld > C
     full = g.as_strided((R, ld), (ld, 1))
@@ -211,6 +210,8 @@ def test_filip_loss_fn_cfg3_single_gpu(cuda_device):
 # --------------------------------------------------------------------------- refusals
 
 def test_segmax_any_and_expand_refuse_bad_arguments_without_launching(cuda_device):
+    """xclip_filip_segmax_arg16 and xclip_filip_expand16 refuse bad arguments before any launch; either
+    output of the segment max may be null, not both."""
     from x_clip_b200 import _lib
     lib = _lib.load()
     dev = cuda_device
@@ -220,7 +221,7 @@ def test_segmax_any_and_expand_refuse_bad_arguments_without_launching(cuda_devic
     b = torch.zeros((C + 8, D), device=dev, dtype=BF16)
     t = torch.ones(2, device=dev, dtype=F32)
     m = torch.empty(R * nseg + 1, device=dev, dtype=F32)
-    arg = torch.empty(R * nseg + 1, device=dev, dtype=torch.int32)
+    arg = torch.empty(R * nseg + 1, device=dev, dtype=torch.int16)
     keys = torch.empty(R * nseg + 1, device=dev, dtype=torch.int64)
     cm = torch.ones(C, device=dev, dtype=F32)
     good = dict(a=a.data_ptr(), b=b.data_ptr(), R=R, C=C, D=D, t=t.data_ptr(), L=L, cm=None, ca=None,
@@ -228,36 +229,43 @@ def test_segmax_any_and_expand_refuse_bad_arguments_without_launching(cuda_devic
 
     def call(**kw):
         v = dict(good, **kw)
-        _lib.call("xclip_filip_segmax_any", v["a"], v["b"], v["R"], v["C"], v["D"], v["t"], v["L"], v["cm"],
+        _lib.call("xclip_filip_segmax_arg16", v["a"], v["b"], v["R"], v["C"], v["D"], v["t"], v["L"], v["cm"],
                   v["ca"], v["m"], v["arg"], v["keys"], None)
 
-    bad = [dict(L=0), dict(L=-3), dict(L=76), dict(C=C + 1), dict(a=None), dict(keys=None),
-           dict(m=None), dict(a=a.data_ptr() + 2), dict(b=b.data_ptr() + 8), dict(keys=keys.data_ptr() + 4),
-           dict(m=m.data_ptr() + 2), dict(arg=arg.data_ptr() + 1), dict(cm=cm.data_ptr()),
-           dict(ca=cm.data_ptr()), dict(D=100)]
+    bad = [dict(L=0), dict(L=-3), dict(L=76), dict(L=65536, C=65536 * nseg), dict(C=C + 1), dict(a=None),
+           dict(b=None), dict(keys=None), dict(m=None, arg=None), dict(a=a.data_ptr() + 2),
+           dict(b=b.data_ptr() + 8), dict(keys=keys.data_ptr() + 4), dict(m=m.data_ptr() + 2),
+           dict(arg=arg.data_ptr() + 1), dict(cm=cm.data_ptr()), dict(ca=cm.data_ptr()), dict(D=100)]
     torch.cuda.synchronize()
     for kw in bad:
         n0 = lib.xclip_launch_count()
-        with pytest.raises(_lib.XClipB200Error, match="filip_segmax_any"):
+        with pytest.raises(_lib.XClipB200Error, match="filip_segmax_arg16"):
             call(**kw)
         assert lib.xclip_launch_count() == n0, f"a refused call launched a kernel: {kw}"
     n0 = lib.xclip_launch_count()
-    call(m=m[1:].data_ptr(), arg=arg[1:].data_ptr(), keys=keys[1:].data_ptr())    # 4 / 4 / 8-byte aligned
+    call(m=m[1:].data_ptr(), arg=arg[1:].data_ptr(), keys=keys[1:].data_ptr())    # 4 / 2 / 8-byte aligned
+    call(m=None)
+    call(arg=None)
     torch.cuda.synchronize()
-    assert lib.xclip_launch_count() == n0 + 2
+    assert lib.xclip_launch_count() == n0 + 6
 
     g = torch.empty((R, 240), device=dev, dtype=BF16)
     w = torch.zeros((1, nseg), device=dev, dtype=F32)
     rs = torch.zeros(R, device=dev, dtype=F32)
-    eg = dict(L=L, ldg=240, g=g.data_ptr())
+    eg = dict(arg=arg.data_ptr(), L=L, ldg=240, g=g.data_ptr(), row0=0)
 
     def expand(**kw):
         v = dict(eg, **kw)
-        _lib.call("xclip_filip_expand", arg.data_ptr(), m.data_ptr(), w.data_ptr(), rs.data_ptr(), t.data_ptr(),
-                  0, R, R, v["L"], nseg, v["g"], v["ldg"], None, None)
+        _lib.call("xclip_filip_expand16", v["arg"], w.data_ptr(), rs.data_ptr(), t.data_ptr(), v["row0"], R, R,
+                  v["L"], nseg, v["g"], v["ldg"], None)
 
-    for kw in [dict(L=0), dict(ldg=236), dict(ldg=224), dict(g=g.data_ptr() + 2)]:
+    for kw in [dict(L=0), dict(L=65536), dict(ldg=236), dict(ldg=224), dict(g=g.data_ptr() + 2),
+               dict(arg=None), dict(arg=arg.data_ptr() + 1), dict(row0=-1)]:
         n0 = lib.xclip_launch_count()
-        with pytest.raises(_lib.XClipB200Error, match="filip_expand"):
+        with pytest.raises(_lib.XClipB200Error, match="filip_expand16"):
             expand(**kw)
         assert lib.xclip_launch_count() == n0, f"a refused call launched a kernel: {kw}"
+    n0 = lib.xclip_launch_count()
+    expand()
+    torch.cuda.synchronize()
+    assert lib.xclip_launch_count() == n0 + 1

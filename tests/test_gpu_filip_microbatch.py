@@ -8,8 +8,8 @@ from pathlib import Path
 import pytest
 import torch
 
-from test_gpu_filip import (_col_mask_tables, _compare_filip, _filip_inputs, _gen, _oracle_filip, _split,
-                            _unit, oracle_filip_chunked)
+from test_gpu_filip import (_col_mask_tables, _compare_filip, _filip_inputs, _gen, _oracle_filip, _run_segmax,
+                            _split, _unit, oracle_filip_chunked)
 
 pytestmark = pytest.mark.gpu
 BF16, F32 = torch.bfloat16, torch.float32
@@ -20,106 +20,66 @@ GOLD = Path(__file__).parent / "golden"
 
 @pytest.mark.parametrize("seg_len,nseg,masked", [(1, 300, False), (7, 40, True), (8, 33, False),
                                                  (98, 9, True), (256, 3, False), (577, 2, True)])
-def test_unpack16_equals_segmax_any(cuda_device, seg_len, nseg, masked):
+def test_segmax16_outputs_match_fp64_and_each_other(cuda_device, seg_len, nseg, masked):
+    """The full call against fp64 (_run_segmax), then the partial calls: the argmax alone
+    (want_max=False), the maximum alone (seg_arg=False) and the argmax written into a given buffer
+    (seg_arg=into) equal the full call bit for bit."""
     from x_clip_b200 import kernels as K
     dev = cuda_device
     gen = _gen(dev, seg_len)
     R, D = 333, 128
-    a_row, _ = _split(_unit((R, D), gen, dev))
-    _, b_col = _split(_unit((nseg * seg_len, D), gen, dev))
-    t = torch.tensor([2.5], device=dev, dtype=F32)
+    za, zb = _unit((R, D), gen, dev), _unit((nseg * seg_len, D), gen, dev)
     cm = ca = None
     if masked:
         mask = torch.rand(nseg * seg_len, generator=gen, device=dev) < 0.7
         mask.view(nseg, seg_len)[0] = False                  # a segment with every column masked
         cm, ca = _col_mask_tables(mask)
-    m32, a32 = K.filip_segmax(a_row, b_col, t, seg_len, cm, ca)
-    m16, a16 = K.filip_segmax16(a_row, b_col, t, seg_len, cm, ca)
-    assert torch.equal(m16.view(torch.int32), m32.view(torch.int32))
-    assert torch.equal(a16.to(torch.int32) & 0xFFFF, a32)
+    m, arg, _, _ = _run_segmax(za, zb, 2.5, seg_len, cm, ca)
+    a_row, _ = _split(za)
+    _, b_col = _split(zb)
+    t = torch.tensor([2.5], device=dev, dtype=F32)
     _, a_only = K.filip_segmax16(a_row, b_col, t, seg_len, cm, ca, want_max=False)
     m_only, none = K.filip_segmax16(a_row, b_col, t, seg_len, cm, ca, seg_arg=False)
-    assert none is None and torch.equal(a_only, a16) and torch.equal(m_only.view(torch.int32), m32.view(torch.int32))
+    assert none is None and torch.equal(a_only.to(torch.int32) & 0xFFFF, arg)
+    assert torch.equal(m_only.view(torch.int32), m.view(torch.int32))
     into = torch.full((R, nseg), -1, device=dev, dtype=torch.int16)
     K.filip_segmax16(a_row, b_col, t, seg_len, cm, ca, seg_arg=into)
-    assert torch.equal(into, a16)
+    assert torch.equal(into, a_only)
 
 
 @pytest.mark.parametrize("seg_len", [1, 7, 8, 98, 256, 577])
-def test_expand16_writes_the_same_g_bits_as_expand(cuda_device, seg_len):
+def test_expand16_window_matches_dense_construction(cuda_device, seg_len):
     """Random argmax, weights with zeros (masked rows and samples), windows at row0 > 0 and a row stride
-    ldg > C: the whole G buffer, pad columns and the untouched tail included, is bit-identical."""
+    ldg > C, over a buffer of random bits: columns [0, C) equal G built densely in torch, the pad
+    columns [C, roundup8(C)) are zero and columns [roundup8(C), ldg) keep their random bits."""
     from x_clip_b200 import _lib
     dev = cuda_device
     gen = _gen(dev, 100 + seg_len)
     samples, rps, nseg = 6, 13, 5
     R, C = samples * rps, nseg * seg_len
-    arg32 = torch.randint(0, seg_len, (R, nseg), generator=gen, device=dev, dtype=torch.int32)
-    arg16 = arg32.to(torch.int16)                             # seg_len <= 577 < 32768
-    seg_max = torch.randn((R, nseg), generator=gen, device=dev)
+    arg16 = torch.randint(0, seg_len, (R, nseg), generator=gen, device=dev, dtype=torch.int16)
     wmat = torch.randn((samples, nseg), generator=gen, device=dev)
     wmat[1, 2] = 0.0
     rowscale = torch.rand(R, generator=gen, device=dev)
     rowscale[rps:2 * rps:3] = 0.0                             # masked text tokens
     t = torch.tensor([3.0], device=dev, dtype=F32)
-    ldg = (C + 7) // 8 * 8 + 24
+    C8 = (C + 7) // 8 * 8
+    ldg = C8 + 24
     for row0, rows in ((0, R), (5, 40), (R - 1, 1)):
         fill = torch.randint(-2 ** 15, 2 ** 15, (rows, ldg), generator=gen, device=dev, dtype=torch.int16)
-        g32, g16 = fill.clone().view(BF16), fill.clone().view(BF16)
-        _lib.call("xclip_filip_expand", arg32.data_ptr(), seg_max.data_ptr(), wmat.data_ptr(), rowscale.data_ptr(),
-                  t.data_ptr(), row0, rows, rps, seg_len, nseg, g32.data_ptr(), ldg, None, None)
+        g = fill.clone().view(BF16)
         _lib.call("xclip_filip_expand16", arg16[row0:row0 + rows].data_ptr(), wmat.data_ptr(), rowscale.data_ptr(),
-                  t.data_ptr(), row0, rows, rps, seg_len, nseg, g16.data_ptr(), ldg, None)
+                  t.data_ptr(), row0, rows, rps, seg_len, nseg, g.data_ptr(), ldg, None)
         torch.cuda.synchronize()
-        assert torch.equal(g16.view(torch.int16), g32.view(torch.int16)), (seg_len, row0, rows)
-        assert int((g16[:, :C].float() != 0).sum()) > 0
-
-
-def test_compact_entry_points_refuse_without_launching(cuda_device):
-    from x_clip_b200 import _lib
-    lib = _lib.load()
-    dev = cuda_device
-    R, L, nseg, D = 64, 7, 3, 64
-    C = L * nseg
-    a = torch.zeros((R, D), device=dev, dtype=BF16)
-    b = torch.zeros((C, D), device=dev, dtype=BF16)
-    t = torch.ones(1, device=dev, dtype=F32)
-    m = torch.empty(R * nseg + 1, device=dev, dtype=F32)
-    arg = torch.empty(R * nseg + 1, device=dev, dtype=torch.int16)
-    keys = torch.empty(R * nseg, device=dev, dtype=torch.int64)
-    good = dict(a=a.data_ptr(), C=C, L=L, m=m.data_ptr(), arg=arg.data_ptr(), keys=keys.data_ptr())
-
-    def seg(**kw):
-        v = dict(good, **kw)
-        _lib.call("xclip_filip_segmax_arg16", v["a"], b.data_ptr(), R, v["C"], D, t.data_ptr(), v["L"], None,
-                  None, v["m"], v["arg"], v["keys"], None)
-
-    g = torch.empty((R, 32), device=dev, dtype=BF16)
-    w = torch.zeros((R, nseg), device=dev, dtype=F32)
-    rs = torch.zeros(R, device=dev, dtype=F32)
-    eg = dict(arg=arg.data_ptr(), L=L, ldg=32, g=g.data_ptr(), row0=0)
-
-    def exp(**kw):
-        v = dict(eg, **kw)
-        _lib.call("xclip_filip_expand16", v["arg"], w.data_ptr(), rs.data_ptr(), t.data_ptr(), v["row0"], R, 1,
-                  v["L"], nseg, v["g"], v["ldg"], None)
-
-    cases = [(seg, dict(L=65536, C=65536 * nseg)), (seg, dict(m=None, arg=None)), (seg, dict(arg=arg.data_ptr() + 1)),
-             (seg, dict(m=m.data_ptr() + 2)), (seg, dict(a=None)), (seg, dict(L=0)), (seg, dict(keys=keys.data_ptr() + 4)),
-             (exp, dict(L=65536)), (exp, dict(arg=arg.data_ptr() + 1)), (exp, dict(arg=None)), (exp, dict(ldg=16)),
-             (exp, dict(g=g.data_ptr() + 2)), (exp, dict(row0=-1))]
-    torch.cuda.synchronize()
-    for fn, kw in cases:
-        n0 = lib.xclip_launch_count()
-        with pytest.raises(_lib.XClipB200Error, match="filip_(segmax_arg16|expand16)"):
-            fn(**kw)
-        assert lib.xclip_launch_count() == n0, f"a refused call launched a kernel: {kw}"
-    n0 = lib.xclip_launch_count()
-    seg(m=None)
-    seg(arg=None)
-    exp()
-    torch.cuda.synchronize()
-    assert lib.xclip_launch_count() == n0 + 5
+        r = torch.arange(row0, row0 + rows, device=dev)
+        w = wmat[r // rps] * rowscale[r, None]
+        want = torch.zeros((rows, C), device=dev, dtype=BF16)
+        cols = torch.arange(nseg, device=dev)[None, :] * seg_len + arg16[row0:row0 + rows].long()
+        want.scatter_(1, cols, torch.where(w != 0, w * t, 0.0).to(BF16))     # a zero weight writes +0
+        assert torch.equal(g[:, :C].view(torch.int16), want.view(torch.int16)), (seg_len, row0, rows)
+        assert not bool(g[:, C:C8].view(torch.int16).any()), (seg_len, row0, rows)
+        assert torch.equal(g[:, C8:].view(torch.int16), fill[:, C8:]), (seg_len, row0, rows)
+        assert int((g[:, :C].float() != 0).sum()) > 0
 
 
 # --------------------------------------------------------------------------- the loss under each plan

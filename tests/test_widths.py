@@ -70,7 +70,8 @@ ROW_KERNELS = ("ln_fwd_kernel", "ln_bwd_kernel", "l2norm_fwd_kernel", "l2norm_bw
 
 
 def _row_kernel(mangled):
-    """which of ROW_KERNELS a mangled name instantiates (geglu_ln_fwd_kernel is not ln_fwd_kernel)"""
+    """which of ROW_KERNELS a mangled name instantiates (the length prefix of the mangled name keeps a
+    kernel from matching inside a longer name that ends in it)"""
     return next((k for k in ROW_KERNELS if f"xclip{len(k)}{k}I" in mangled), None)
 
 

@@ -1,4 +1,4 @@
-"""Time the pieces of the feed-forward block: fused (csrc/ff.cu) vs separate kernels.
+"""Time the pieces of the feed-forward block: fused (csrc/ff.cu) vs plain GEMMs of the same shapes.
 
     python tools/ff_bench.py [M,d ...]     (default: cfg3 ViT micro-batch 512, cfg3 text, cfg2 text)"""
 import os
@@ -45,16 +45,12 @@ for (M, d) in shapes:
     w1p, w2g, colvec = K.ff_weights(w1, w2, g4)
     u, hp, rowsum = K.ff_up(x, w1p)
     x2, acc, stats = K.ff_down(hp, w2g, colvec, rowsum, res, 1e-5)
-    h, st = K.geglu_ln_fwd(u, g4)
-    dh = K.gemm(dx, w2b, b_major=1)
     t = {}
     t["gemm up (plain)"] = timeit(lambda: K.gemm(x, w1b))
     t["ff_up (fused GEGLU)"] = timeit(lambda: K.ff_up(x, w1p))
-    t["geglu_ln_fwd"] = timeit(lambda: K.geglu_ln_fwd(u, g4))
-    t["gemm down (plain)"] = timeit(lambda: K.gemm(h, w2b, residual=res))
+    t["gemm down (plain)"] = timeit(lambda: K.gemm(hp, w2b, residual=res))
     t["ff_down (fused LN)"] = timeit(lambda: K.ff_down(hp, w2g, colvec, rowsum, res, 1e-5))
     t["gemm dgrad down (plain)"] = timeit(lambda: K.gemm(dx, w2b, b_major=1))
-    t["geglu_ln_bwd"] = timeit(lambda: K.geglu_ln_bwd(dh, u, st, g4))
     t["ff_bwd_prep"] = timeit(lambda: K.ff_bwd_prep(dx, stats))
     t["gemm wgrad up (plain, split-K fp32)"] = timeit(lambda: K.gemm(u, x, a_major=1, b_major=1, accumulate=True))
     t["gemm dgrad up (plain)"] = timeit(lambda: K.gemm(u, w1b, b_major=1))

@@ -64,7 +64,7 @@ def segmax_pass(R, C, seg_len, D, dev, reps):
     a, _ = _split(_unit((R, D), dev))
     _, b = _split(_unit((C, D), dev))
     t = torch.tensor([100.0], device=dev, dtype=F32)
-    (ms,) = _time([lambda: K.filip_segmax(a, b, t, seg_len, None, None)], reps)
+    (ms,) = _time([lambda: K.filip_segmax16(a, b, t, seg_len, None, None)], reps)
     fl = 2.0 * R * C * 3 * D
     return dict(R=R, C=C, seg_len=seg_len, segmax_ms=round(ms, 3), segmax_tflops=round(fl / ms / 1e9, 1))
 

@@ -45,10 +45,6 @@ SIGNATURES = {
     "xclip_layernorm_bwd": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p,
                                     c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int, c_int,
                                     c_void_p]),
-    "xclip_geglu_ln_fwd": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_int64, c_void_p,
-                                   c_int, c_int, c_float, c_void_p]),
-    "xclip_geglu_ln_bwd": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p,
-                                   c_void_p, c_int64, c_void_p, c_int, c_int, c_void_p]),
     "xclip_l2norm_fwd": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
                                  c_int, c_void_p]),
     "xclip_l2norm_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p]),
@@ -97,16 +93,12 @@ SIGNATURES = {
                                  c_float, c_float, c_int, c_float, c_void_p]),
     "xclip_rotary_inplace": (c_int, [c_void_p, c_int64, c_int64, c_int, c_int, c_void_p, c_void_p, c_int,
                                      c_void_p]),
-    "xclip_filip_segmax_any": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int,
-                                       c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "xclip_filip_reduce": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int,
                                    c_void_p]),
     "xclip_filip_nce_fwd": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                     c_float, c_void_p]),
     "xclip_filip_nce_bwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
                                     c_void_p, c_void_p]),
-    "xclip_filip_expand": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
-                                   c_int, c_int, c_int, c_void_p, c_int64, c_void_p, c_void_p]),
     "xclip_filip_segmax_arg16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int,
                                          c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "xclip_filip_expand16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,

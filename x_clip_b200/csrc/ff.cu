@@ -3,8 +3,8 @@
 //   x2 = LN_4d(hp) g W2^T + x1                     one GEMM, LayerNorm folded into
 //                                                  weight + epilogue                (xclip_ff_down)
 // so the [tokens, 8d] / [tokens, 4d] hidden activations make no extra round trip through HBM for
-// the activation and the normalisation (the separate geglu_ln_fwd kernel was 10 % of the cfg3 step
-// and instruction-issue bound).  The LayerNorm fold:
+// the activation and the normalisation (a separate GEGLU + LayerNorm row kernel was 10 % of the cfg3
+// step and instruction-issue bound).  The LayerNorm fold:
 //   LN(hp)_k g_k = (hp_k - mean) rstd g_k   =>   x2_j = rstd (sum_k hp_k W2g_jk - mean c_j),
 //   W2g = W2 . g (column scaling), c_j = sum_k W2g_jk.
 // Backward pieces that replace the LayerNorm output h (never materialised now):

@@ -6,13 +6,13 @@
 //              [text,image] orientation for i2t as well)
 //
 // The 6-D similarity tensor (68.7 G elements at cfg4) is never materialised:
-//   xclip_filip_segmax_any : the wgmma GEMM with the EPI_SEGMAX epilogue produces, per token row
-//                        and per sample of the other modality, max + argmax over that sample's
-//                        tokens, for any token count (256-column tiles, samples cut by a tile
-//                        edge merged through 64-bit keys, then unpacked)
+//   xclip_filip_segmax_arg16 : the wgmma GEMM with the EPI_SEGMAX epilogue produces, per token row
+//                        and per sample of the other modality, max + 16-bit argmax over that
+//                        sample's tokens, for any token count up to 65535 (256-column tiles,
+//                        samples cut by a tile edge merged through 64-bit keys, then unpacked)
 //   xclip_filip_reduce : [tokens, B] maxima -> [B, B] similarity (masked mean / mean)
 //   xclip_filip_nce_*  : row-wise InfoNCE / DCL on a [B,B] fp32 matrix (warp-shuffle reductions)
-//   xclip_filip_expand : backward: one-hot (at the argmax) weighted bf16 operand G[rows, cols]
+//   xclip_filip_expand16 : backward: one-hot (at the argmax) weighted bf16 operand G[rows, cols]
 //                        for a chunk of rows, which then feeds two plain wgmma GEMMs
 //                        (d rows = G @ Zcols, d cols += G^T @ Zrows).
 #include "gemm.cuh"
@@ -91,20 +91,14 @@ filip_nce_bwd_kernel(const float* __restrict__ s, const float* __restrict__ lse,
 }
 
 // G[r, c] (bf16) for rows [row0, row0+rows): alpha * wmat[sample(r), seg(c)] * rowscale[r] at the
-// argmax column of each segment, zero elsewhere.  dtemp += sum_r,seg w * segmax (w without alpha).
-// Idx = int: seg_arg / seg_max are indexed by the global row r.  Idx = unsigned short (the compact
-// form): seg_arg holds rows [row0, row0 + rows) only, and there is no seg_max and no dtemp.
-template <typename Idx>
+// argmax column of each segment, zero elsewhere.  seg_arg holds rows [row0, row0 + rows) only.
 __global__ void __launch_bounds__(256)
-filip_expand_kernel(const Idx* __restrict__ seg_arg, const float* __restrict__ seg_max,
-                    const float* __restrict__ wmat, const float* __restrict__ rowscale,
-                    const float* __restrict__ alpha_dev, int row0, int rows, int rows_per_sample,
-                    int seg_len, int nseg, bf16* __restrict__ g, long long ldg,
-                    float* __restrict__ dtemp) {
-  constexpr bool kCompact = sizeof(Idx) == 2;
+filip_expand_kernel(const unsigned short* __restrict__ seg_arg, const float* __restrict__ wmat,
+                    const float* __restrict__ rowscale, const float* __restrict__ alpha_dev, int row0,
+                    int rows, int rows_per_sample, int seg_len, int nseg, bf16* __restrict__ g,
+                    long long ldg) {
   const float alpha = __ldg(alpha_dev);
   const int vec_per_row = nseg * seg_len / 8;
-  float tsum = 0.f;
   for (long long v = blockIdx.x * (long long)blockDim.x + threadIdx.x;
        v < (long long)rows * vec_per_row; v += (long long)gridDim.x * blockDim.x) {
     const int lr = (int)(v / vec_per_row);
@@ -112,12 +106,11 @@ filip_expand_kernel(const Idx* __restrict__ seg_arg, const float* __restrict__ s
     const long long r = row0 + lr;
     const int seg = c0 / seg_len;
     const int in_seg = c0 - seg * seg_len;
-    const int a = seg_arg[(kCompact ? lr : r) * nseg + seg];
+    const int a = seg_arg[(long long)lr * nseg + seg];
     uint4 o = make_uint4(0, 0, 0, 0);
     if (a >= in_seg && a < in_seg + 8) {
       const float w = wmat[(r / rows_per_sample) * nseg + seg] * rowscale[r];
       if (w != 0.f) {
-        if constexpr (!kCompact) tsum += w * seg_max[r * nseg + seg];
         bf16 vals[8];
 #pragma unroll
         for (int k = 0; k < 8; ++k) vals[k] = __float2bfloat16_rn(0.f);
@@ -127,33 +120,25 @@ filip_expand_kernel(const Idx* __restrict__ seg_arg, const float* __restrict__ s
     }
     *reinterpret_cast<uint4*>(g + lr * ldg + c0) = o;
   }
-  if (!kCompact && dtemp != nullptr) {
-    tsum = warp_sum(tsum);
-    if ((threadIdx.x & 31) == 0 && tsum != 0.f) atomicAdd(dtemp, tsum);
-  }
 }
 
 // filip_expand_kernel for seg_len % 8 != 0: an 8-column vector may hold the end of one segment and
 // the start of the next (several when seg_len < 8), so every column steps its own (segment,
 // position).  Columns [nseg * seg_len, roundup8) of the last vector are written as zeros.
-template <typename Idx>
 __global__ void __launch_bounds__(256)
-filip_expand_any_kernel(const Idx* __restrict__ seg_arg, const float* __restrict__ seg_max,
-                        const float* __restrict__ wmat, const float* __restrict__ rowscale,
-                        const float* __restrict__ alpha_dev, int row0, int rows, int rows_per_sample,
-                        int seg_len, int nseg, bf16* __restrict__ g, long long ldg,
-                        float* __restrict__ dtemp) {
-  constexpr bool kCompact = sizeof(Idx) == 2;
+filip_expand_any_kernel(const unsigned short* __restrict__ seg_arg, const float* __restrict__ wmat,
+                        const float* __restrict__ rowscale, const float* __restrict__ alpha_dev,
+                        int row0, int rows, int rows_per_sample, int seg_len, int nseg,
+                        bf16* __restrict__ g, long long ldg) {
   const float alpha = __ldg(alpha_dev);
   const int C = nseg * seg_len;
   const int vec_per_row = (C + 7) / 8;
-  float tsum = 0.f;
   for (long long v = blockIdx.x * (long long)blockDim.x + threadIdx.x;
        v < (long long)rows * vec_per_row; v += (long long)gridDim.x * blockDim.x) {
     const int lr = (int)(v / vec_per_row);
     const int c0 = (int)(v % vec_per_row) * 8;
     const long long r = row0 + lr;
-    const Idx* arg_row = seg_arg + (kCompact ? lr : r) * nseg;
+    const unsigned short* arg_row = seg_arg + (long long)lr * nseg;
     const float* w_row = wmat + (r / rows_per_sample) * nseg;
     int seg = c0 / seg_len;
     int pos = c0 - seg * seg_len;
@@ -165,10 +150,7 @@ filip_expand_any_kernel(const Idx* __restrict__ seg_arg, const float* __restrict
       if (c0 + k < C) {
         if (pos == a) {
           const float w = w_row[seg] * rowscale[r];
-          if (w != 0.f) {
-            if constexpr (!kCompact) tsum += w * seg_max[r * nseg + seg];
-            vals[k] = __float2bfloat16_rn(w * alpha);
-          }
+          if (w != 0.f) vals[k] = __float2bfloat16_rn(w * alpha);
         }
         if (++pos == seg_len) {
           pos = 0;
@@ -177,22 +159,6 @@ filip_expand_any_kernel(const Idx* __restrict__ seg_arg, const float* __restrict
       }
     }
     *reinterpret_cast<uint4*>(g + lr * ldg + c0) = *reinterpret_cast<const uint4*>(vals);
-  }
-  if (!kCompact && dtemp != nullptr) {
-    tsum = warp_sum(tsum);
-    if ((threadIdx.x & 31) == 0 && tsum != 0.f) atomicAdd(dtemp, tsum);
-  }
-}
-
-// keys of EPI_SEGMAX -> seg_max (f32) and seg_arg (int32)
-__global__ void __launch_bounds__(256)
-filip_unpack_keys_kernel(const unsigned long long* __restrict__ keys, long long n,
-                         float* __restrict__ seg_max, int* __restrict__ seg_arg) {
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n;
-       i += (long long)gridDim.x * blockDim.x) {
-    const unsigned long long k = keys[i];
-    seg_max[i] = segmax_key_value(k);
-    seg_arg[i] = segmax_key_index(k);
   }
 }
 
@@ -213,8 +179,8 @@ filip_unpack_keys16_kernel(const unsigned long long* __restrict__ keys, long lon
 
 using namespace xclip;
 
-// The segment-max GEMM shared by both unpack forms: checks its arguments, zeroes the keys and
-// launches EPI_SEGMAX.  Returns non-zero (nothing launched) when an argument is refused.
+// The segment-max GEMM: checks its arguments, zeroes the keys and launches EPI_SEGMAX.  Returns
+// non-zero (nothing launched) when an argument is refused.
 static int filip_segmax_keys(const char* who, const void* a, const void* b, int R, int C, int D,
                              const float* temp_exp, int seg_len, const float* col_mul,
                              const float* col_add, void* keys, cudaStream_t st) {
@@ -263,25 +229,6 @@ static int unpack_blocks(long long nkeys) {
   long long blocks = (nkeys + 255) / 256;
   if (blocks > (long long)num_sms() * 16) blocks = (long long)num_sms() * 16;
   return (int)blocks;
-}
-
-extern "C" int xclip_filip_segmax_any(const void* a, const void* b, int R, int C, int D,
-                                      const float* temp_exp, int seg_len, const float* col_mul,
-                                      const float* col_add, float* seg_max, int* seg_arg, void* keys,
-                                      xclip_stream_t stream) {
-  int rc = xclip_init();
-  if (rc) return rc;
-  XCLIP_REQUIRE(seg_max && seg_arg, "filip_segmax_any: null pointer");
-  XCLIP_REQUIRE(((reinterpret_cast<uintptr_t>(seg_max) | reinterpret_cast<uintptr_t>(seg_arg)) & 3) == 0,
-                "filip_segmax_any: misaligned fp32 / int32 pointer");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  rc = filip_segmax_keys("filip_segmax_any", a, b, R, C, D, temp_exp, seg_len, col_mul, col_add, keys, st);
-  if (rc) return rc;
-  const long long nkeys = (long long)R * (C / seg_len);
-  filip_unpack_keys_kernel<<<unpack_blocks(nkeys), 256, 0, st>>>(
-      reinterpret_cast<const unsigned long long*>(keys), nkeys, seg_max, seg_arg);
-  XCLIP_LAUNCH_CHECK("filip_unpack_keys_kernel");
-  return XCLIP_OK;
 }
 
 extern "C" int xclip_filip_segmax_arg16(const void* a, const void* b, int R, int C, int D,
@@ -345,34 +292,6 @@ extern "C" int xclip_filip_nce_bwd(const float* s, const float* lse, int R, int 
   return XCLIP_OK;
 }
 
-extern "C" int xclip_filip_expand(const int* seg_arg, const float* seg_max, const float* wmat,
-                                  const float* rowscale, const float* temp_exp, int row0, int rows,
-                                  int rows_per_sample, int seg_len, int nseg, void* g, int64_t ldg,
-                                  float* dtemp, xclip_stream_t stream) {
-  int rc = xclip_init();
-  if (rc) return rc;
-  XCLIP_REQUIRE(seg_arg && seg_max && wmat && rowscale && temp_exp && g, "filip_expand: null pointer");
-  XCLIP_REQUIRE(rows > 0 && rows_per_sample > 0 && seg_len >= 1 && nseg > 0 &&
-                    ldg >= (int64_t)nseg * seg_len && ldg % 8 == 0,
-                "filip_expand: bad sizes");
-  XCLIP_REQUIRE((reinterpret_cast<uintptr_t>(g) & 15) == 0, "filip_expand: misaligned g");
-  const long long vecs = (long long)rows * ((nseg * seg_len + 7) / 8);
-  long long blocks = (vecs + 255) / 256;
-  if (blocks > (long long)num_sms() * 16) blocks = (long long)num_sms() * 16;
-  if (seg_len % 8 == 0) {
-    filip_expand_kernel<int><<<(int)blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-        seg_arg, seg_max, wmat, rowscale, temp_exp, row0, rows, rows_per_sample, seg_len, nseg,
-        reinterpret_cast<bf16*>(g), ldg, dtemp);
-    XCLIP_LAUNCH_CHECK("filip_expand_kernel");
-  } else {
-    filip_expand_any_kernel<int><<<(int)blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-        seg_arg, seg_max, wmat, rowscale, temp_exp, row0, rows, rows_per_sample, seg_len, nseg,
-        reinterpret_cast<bf16*>(g), ldg, dtemp);
-    XCLIP_LAUNCH_CHECK("filip_expand_any_kernel");
-  }
-  return XCLIP_OK;
-}
-
 extern "C" int xclip_filip_expand16(const uint16_t* seg_arg, const float* wmat, const float* rowscale,
                                     const float* temp_exp, int row0, int rows, int rows_per_sample,
                                     int seg_len, int nseg, void* g, int64_t ldg, xclip_stream_t stream) {
@@ -389,15 +308,15 @@ extern "C" int xclip_filip_expand16(const uint16_t* seg_arg, const float* wmat, 
   if (blocks > (long long)num_sms() * 16) blocks = (long long)num_sms() * 16;
   const unsigned short* arg = reinterpret_cast<const unsigned short*>(seg_arg);
   if (seg_len % 8 == 0) {
-    filip_expand_kernel<unsigned short><<<(int)blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-        arg, nullptr, wmat, rowscale, temp_exp, row0, rows, rows_per_sample, seg_len, nseg,
-        reinterpret_cast<bf16*>(g), ldg, nullptr);
-    XCLIP_LAUNCH_CHECK("filip_expand_kernel<u16>");
+    filip_expand_kernel<<<(int)blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+        arg, wmat, rowscale, temp_exp, row0, rows, rows_per_sample, seg_len, nseg,
+        reinterpret_cast<bf16*>(g), ldg);
+    XCLIP_LAUNCH_CHECK("filip_expand_kernel");
   } else {
-    filip_expand_any_kernel<unsigned short><<<(int)blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-        arg, nullptr, wmat, rowscale, temp_exp, row0, rows, rows_per_sample, seg_len, nseg,
-        reinterpret_cast<bf16*>(g), ldg, nullptr);
-    XCLIP_LAUNCH_CHECK("filip_expand_any_kernel<u16>");
+    filip_expand_any_kernel<<<(int)blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+        arg, wmat, rowscale, temp_exp, row0, rows, rows_per_sample, seg_len, nseg,
+        reinterpret_cast<bf16*>(g), ldg);
+    XCLIP_LAUNCH_CHECK("filip_expand_any_kernel");
   }
   return XCLIP_OK;
 }

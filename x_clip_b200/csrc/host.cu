@@ -163,7 +163,7 @@ int xclip_tune_set(int knob, int value) {
   return prev;
 }
 
-int xclip_abi_version(void) { return 2; }
+int xclip_abi_version(void) { return 3; }
 
 const char* xclip_last_error(void) { return xclip::g_err; }
 

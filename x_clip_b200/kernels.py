@@ -183,27 +183,6 @@ def layernorm_bwd(dy, x, stats, g, *, add=None, dg=None):
     return dx
 
 
-def geglu_ln_fwd(u, g, *, eps=1e-5):
-    _need(u, BF16, "u"); _rows2d(u, "u"); _need(g, F32, "g")
-    rows, two_dh = u.shape
-    dh = two_dh // 2
-    h = torch.empty((rows, dh), device=u.device, dtype=BF16)
-    stats = torch.empty((rows, 2), device=u.device, dtype=F32)
-    _call(u, "geglu_ln_fwd", 0.0, 2.0 * rows * dh * 3, "xclip_geglu_ln_fwd", u.data_ptr(), u.stride(0), g.data_ptr(), h.data_ptr(),
-              h.stride(0), stats.data_ptr(), rows, dh, float(eps))
-    return h, stats
-
-
-def geglu_ln_bwd(dh_grad, u, stats, g, *, dg=None):
-    _need(dh_grad, BF16, "dh"); _rows2d(dh_grad, "dh"); _need(u, BF16, "u")
-    rows, two_dh = u.shape
-    du = torch.empty((rows, two_dh), device=u.device, dtype=BF16)
-    _call(dh_grad, "geglu_ln_bwd", 0.0, 2.0 * rows * (two_dh // 2) * 5, "xclip_geglu_ln_bwd", dh_grad.data_ptr(), dh_grad.stride(0), u.data_ptr(),
-              u.stride(0), stats.data_ptr(), g.data_ptr(), du.data_ptr(), du.stride(0), _ptr(dg),
-              rows, two_dh // 2)
-    return du
-
-
 def l2norm_fwd(p):
     _need(p, F32, "p"); _rows2d(p, "p")
     rows, d = p.shape
@@ -564,22 +543,6 @@ def simreg_bwd(a, b, diag_offset, gscale):
     return g
 
 
-def filip_segmax(a, b, temp_exp, seg_len, col_mul, col_add):
-    """Per row of a and per seg_len-long block of rows of b: max / argmax of temp * <a_r, b_c>, for
-    any seg_len >= 1.  xclip_filip_segmax_any needs a temporary key buffer of 8 bytes per result."""
-    _need(a, BF16, "a"); _need(b, BF16, "b")
-    R, D = a.shape
-    C = b.shape[0]
-    nseg = C // seg_len
-    seg_max = torch.empty((R, nseg), device=a.device, dtype=F32)
-    seg_arg = torch.empty((R, nseg), device=a.device, dtype=torch.int32)
-    keys = torch.empty((R, nseg), device=a.device, dtype=torch.int64)
-    _call(a, "filip_segmax", 2.0 * R * C * D, 2.0 * (R + C) * D + 32.0 * R * nseg, "xclip_filip_segmax_any",
-          a.data_ptr(), b.data_ptr(), R, C, D, temp_exp.data_ptr(), int(seg_len), _ptr(col_mul),
-          _ptr(col_add), seg_max.data_ptr(), seg_arg.data_ptr(), keys.data_ptr())
-    return seg_max, seg_arg
-
-
 def filip_reduce(seg_max, weights, samples, length, nseg, transpose):
     out = torch.empty((nseg, samples) if transpose else (samples, nseg), device=seg_max.device, dtype=F32)
     _call(seg_max, "filip_small", 0.0, 4.0 * seg_max.numel(), "xclip_filip_reduce", seg_max.data_ptr(),
@@ -612,19 +575,6 @@ def filip_nce_bwd(s, lse, diag_off, dcl, gscale, row_valid=None):
     return g
 
 
-def filip_expand(seg_arg, seg_max, wmat, rowscale, temp_exp, row0, rows, rows_per_sample, seg_len,
-                 nseg, dtemp):
-    """bf16 G [rows, C] (C = nseg * seg_len): a view of a [rows, roundup8(C)] buffer, so that its row
-    stride stays a multiple of 8 elements for the gradient GEMMs; see xclip_filip_expand."""
-    C = nseg * seg_len
-    g = torch.empty((rows, (C + 7) // 8 * 8), device=seg_arg.device, dtype=BF16)
-    _call(seg_arg, "filip_expand", 0.0, 2.0 * g.numel(), "xclip_filip_expand", seg_arg.data_ptr(),
-          seg_max.data_ptr(), wmat.data_ptr(), rowscale.data_ptr(), temp_exp.data_ptr(), int(row0),
-          int(rows), int(rows_per_sample), int(seg_len), int(nseg), g.data_ptr(), g.stride(0),
-          _ptr(dtemp))
-    return g[:, :C]
-
-
 ARG16_MAX_SEG_LEN = 65535
 
 
@@ -636,9 +586,11 @@ def check_arg16_seg_len(seg_len):
 
 
 def filip_segmax16(a, b, temp_exp, seg_len, col_mul, col_add, want_max=True, seg_arg=None):
-    """filip_segmax with the compact argmax: -> (seg_max f32 [R, nseg] or None, seg_arg int16 [R, nseg]
-    holding the unsigned 16-bit index, or None).  seg_arg may be a preallocated contiguous int16
-    [R, nseg] (a slice of a saved buffer); pass seg_arg=False for seg_max only."""
+    """Per row of a and per seg_len-long block of rows of b: max / argmax of temp * <a_r, b_c>, for
+    any 1 <= seg_len <= 65535 -> (seg_max f32 [R, nseg] or None, seg_arg int16 [R, nseg] holding the
+    unsigned 16-bit index, or None).  seg_arg may be a preallocated contiguous int16 [R, nseg] (a
+    slice of a saved buffer); pass seg_arg=False for seg_max only.  xclip_filip_segmax_arg16 needs a
+    temporary key buffer of 8 bytes per result."""
     check_arg16_seg_len(seg_len)
     _need(a, BF16, "a"); _need(b, BF16, "b")
     R, D = a.shape
@@ -660,8 +612,9 @@ def filip_segmax16(a, b, temp_exp, seg_len, col_mul, col_add, want_max=True, seg
 
 
 def filip_expand16(seg_arg, wmat, rowscale, temp_exp, row0, rows_per_sample, seg_len, nseg):
-    """filip_expand on a compact int16 argmax holding rows [row0, row0 + seg_arg.shape[0]) only; no
-    d temperature.  Same G bits and layout as filip_expand."""
+    """bf16 G [rows, C] (C = nseg * seg_len) for rows [row0, row0 + rows) from an int16 argmax that
+    holds those rows only (rows = seg_arg.shape[0]): a view of a [rows, roundup8(C)] buffer, so that
+    its row stride stays a multiple of 8 elements for the gradient GEMMs; see xclip_filip_expand16."""
     check_arg16_seg_len(seg_len)
     if seg_arg.dtype != torch.int16 or seg_arg.dim() != 2 or seg_arg.shape[1] != nseg or not seg_arg.is_contiguous():
         raise _lib.XClipB200Error(f"filip_expand16: seg_arg must be a contiguous int16 [rows, {nseg}]")
