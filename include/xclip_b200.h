@@ -263,6 +263,33 @@ int xclip_filip_expand16(const uint16_t* seg_arg, const float* wmat, const float
                          const float* temp_exp, int row0, int rows, int rows_per_sample,
                          int seg_len, int nseg, void* g, int64_t ldg, xclip_stream_t stream);
 
+/* ---- FILIP with augmented views (x_clip/x_clip.py:625-650, :797-811, :821-868) ----------------
+ * s f32 [m*b, n*B] with row stride lds >= n*B: every (text view i, image view j) block is the [b, B]
+ * similarity of this rank's b texts of view i against the B images of view j (all ranks).  Row
+ * i*b + x; block j's global sample k lives at column
+ *     (k / col_run) * n * col_run + j * col_run + k % col_run
+ * with col_run = b (rank-major: the column order of the image-token all-gather, rank r's n views
+ * in turn) or col_run = B (view-major); col_run must be b or B.  The positive of row i*b + x in
+ * every block is k = x + diag_off (this rank's r*b), 0 <= diag_off <= B - b.
+ * blocks_fwd : lse[(i*b + x) * n + j] = log sum_k exp(s) over block (i, j) (the positive left out
+ *          when dcl; dcl with B == 1 gives lse = ln(1e-20), the reference's empty denominator);
+ *          *loss_accum += sum over rows and blocks of block_w[i*n + j] * (lse - s[positive])
+ *          (loss_accum may be NULL).  block_w: DEVICE f32 [m*n], each block's loss weight (scale
+ *          included).  row_valid (optional, one byte per row [m*b]): as for nce_fwd, a row with
+ *          row_valid 0 adds no loss, has lse 0 in every block.  One launch for the whole matrix.
+ * blocks_bwd : g[row, col] = *gscale * block_w[block] * (exp(s - lse) [not on the positive when
+ *          dcl] - [positive]) for g f32 [m*b, ldg >= n*B]; rows with row_valid 0 get g = 0.
+ * Both refuse without a launch: bad sizes, col_run not b or B, diag_off outside [0, B - b], a
+ * matrix of 2^31 or more elements. */
+int xclip_filip_nce_blocks_fwd(const float* s, int64_t lds, int m, int n, int b, int B, int col_run,
+                               int diag_off, int dcl, const unsigned char* row_valid,
+                               const float* block_w, float* lse, float* loss_accum,
+                               xclip_stream_t stream);
+int xclip_filip_nce_blocks_bwd(const float* s, int64_t lds, const float* lse, int m, int n, int b,
+                               int B, int col_run, int diag_off, int dcl,
+                               const unsigned char* row_valid, const float* block_w,
+                               const float* gscale, float* g, int64_t ldg, xclip_stream_t stream);
+
 /* ---- text embedding (x_clip/x_clip.py:320-332) ---------------------------------------------
  * fwd: out bf16 [B, n+1, d]: out[b,0] = cls, out[b,1+t] = tok[ids[b,t]] + pos[t]  (fp32 tables,
  *      ids int64 [B,n]; an id outside [0, vocab) traps the kernel - the launch

@@ -103,6 +103,10 @@ SIGNATURES = {
                                          c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "xclip_filip_expand16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                                      c_int, c_void_p, c_int64, c_void_p]),
+    "xclip_filip_nce_blocks_fwd": (c_int, [c_void_p, c_int64, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
+                                           c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "xclip_filip_nce_blocks_bwd": (c_int, [c_void_p, c_int64, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
+                                           c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
 }
 
 

@@ -19,7 +19,9 @@ widths that are not 128 * {1..8}, a causal text tower longer than
 x_clip.py:328) and conv-downsampled image latents.  Attention dropout (`attn_dropout`, 0 <= p <= 1)
 runs inside the attention kernels, with a counter-based mask that a re-encode regenerates exactly
 (engine.TransformerDropoutFn); `ff_dropout` is accepted and, as in the reference's Transformer
-(x_clip.py:268), not applied.  MLM, SimSiam / SimCLR and the multiview term run through the fast encoders (aux.py).  The similarity-regularisation term
+(x_clip.py:268), not applied.  MLM, SimSiam / SimCLR and the multiview term run through the fast encoders (aux.py);
+with FILIP, the augmented views (`aug_text` / `aug_image`) run every (text view, image view) pair in one
+pair of segment-max passes (filip.FilipLossFn), each text view masked by its own pad pattern.  The similarity-regularisation term
 (`sim_reg_loss_weight > 0`) runs fused with the contrastive loss (engine.ContrastiveLossFn) where the
 reference itself runs it: with `extra_latent_projection=True`, without FILIP and with a single view;
 the other combinations fail inside the reference (x_clip.py:779) and raise `Unsupported` here.
@@ -570,8 +572,6 @@ class CLIP(nn.Module):
         assert not (not return_loss and is_multiview), 'do not pass in augmented texts or images if not training'
         assert not (self.multiview_loss_weight == 0 and is_multiview), \
             'multiview loss weight cannot be 0 if augmented text or images passed in'
-        _require(not (is_multiview and self.use_all_token_embeds),
-                 "multiview with use_all_token_embeds is not implemented")
 
         has_aux = is_multiview or self.use_mlm or self.use_visual_ssl
         text_args = (text,) if self.text_encode_without_mask else (text, text_mask)
@@ -615,10 +615,18 @@ class CLIP(nn.Module):
 
         if self.use_all_token_embeds:
             from .filip import filip_loss
+            if is_multiview:
+                # every (text view, image view) pair in one pair of segment-max passes, each pair's
+                # InfoNCE weighted inside the loss: cl_w * L[0, 0] + mv_w * mean(the others) (:851-868)
+                cl_w = 1 - (self.text_ssl_loss_weight + self.image_ssl_loss_weight + self.multiview_loss_weight)
+                loss = filip_loss(self, zt, zi, zt_x, zi_x, ops, text_mask, views=(num_batch_texts, num_batch_images),
+                                  weights=(cl_w, self.multiview_loss_weight))
+                return loss + text_ssl_loss * self.text_ssl_loss_weight \
+                    + image_ssl_loss * self.image_ssl_loss_weight
             loss = filip_loss(self, zt, zi, zt_x, zi_x, ops, text_mask)
             if not has_aux:
                 return loss
-            # weighted with the auxiliary terms as the reference does (:851-865); multiview was refused
+            # weighted with the auxiliary terms as the reference does (:851-865)
             cl_w = 1 - (self.text_ssl_loss_weight + self.image_ssl_loss_weight)
             return loss * cl_w + text_ssl_loss * self.text_ssl_loss_weight \
                 + image_ssl_loss * self.image_ssl_loss_weight

@@ -90,6 +90,76 @@ filip_nce_bwd_kernel(const float* __restrict__ s, const float* __restrict__ lse,
   g[idx] = v * __ldg(gscale);
 }
 
+// Block-structured InfoNCE / DCL for augmented views: s [m*b, n*B] (row stride lds) holds one [b, B]
+// block per (text view i, image view j).  Rows i*b + x; block j's global sample k sits at column
+// filip_block_col(j, k): runs of col_run consecutive samples, the n views' runs interleaved (col_run = b:
+// the rank-major order of the image-token all-gather; col_run = B: view-major).  The positive of row
+// i*b + x in every block is k = x + diag_off.  lse is [m*b, n], one entry per (row, block).
+__device__ __forceinline__ long long filip_block_col(int j, int k, int n, int col_run) {
+  return (long long)(k / col_run) * n * col_run + (long long)j * col_run + k % col_run;
+}
+
+// one warp per (row, block); block weights w_blk[i*n + j] carry the loss scale of each block
+__global__ void __launch_bounds__(256)
+filip_nce_blocks_fwd_kernel(const float* __restrict__ s, long long lds, int m, int n, int b, int B,
+                            int col_run, int diag_off, int dcl, const unsigned char* __restrict__ row_valid,
+                            const float* __restrict__ w_blk, float* __restrict__ lse,
+                            float* __restrict__ loss_accum) {
+  const int lane = threadIdx.x & 31;
+  const long long wid = blockIdx.x * (long long)(blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (wid >= (long long)m * b * n) return;
+  const int row = (int)(wid / n), j = (int)(wid % n);
+  if (row_valid != nullptr && !row_valid[row]) {          // warp-uniform
+    if (lane == 0) lse[wid] = 0.f;
+    return;
+  }
+  const float* r = s + (long long)row * lds;
+  const int pos = row % b + diag_off;
+  float mx = -INFINITY;
+  for (int k = lane; k < B; k += 32)
+    if (!(dcl && k == pos)) mx = fmaxf(mx, r[filip_block_col(j, k, n, col_run)]);
+  mx = warp_max(mx);
+  float sum = 0.f;
+  for (int k = lane; k < B; k += 32)
+    if (!(dcl && k == pos)) sum += __expf(r[filip_block_col(j, k, n, col_run)] - mx);
+  sum = warp_sum(sum);
+  if (lane == 0) {
+    // DCL over a global batch of 1 leaves the denominator empty: the reference's log(0 + 1e-20)
+    const float l = (dcl && B == 1) ? logf(1e-20f) : mx + logf(sum);
+    lse[wid] = l;
+    if (loss_accum) {
+      const float w = w_blk[(row / b) * n + j];
+      atomicAdd(loss_accum, (l - r[filip_block_col(j, pos, n, col_run)]) * w);
+    }
+  }
+}
+
+// g[row, col] = *gscale * w_blk[block] * (exp(s - lse[row, j]) [skipped on the positive when dcl]
+// - [positive]); rows with row_valid[row] == 0 get g = 0.  g is [m*b, ldg].
+__global__ void __launch_bounds__(256)
+filip_nce_blocks_bwd_kernel(const float* __restrict__ s, long long lds, const float* __restrict__ lse,
+                            int m, int n, int b, int B, int col_run, int diag_off, int dcl,
+                            const unsigned char* __restrict__ row_valid, const float* __restrict__ w_blk,
+                            const float* __restrict__ gscale, float* __restrict__ g, long long ldg) {
+  const int C = n * B;
+  const long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (idx >= (long long)m * b * C) return;
+  const int row = (int)(idx / C), col = (int)(idx % C);
+  float* out = g + (long long)row * ldg + col;
+  if (row_valid != nullptr && !row_valid[row]) {
+    *out = 0.f;
+    return;
+  }
+  const int run = n * col_run;
+  const int j = (col % run) / col_run;
+  const int k = (col / run) * col_run + col % col_run;
+  const bool is_pos = (k == row % b + diag_off);
+  float v = 0.f;
+  if (!(dcl && is_pos)) v = __expf(s[(long long)row * lds + col] - lse[(long long)row * n + j]);
+  if (is_pos) v -= 1.f;
+  *out = v * (__ldg(gscale) * w_blk[(row / b) * n + j]);
+}
+
 // G[r, c] (bf16) for rows [row0, row0+rows): alpha * wmat[sample(r), seg(c)] * rowscale[r] at the
 // argmax column of each segment, zero elsewhere.  seg_arg holds rows [row0, row0 + rows) only.
 __global__ void __launch_bounds__(256)
@@ -289,6 +359,51 @@ extern "C" int xclip_filip_nce_bwd(const float* s, const float* lse, int R, int 
   filip_nce_bwd_kernel<<<(int)((n + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       s, lse, R, C, diag_off, dcl, row_valid, gscale, g);
   XCLIP_LAUNCH_CHECK("filip_nce_bwd_kernel");
+  return XCLIP_OK;
+}
+
+static int filip_nce_blocks_check(const char* who, const float* s, int64_t lds, int m, int n, int b,
+                                  int B, int col_run, int diag_off) {
+  XCLIP_REQUIRE(s != nullptr, "%s: null s", who);
+  XCLIP_REQUIRE(m > 0 && n > 0 && b > 0 && B >= b && col_run > 0 && B % col_run == 0 &&
+                    (col_run == B || col_run == b) && lds >= (int64_t)n * B,
+                "%s: bad sizes (m %d n %d b %d B %d col_run %d lds %lld)", who, m, n, b, B, col_run,
+                (long long)lds);
+  XCLIP_REQUIRE(diag_off >= 0 && diag_off + b <= B, "%s: diag_off %d outside [0, B - b]", who, diag_off);
+  XCLIP_REQUIRE((long long)m * b * n * B < (1LL << 31), "%s: matrix too large", who);
+  return XCLIP_OK;
+}
+
+extern "C" int xclip_filip_nce_blocks_fwd(const float* s, int64_t lds, int m, int n, int b, int B,
+                                          int col_run, int diag_off, int dcl,
+                                          const unsigned char* row_valid, const float* block_w,
+                                          float* lse, float* loss_accum, xclip_stream_t stream) {
+  int rc = xclip_init();
+  if (rc) return rc;
+  rc = filip_nce_blocks_check("filip_nce_blocks_fwd", s, lds, m, n, b, B, col_run, diag_off);
+  if (rc) return rc;
+  XCLIP_REQUIRE(lse && block_w, "filip_nce_blocks_fwd: null lse / block_w");
+  const long long warps = (long long)m * b * n;
+  filip_nce_blocks_fwd_kernel<<<(int)((warps + 7) / 8), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      s, lds, m, n, b, B, col_run, diag_off, dcl, row_valid, block_w, lse, loss_accum);
+  XCLIP_LAUNCH_CHECK("filip_nce_blocks_fwd_kernel");
+  return XCLIP_OK;
+}
+
+extern "C" int xclip_filip_nce_blocks_bwd(const float* s, int64_t lds, const float* lse, int m, int n,
+                                          int b, int B, int col_run, int diag_off, int dcl,
+                                          const unsigned char* row_valid, const float* block_w,
+                                          const float* gscale, float* g, int64_t ldg,
+                                          xclip_stream_t stream) {
+  int rc = xclip_init();
+  if (rc) return rc;
+  rc = filip_nce_blocks_check("filip_nce_blocks_bwd", s, lds, m, n, b, B, col_run, diag_off);
+  if (rc) return rc;
+  XCLIP_REQUIRE(lse && block_w && gscale && g && ldg >= (int64_t)n * B, "filip_nce_blocks_bwd: bad arguments");
+  const long long elems = (long long)m * b * n * B;
+  filip_nce_blocks_bwd_kernel<<<(int)((elems + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      s, lds, lse, m, n, b, B, col_run, diag_off, dcl, row_valid, block_w, gscale, g, ldg);
+  XCLIP_LAUNCH_CHECK("filip_nce_blocks_bwd_kernel");
   return XCLIP_OK;
 }
 

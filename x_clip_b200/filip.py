@@ -61,17 +61,18 @@ def chunk_transient_bytes(rows: int, R: int, nseg: int, seg_len: int, budget: in
     return max(e * (KEY_BYTES + MAX_BYTES), e * (KEY_BYTES + ARG_BYTES), e * ARG_BYTES + g)
 
 
-def saved_bytes(b: int, B: int, T: int, I: int) -> int:
-    """Compact argmax of both passes when every chunk is saved: [b T, B] + [B I, b] at 2 B."""
-    return ARG_BYTES * (b * T * B + B * I * b)
+def saved_bytes(b: int, B: int, T: int, I: int, m: int = 1, n: int = 1) -> int:
+    """Compact argmax of both passes when every chunk is saved: [m b T, n B] + [n B I, m b] at 2 B
+    (m text views, n image views; one view each is the single-view loss)."""
+    return ARG_BYTES * (m * b * T * n * B + n * B * I * m * b)
 
 
-def step_reserve_bytes(b: int, B: int, T: int, I: int, D: int, extra: bool) -> int:
+def step_reserve_bytes(b: int, B: int, T: int, I: int, D: int, extra: bool, m: int = 1, n: int = 1) -> int:
     """HBM the micro-batched step leaves to the loss when it plans which encoder chunks to keep: the
     saved argmax of both passes, the chunk budget, and per token row and latent pair 24 D bytes (the
     fp32 leaf and its gradient, the two split-bf16 operands)."""
     pairs = 2 if extra else 1
-    return saved_bytes(b, B, T, I) + FILIP_CHUNK_BYTES + 24 * D * (b * T + B * I) * pairs
+    return saved_bytes(b, B, T, I, m, n) + FILIP_CHUNK_BYTES + 24 * D * (m * b * T + n * B * I) * pairs
 
 
 class _Pass:
@@ -154,43 +155,57 @@ class FilipLossFn(torch.autograd.Function):
     Both passes run in row chunks of whole samples (pass A: captions of T rows; pass B: images of I
     rows), bounded by FILIP_CHUNK_BYTES.  The argmax of a chunk prefix is saved in 16 bits (the plan:
     FILIP_SAVE_BYTES, or the free HBM); the other chunks keep nothing and re-run their segment-max GEMM
-    in backward.  The loss does not depend on the plan.  `stats`, a dict, receives the plan's rows."""
+    in backward.  The loss does not depend on the plan.  `stats`, a dict, receives the plan's rows.
+
+    Augmented views (x_clip.py:625-650, :821-868): views = (m, n) with zt / text_mask holding m text
+    views and zi n image views of the same b pairs, stacked along the batch; weights = (cl_w, mv_w).
+    Every (text view i, image view j) pair is a FILIP loss of its own, text view i masked by its own
+    rows of text_mask, and the result is cl_w L[0, 0] + mv_w mean(the other m n - 1 pairs).  The two
+    passes simply grow: pass A's rows are the m views' text tokens [m b T] against the n views' image
+    tokens of every rank [n B I], pass B the reverse; t2i and i2t become [m b, n B] and the block
+    kernels (xclip_filip_nce_blocks_fwd / _bwd) run the InfoNCE / DCL of all m n blocks in one launch
+    per direction.  Image columns are rank-major - rank r's n views in turn, the order the one
+    all-gather of the stacked local views gives and the reduce-scatter takes back - so image view j's
+    sample r b + y is column r n b + j b + y (positive_column).  views = (1, 1) is the single-view
+    loss, on the single-view kernels."""
 
     @staticmethod
     def forward(ctx, zt, zi, zt_x, zi_x, temperature, ops, text_mask, dcl: bool, use_gather: bool,
-                stats=None):
+                stats=None, views=(1, 1), weights=None):
+        m, n = views
         extra = len(ops) == 4
         rank, world = D_.world() if use_gather else (0, 1)
-        b, T, D = zt.shape
+        T, D = zt.shape[1], zt.shape[2]
+        b = zt.shape[0] // m
         I = zi.shape[1]
         B, off = world * b, rank * b
         dev = zt.device
         temp_exp = temperature.detach().float().exp().reshape(1)
-        mask = text_mask.reshape(b * T)
+        mask = text_mask.reshape(m * b * T)
         cnt = text_mask.sum(dim=1).clamp(min=1e-6).float()                       # x_clip.py:40-44
-        w_t = (text_mask.float() / cnt[:, None]).reshape(b * T).contiguous()
-        w_i = torch.full((B * I,), 1.0 / I, device=dev, dtype=F32)
+        w_t = (text_mask.float() / cnt[:, None]).reshape(m * b * T).contiguous()
+        w_i = torch.full((n * B * I,), 1.0 / I, device=dev, dtype=F32)
         col_mul = mask.float().contiguous()
         col_add = torch.where(mask, torch.zeros((), device=dev),
                               torch.full((), -torch.finfo(F32).max, device=dev)).contiguous()
 
         img = list(ops[1]) + (list(ops[3]) if extra else [])       # (row, col) forms of image tokens
-        img_all = D_.gather_rows(img) if world > 1 else img        # ONE all-gather: [B*I, 3D] each
+        img_all = D_.gather_rows(img) if world > 1 else img        # ONE all-gather: [n*B*I, 3D] each
         irow_all, icol_all = img_all[0], img_all[1]
         trow, tcol = ops[0]
         if extra:
             rows_i, cols_t = img_all[2], ops[2][1]
         else:
             rows_i, cols_t = irow_all, tcol
-        pa = _Pass(trow, icol_all, I, None, None, T)                              # [b*T, B]
-        pb = _Pass(rows_i, cols_t, T, col_mul, col_add, I)                        # [B*I, b]
+        pa = _Pass(trow, icol_all, I, None, None, T)                              # [m*b*T, n*B]
+        pb = _Pass(rows_i, cols_t, T, col_mul, col_add, I)                        # [n*B*I, m*b]
         budget = FILIP_SAVE_BYTES
         if budget is None:
             budget = max(0, _avail_bytes(dev) - FILIP_SAVE_MARGIN_BYTES - FILIP_CHUNK_BYTES)
         budget -= pa.plan(budget)
         pb.plan(budget)
-        t2i = torch.empty((b, B), device=dev, dtype=F32)
-        i2t = torch.empty((b, B), device=dev, dtype=F32)                          # (text, image)
+        t2i = torch.empty((m * b, n * B), device=dev, dtype=F32)
+        i2t = torch.empty((m * b, n * B), device=dev, dtype=F32)                  # (text, image)
         pa.forward(temp_exp, w_t, t2i, transpose=False)
         pb.forward(temp_exp, w_i, i2t, transpose=True)
 
@@ -200,8 +215,14 @@ class FilipLossFn(torch.autograd.Function):
         has_tokens = text_mask.any(dim=1).contiguous()
 
         loss = torch.zeros(1, device=dev, dtype=F32)
-        lse_t = K.filip_nce_fwd(t2i, off, dcl, loss, 1.0 / (2 * B))
-        lse_i = K.filip_nce_fwd(i2t, off, dcl, loss, 1.0 / (2 * B), row_valid=has_tokens)
+        block_w = None
+        if m * n == 1:
+            lse_t = K.filip_nce_fwd(t2i, off, dcl, loss, 1.0 / (2 * B))
+            lse_i = K.filip_nce_fwd(i2t, off, dcl, loss, 1.0 / (2 * B), row_valid=has_tokens)
+        else:
+            block_w = torch.tensor(view_block_weights(m, n, weights[0], weights[1], B), device=dev, dtype=F32)
+            lse_t = K.filip_nce_blocks_fwd(t2i, m, n, b, off, dcl, block_w, loss)
+            lse_i = K.filip_nce_blocks_fwd(i2t, m, n, b, off, dcl, block_w, loss, row_valid=has_tokens)
         if world > 1:
             D_.all_reduce_sum_(loss)
 
@@ -210,17 +231,22 @@ class FilipLossFn(torch.autograd.Function):
                          rows_recomputed=(pa.R - pa.saved_rows) + (pb.R - pb.saved_rows),
                          saved_bytes=ARG_BYTES * (pa.saved_rows * pa.nseg + pb.saved_rows * pb.nseg),
                          chunks=len(pa.chunks) + len(pb.chunks))
-        ctx.cfg = (dcl, extra, rank, world, b, B, T, I, D, off)
-        ctx.stuff = (temp_exp, ops, img_all, w_t, w_i, pa, pb, t2i, i2t, lse_t, lse_i, has_tokens)
+        ctx.cfg = (dcl, extra, rank, world, m, n, b, B, T, I, D, off)
+        ctx.stuff = (temp_exp, ops, img_all, w_t, w_i, pa, pb, t2i, i2t, lse_t, lse_i, has_tokens, block_w)
         return loss.reshape(())
 
     @staticmethod
     def backward(ctx, gloss):
-        dcl, extra, rank, world, b, B, T, I, D, off = ctx.cfg
-        temp_exp, ops, img_all, w_t, w_i, pa, pb, t2i, i2t, lse_t, lse_i, has_tokens = ctx.stuff
-        gscale = (gloss.detach().float() / (2.0 * B)).reshape(1)
-        g_t = K.filip_nce_bwd(t2i, lse_t, off, dcl, gscale)                      # [x local, y all]
-        g_i = K.filip_nce_bwd(i2t, lse_i, off, dcl, gscale, row_valid=has_tokens)  # [x local, y all]
+        dcl, extra, rank, world, m, n, b, B, T, I, D, off = ctx.cfg
+        temp_exp, ops, img_all, w_t, w_i, pa, pb, t2i, i2t, lse_t, lse_i, has_tokens, block_w = ctx.stuff
+        if block_w is None:
+            gscale = (gloss.detach().float() / (2.0 * B)).reshape(1)
+            g_t = K.filip_nce_bwd(t2i, lse_t, off, dcl, gscale)                      # [x local, y all]
+            g_i = K.filip_nce_bwd(i2t, lse_i, off, dcl, gscale, row_valid=has_tokens)  # [x local, y all]
+        else:                                            # the block weights carry 1 / (2 B)
+            gscale = gloss.detach().float().reshape(1)
+            g_t = K.filip_nce_blocks_bwd(t2i, lse_t, m, n, b, off, dcl, block_w, gscale)
+            g_i = K.filip_nce_blocks_bwd(i2t, lse_i, m, n, b, off, dcl, block_w, gscale, row_valid=has_tokens)
         # t2i and i2t are exp(temperature) times a function of the latents alone, so
         # d loss / d temperature = sum g_t * t2i + sum g_i * i2t.  An empty caption's i2t row (the
         # -FLT_MAX fill, possibly -inf) has g_i = 0 and is left out rather than multiplied.
@@ -243,7 +269,7 @@ class FilipLossFn(torch.autograd.Function):
         if world > 1:
             D_.all_reduce_sum_(dtemp)
         ctx.stuff = None
-        shp_t, shp_i = (b, T, D), (b, I, D)
+        shp_t, shp_i = (m * b, T, D), (n * b, I, D)
         grads = (dzt.view(shp_t), dzi.view(shp_i),
                  None if dzt_x is None else dzt_x.view(shp_t),
                  None if dzi_x is None else dzi_x.view(shp_i),
@@ -251,9 +277,26 @@ class FilipLossFn(torch.autograd.Function):
         return grads + (None,) * (len(ctx.needs_input_grad) - len(grads))
 
 
-def filip_loss(clip, zt, zi, zt_x, zi_x, ops, text_mask, temperature=None, stats=None):
+def view_block_weights(m: int, n: int, cl_w: float, mv_w: float, B: int) -> list:
+    """Loss weight of each (text view i, image view j) block, i * n + j, scale 1 / (2 B) included:
+    cl_w on the (0, 0) pair, mv_w / (m n - 1) on every other (x_clip.py:851-868)."""
+    other = mv_w / (m * n - 1) if m * n > 1 else 0.0
+    return [(cl_w if k == 0 else other) / (2 * B) for k in range(m * n)]
+
+
+def positive_column(i: int, j: int, x: int, rank: int, b: int, n: int, col_run: int) -> int:
+    """Column of the positive of text view i's local row x in image view j's block, in a view-block
+    matrix with runs of col_run samples (col_run = b: rank-major, FilipLossFn's order; col_run = W b:
+    view-major); the arithmetic of xclip_filip_nce_blocks_fwd.  i does not move it."""
+    k = rank * b + x
+    return (k // col_run) * n * col_run + j * col_run + k % col_run
+
+
+def filip_loss(clip, zt, zi, zt_x, zi_x, ops, text_mask, temperature=None, stats=None, views=(1, 1),
+               weights=None):
+    """views = (m, n) text / image views stacked along the batch, weights = (cl_w, mv_w): FilipLossFn."""
     extra = clip.extra_latent_projection
     return FilipLossFn.apply(zt, zi, zt_x if extra else None, zi_x if extra else None,
                              clip.temperature if temperature is None else temperature, tuple(ops),
                              text_mask.contiguous(), clip.decoupled_contrastive_learning,
-                             clip.requires_all_gather, stats)
+                             clip.requires_all_gather, stats, tuple(views), weights)

@@ -575,6 +575,40 @@ def filip_nce_bwd(s, lse, diag_off, dcl, gscale, row_valid=None):
     return g
 
 
+def _blocks_args(s, m, n, row_valid, block_w):
+    """(rows per view b, global batch B) of a view-block matrix s [m*b, n*B] with unit column stride."""
+    R, C = s.shape
+    if s.dtype != F32 or s.stride(1) != 1 or R % m or C % n:
+        raise _lib.XClipB200Error(f"filip_nce_blocks: s must be f32 [m*b, n*B] with unit column stride, "
+                                  f"got {tuple(s.shape)} for m={m}, n={n}")
+    if block_w.dtype != F32 or block_w.numel() != m * n or not block_w.is_contiguous() or block_w.device != s.device:
+        raise _lib.XClipB200Error(f"filip_nce_blocks: block_w must be a contiguous f32 [{m * n}] on the device of s")
+    _row_valid(row_valid, s)
+    return R // m, C // n
+
+
+def filip_nce_blocks_fwd(s, m, n, col_run, diag_off, dcl, block_w, loss_accum, row_valid=None):
+    """lse [m*b, n] of every (row, view block) of s; see xclip_filip_nce_blocks_fwd."""
+    b, B = _blocks_args(s, m, n, row_valid, block_w)
+    lse = torch.empty((m * b, n), device=s.device, dtype=F32)
+    _call(s, "filip_small", 0.0, 4.0 * s.numel(), "xclip_filip_nce_blocks_fwd", s.data_ptr(), s.stride(0), m, n,
+          b, B, int(col_run), int(diag_off), 1 if dcl else 0, _ptr(row_valid), block_w.data_ptr(), lse.data_ptr(),
+          _ptr(loss_accum))
+    return lse
+
+
+def filip_nce_blocks_bwd(s, lse, m, n, col_run, diag_off, dcl, block_w, gscale, row_valid=None):
+    """g f32 [m*b, n*B] (contiguous) of the view-block loss; see xclip_filip_nce_blocks_bwd."""
+    b, B = _blocks_args(s, m, n, row_valid, block_w)
+    if lse.dtype != F32 or tuple(lse.shape) != (m * b, n) or not lse.is_contiguous():
+        raise _lib.XClipB200Error(f"filip_nce_blocks_bwd: lse must be a contiguous f32 [{m * b}, {n}]")
+    g = torch.empty((m * b, n * B), device=s.device, dtype=F32)
+    _call(s, "filip_small", 0.0, 8.0 * s.numel(), "xclip_filip_nce_blocks_bwd", s.data_ptr(), s.stride(0),
+          lse.data_ptr(), m, n, b, B, int(col_run), int(diag_off), 1 if dcl else 0, _ptr(row_valid),
+          block_w.data_ptr(), gscale.data_ptr(), g.data_ptr(), g.stride(0))
+    return g
+
+
 ARG16_MAX_SEG_LEN = 65535
 
 
