@@ -351,20 +351,32 @@ int xclip_adamw_step(float* p, const float* g, float* m, float* v, int64_t n, fl
 /* ---- patch-embedding front end (x_clip/x_clip.py:356-359 patchify, :134-151 PatchDropout) -------
  * patchify_gather : img f32 [B,C,H,W] -> bf16 [B*k, patch*patch*C] rows in the reference's
  *                   (p1 p2 c) order for the patches keep[b, j] (int64 [B,k]; NULL = all k = n patches,
- *                   in order): only kept patches are read and embedded.
+ *                   in order): only kept patches are read and embedded.  patch*patch*C %% 8 == 0.
+ * patchify_gather_rows: the same for any patch*patch*C, into rows of stride ldo (ldo %% 8 == 0,
+ *                   ldo >= patch*patch*C, out 16-byte aligned); columns patch*patch*C .. ldo-1 are
+ *                   written as zeros, so the rows are a GEMM operand with K = ldo.  patchify_gather is
+ *                   this call with ldo = patch*patch*C.
  * patchify_scatter: the inverse (the image gradient): src f32 [B*k, patch*patch*C] (row stride lds, rows
  *                   in the gather's order, (p1 p2 c) inside a row) -> img_grad f32 [B,C,H,W].  Every
  *                   element is written: pixels of the patch keep[b, j] take row b*k + j, pixels of
  *                   patches absent from keep[b, :] are 0 (allocate img_grad uninitialised).  The indices
  *                   of one sample must be distinct (PatchDropout draws them with topk), so no pixel has
  *                   two sources and no atomics are used; with duplicates the result is unspecified.
- *                   src and img_grad 16-byte aligned, lds %% 4 == 0; the other refusals are the gather's.
+ *                   src and img_grad 16-byte aligned, lds %% 4 == 0, patch*patch*C %% 8 == 0,
+ *                   0 < k <= n patches; the other refusals are the gather's.
+ * patchify_scatter_rows: the same for any patch*patch*C; reads only the first patch*patch*C columns
+ *                   of each src row (lds >= patch*patch*C).  patchify_scatter is this call after its
+ *                   patch*patch*C %% 8 check.
  * scatter_add_rows: dst f32 [V,d] rows idx[r] (or r %% period) += src bf16 [rows,d]  (gradient of the
  *                   gathered position table);  colsum_rows: dst[d] += column sums (bias gradient). */
 int xclip_patchify_gather(const float* img, int B, int C, int H, int W, int patch, const int64_t* keep,
                           int k, void* out, xclip_stream_t stream);
 int xclip_patchify_scatter(const float* src, int64_t lds, int B, int C, int H, int W, int patch,
                            const int64_t* keep, int k, float* img_grad, xclip_stream_t stream);
+int xclip_patchify_gather_rows(const float* img, int B, int C, int H, int W, int patch,
+                               const int64_t* keep, int k, void* out, int64_t ldo, xclip_stream_t stream);
+int xclip_patchify_scatter_rows(const float* src, int64_t lds, int B, int C, int H, int W, int patch,
+                                const int64_t* keep, int k, float* img_grad, xclip_stream_t stream);
 int xclip_scatter_add_rows(const int32_t* idx, int period, const void* src, int64_t lds, float* dst,
                            int64_t rows, int d, int V, xclip_stream_t stream);
 int xclip_colsum_rows(const void* src, int64_t lds, float* dst, int64_t rows, int d,

@@ -36,6 +36,10 @@ SIGNATURES = {
                                       c_void_p]),
     "xclip_patchify_scatter": (c_int, [c_void_p, c_int64, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int,
                                        c_void_p, c_void_p]),
+    "xclip_patchify_gather_rows": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int,
+                                           c_void_p, c_int64, c_void_p]),
+    "xclip_patchify_scatter_rows": (c_int, [c_void_p, c_int64, c_int, c_int, c_int, c_int, c_int, c_void_p,
+                                            c_int, c_void_p, c_void_p]),
     "xclip_scatter_add_rows": (c_int, [c_void_p, c_int, c_void_p, c_int64, c_void_p, c_int64, c_int, c_int,
                                        c_void_p]),
     "xclip_colsum_rows": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_int, c_void_p]),

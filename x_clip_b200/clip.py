@@ -12,7 +12,9 @@ Sequence length is not limited by the non-causal attention: image towers such as
 tokens: cfg3's 77 x 196 (98 under patch dropout), 576-patch towers and grids smaller than 16 tokens
 run on the same segment-max kernels.  Model and latent widths may be any multiple of 128 from 128 to
 1024 (ViT-S at 384, B/16-plus at 640 / 896, tiny 128-wide ablations), with any head count: the
-attention width heads * 64 need not equal the model width.  Feature combinations the kernels do not
+attention width heads * 64 need not equal the model width.  Any patch size works, ViT-L/14's 588
+values per patch included: the patch embedding pads rows of channels * patch^2 values to a multiple of
+8 with zero columns (engine.patch_rows), which adds exact zeros to its sums.  Feature combinations the kernels do not
 cover raise at construction (never a silent CPU or eager fallback): dim_head != 64, model or latent
 widths that are not 128 * {1..8}, a causal text tower longer than
 128 tokens, rotary + causal together (broken in the reference itself: n+1 angles for n tokens,
@@ -256,7 +258,6 @@ class VisionTransformer(nn.Module):
         self.patch_size = patch_size
         num_patches = (image_size // patch_size) ** 2
         patch_dim = channels * patch_size ** 2
-        _require(patch_dim % 8 == 0, "channels * patch_size^2 must be a multiple of 8")
         self.to_tokens = nn.Sequential(_Slot(), nn.Linear(patch_dim, dim))
         self.pos_emb = nn.Embedding(num_patches, dim)
         self.patch_dropout = PatchDropout(patch_dropout)
@@ -288,7 +289,7 @@ class VisionTransformer(nn.Module):
             # patch gradients back to pixels; every other call keeps the launch sequence below
             tok = E.PatchifyFn.apply(x, p, keep, index, lin.weight, lin.bias, self.pos_emb.weight)
         else:
-            patches = E.K.patchify_gather(x, p, keep)
+            patches = E.patch_rows(x, p, keep)
             tok = E.PatchEmbedFn.apply(patches, index, lin.weight, lin.bias, self.pos_emb.weight)
         out = self.transformer(tok.view(b, k, -1))
         pooled = out.float().mean(dim=1).to(BF16)

@@ -3,6 +3,8 @@
 //   fwd : out[b,0,:] = cls ; out[b,1+t,:] = tok[ids[b,t],:] + pos[t,:]      fp32 tables -> bf16
 //   bwd : dtok[ids[b,t],:] += dx[b,1+t,:]   (vector fp32 reductions into the table gradient)
 //         dpos[t,:] = sum_b dx[b,1+t,:] ; dcls = sum_b dx[b,0,:]            (column sums, no atomics)
+#include <climits>
+
 #include "common.cuh"
 #include "host.h"
 
@@ -225,13 +227,15 @@ extern "C" int xclip_rotary_inplace(void* qkv, int64_t ld, int64_t rows, int n, 
 // kept ones gives the same tokens (the position-table row is selected by the same index).
 // ---------------------------------------------------------------------------------------------
 namespace xclip {
+// Rows have stride ldo (a multiple of 8): columns patch_dim .. ldo-1 are written as exact zeros, so a
+// row of any patch_dim is a whole number of 16-byte stores and a GEMM A operand with K = ldo.
 __global__ void __launch_bounds__(256)
 patchify_gather_kernel(const float* __restrict__ img, int B, int C, int H, int W, int P,
                        const long long* __restrict__ keep, int k, int n_patches,
-                       bf16* __restrict__ out) {
+                       bf16* __restrict__ out, int ldo) {
   const int gw_n = W / P;
   const int patch_dim = P * P * C;
-  const int vec_per_row = patch_dim / 8;
+  const int vec_per_row = ldo / 8;
   const long long total = (long long)B * k * vec_per_row;
   for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
        idx += (long long)gridDim.x * blockDim.x) {
@@ -247,12 +251,14 @@ patchify_gather_kernel(const float* __restrict__ img, int B, int C, int H, int W
       const int el = e0 + e;
       const int q = el / C, c = el - q * C;
       const int p1 = q / P, p2 = q - p1 * P;
-      f[e] = __ldg(img + ((b * C + c) * H + gh * P + p1) * (long long)W + gw * P + p2);
+      f[e] = el < patch_dim
+                 ? __ldg(img + ((b * C + c) * H + gh * P + p1) * (long long)W + gw * P + p2)
+                 : 0.f;
     }
     uint4 o;
     o.x = pack_bf16x2(f[0], f[1]); o.y = pack_bf16x2(f[2], f[3]);
     o.z = pack_bf16x2(f[4], f[5]); o.w = pack_bf16x2(f[6], f[7]);
-    *reinterpret_cast<uint4*>(out + row * patch_dim + e0) = o;
+    *reinterpret_cast<uint4*>(out + row * ldo + e0) = o;
   }
 }
 
@@ -260,14 +266,20 @@ patchify_gather_kernel(const float* __restrict__ img, int B, int C, int H, int W
 // and writes every pixel of them, the src row of a kept patch or 0 for a dropped one.  The row of each
 // owned patch comes from an inverse map of keep[b, :] built in shared memory (indices of one sample are
 // distinct, so each slot has at most one writer).
-//   CT > 0 (C == CT, patch % 4 == 0): a thread owns 4 horizontally adjacent pixels of one patch row:
-//          CT 16-byte loads of the (p1 p2 c) row (4 pixels x CT channels, contiguous), transposed in
-//          registers, CT 16-byte stores, one per channel plane.  Consecutive threads walk along p2, so
-//          loads are contiguous across a warp and stores fill whole 32-byte sectors of an image row.
-//   CT == 0: any C / patch, one pixel x C channels per thread with scalar accesses.
+//   CT > 0 (C == CT): a thread owns V horizontally adjacent pixels of one patch row (V = 4 when
+//          patch % 4 == 0, V = 2 when patch % 4 == 2): CT V-wide vector loads of the (p1 p2 c) row
+//          (V pixels x CT channels, contiguous), transposed in registers, CT V-wide stores, one per
+//          channel plane.  Consecutive threads walk along p2, so loads are contiguous across a warp
+//          and stores fill whole 32-byte sectors of an image row.  Vector alignment: lds % 4 == 0 and
+//          16-byte aligned src / img; (p1 * P + p2) * C and every image offset are multiples of V.
+//   CT == 0 (V == 1): any C / patch, one pixel x C channels per thread with scalar accesses.
+// With V < 4 a patch row is not a whole number of 32-byte sectors (14 pixels: 56 bytes), so the work
+// items run along image rows across the block's patches rather than patch by patch: consecutive
+// threads then store consecutive pixels of an image row whichever patch they fall in.
+// Only the first patch_dim columns of a src row are read.
 constexpr int kScatterMaxPatchesPerBlock = 1024;
 
-template <int CT>
+template <int CT, int V>
 __global__ void __launch_bounds__(256)
 patchify_scatter_kernel(const float* __restrict__ src, long long lds, int B, int C, int H, int W, int P,
                         const long long* __restrict__ keep, int k, int n_patches, int ppc,
@@ -288,14 +300,23 @@ patchify_scatter_kernel(const float* __restrict__ src, long long lds, int B, int
     __syncthreads();
   }
   const int gw_n = W / P;
-  const int per_row = (CT > 0) ? P / 4 : P;          // work items per patch row
+  const int per_row = P / V;               // work items per patch row
   const int per_patch = P * per_row;
   const int items = cnt * per_patch;       // < 2^31 for patch sizes up to 2048
   for (int it = threadIdx.x; it < items; it += blockDim.x) {
-    const int pl = it / per_patch;
-    const int w = it - pl * per_patch;
-    const int p1 = w / per_row;
-    const int p2 = (w - p1 * per_row) * (CT > 0 ? 4 : 1);
+    int pl, p1, p2;
+    if constexpr (V == 4) {                // patch by patch: a warp's loads are one contiguous run
+      pl = it / per_patch;
+      const int w = it - pl * per_patch;
+      p1 = w / per_row;
+      p2 = (w - p1 * per_row) * V;
+    } else {                               // pixel row p1 of every owned patch in turn: a warp's
+      const int per_line = cnt * per_row;  // stores run along an image row across patches
+      p1 = it / per_line;
+      const int r = it - p1 * per_line;
+      pl = r / per_row;
+      p2 = (r - pl * per_row) * V;
+    }
     const int pidx = lo + pl;
     const int j = keep != nullptr ? inv[pl] : pidx;
     const int gh = pidx / gw_n, gw = pidx - gh * gw_n;
@@ -303,21 +324,30 @@ patchify_scatter_kernel(const float* __restrict__ src, long long lds, int B, int
     float* dst = img + (b * C) * plane + (long long)(gh * P + p1) * W + gw * P + p2;
     const float* s = j >= 0 ? src + (b * k + j) * lds + (long long)(p1 * P + p2) * C : nullptr;
     if constexpr (CT > 0) {
-      float v[4 * CT];
+      float v[V * CT];
       if (j >= 0) {
 #pragma unroll
         for (int i = 0; i < CT; ++i) {
-          const float4 t = *reinterpret_cast<const float4*>(s + 4 * i);
-          v[4 * i] = t.x; v[4 * i + 1] = t.y; v[4 * i + 2] = t.z; v[4 * i + 3] = t.w;
+          if constexpr (V == 4) {
+            const float4 t = *reinterpret_cast<const float4*>(s + 4 * i);
+            v[4 * i] = t.x; v[4 * i + 1] = t.y; v[4 * i + 2] = t.z; v[4 * i + 3] = t.w;
+          } else {
+            const float2 t = *reinterpret_cast<const float2*>(s + 2 * i);
+            v[2 * i] = t.x; v[2 * i + 1] = t.y;
+          }
         }
       } else {
 #pragma unroll
-        for (int i = 0; i < 4 * CT; ++i) v[i] = 0.f;
+        for (int i = 0; i < V * CT; ++i) v[i] = 0.f;
       }
 #pragma unroll
-      for (int c = 0; c < CT; ++c)
-        *reinterpret_cast<float4*>(dst + c * plane) =
-            make_float4(v[c], v[CT + c], v[2 * CT + c], v[3 * CT + c]);
+      for (int c = 0; c < CT; ++c) {
+        if constexpr (V == 4)
+          *reinterpret_cast<float4*>(dst + c * plane) =
+              make_float4(v[c], v[CT + c], v[2 * CT + c], v[3 * CT + c]);
+        else
+          *reinterpret_cast<float2*>(dst + c * plane) = make_float2(v[c], v[CT + c]);
+      }
     } else {
       for (int c = 0; c < C; ++c) dst[c * plane] = j >= 0 ? s[c] : 0.f;
     }
@@ -365,37 +395,64 @@ colsum_rows_kernel(const bf16* __restrict__ src, long long lds, float* __restric
 }
 }  // namespace xclip
 
-extern "C" int xclip_patchify_gather(const float* img, int B, int C, int H, int W, int patch,
-                                     const int64_t* keep, int k, void* out, xclip_stream_t stream) {
+extern "C" int xclip_patchify_gather_rows(const float* img, int B, int C, int H, int W, int patch,
+                                          const int64_t* keep, int k, void* out, int64_t ldo,
+                                          xclip_stream_t stream) {
   using namespace xclip;
   int rc = xclip_init();
   if (rc) return rc;
   XCLIP_REQUIRE(img && out && B > 0 && C > 0 && patch > 0 && H % patch == 0 && W % patch == 0,
                 "patchify: bad arguments");
   const int n_patches = (H / patch) * (W / patch);
-  XCLIP_REQUIRE((patch * patch * C) % 8 == 0, "patchify: channels*patch^2 must be a multiple of 8");
+  const long long patch_dim = (long long)patch * patch * C;
+  XCLIP_REQUIRE(ldo % 8 == 0 && ldo >= patch_dim && ldo <= INT_MAX,
+                "patchify: ldo=%lld must be a multiple of 8 and >= patch_dim=%lld", (long long)ldo,
+                patch_dim);
   XCLIP_REQUIRE(k > 0 && (keep != nullptr || k == n_patches), "patchify: k=%d", k);
   XCLIP_REQUIRE((reinterpret_cast<uintptr_t>(out) & 15) == 0, "patchify: misaligned output");
-  const long long total = (long long)B * k * (patch * patch * C / 8);
+  const long long total = (long long)B * k * (ldo / 8);
   long long blocks = (total + 255) / 256;
   if (blocks > (long long)num_sms() * 16) blocks = (long long)num_sms() * 16;
   patchify_gather_kernel<<<(int)blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       img, B, C, H, W, patch, reinterpret_cast<const long long*>(keep), k, n_patches,
-      reinterpret_cast<bf16*>(out));
+      reinterpret_cast<bf16*>(out), (int)ldo);
   XCLIP_LAUNCH_CHECK("patchify_gather_kernel");
   return XCLIP_OK;
 }
 
-extern "C" int xclip_patchify_scatter(const float* src, int64_t lds, int B, int C, int H, int W, int patch,
-                                      const int64_t* keep, int k, float* img_grad, xclip_stream_t stream) {
+extern "C" int xclip_patchify_gather(const float* img, int B, int C, int H, int W, int patch,
+                                     const int64_t* keep, int k, void* out, xclip_stream_t stream) {
+  using namespace xclip;
+  XCLIP_REQUIRE(((long long)patch * patch * C) % 8 == 0,
+                "patchify: channels*patch^2 must be a multiple of 8");
+  return xclip_patchify_gather_rows(img, B, C, H, W, patch, keep, k, out,
+                                    (int64_t)patch * patch * C, stream);
+}
+
+namespace xclip {
+template <int V>
+static void launch_scatter_vec(int C, dim3 grid, cudaStream_t s, const float* src, long long lds, int B,
+                               int H, int W, int P, const long long* keep, int k, int n_patches,
+                               int ppc, float* img) {
+  switch (C) {
+    case 1: patchify_scatter_kernel<1, V><<<grid, 256, 0, s>>>(src, lds, B, C, H, W, P, keep, k, n_patches, ppc, img); break;
+    case 2: patchify_scatter_kernel<2, V><<<grid, 256, 0, s>>>(src, lds, B, C, H, W, P, keep, k, n_patches, ppc, img); break;
+    case 3: patchify_scatter_kernel<3, V><<<grid, 256, 0, s>>>(src, lds, B, C, H, W, P, keep, k, n_patches, ppc, img); break;
+    default: patchify_scatter_kernel<4, V><<<grid, 256, 0, s>>>(src, lds, B, C, H, W, P, keep, k, n_patches, ppc, img); break;
+  }
+}
+}  // namespace xclip
+
+extern "C" int xclip_patchify_scatter_rows(const float* src, int64_t lds, int B, int C, int H, int W,
+                                           int patch, const int64_t* keep, int k, float* img_grad,
+                                           xclip_stream_t stream) {
   using namespace xclip;
   int rc = xclip_init();
   if (rc) return rc;
   XCLIP_REQUIRE(src && img_grad && B > 0 && C > 0 && patch > 0 && H % patch == 0 && W % patch == 0,
                 "patchify_scatter: bad arguments");
   const int n_patches = (H / patch) * (W / patch);
-  const int patch_dim = patch * patch * C;
-  XCLIP_REQUIRE(patch_dim % 8 == 0, "patchify_scatter: channels*patch^2 must be a multiple of 8");
+  const long long patch_dim = (long long)patch * patch * C;
   XCLIP_REQUIRE(k > 0 && k <= n_patches && (keep != nullptr || k == n_patches), "patchify_scatter: k=%d", k);
   XCLIP_REQUIRE(lds >= patch_dim && lds % 4 == 0 && (reinterpret_cast<uintptr_t>(src) & 15) == 0 &&
                     (reinterpret_cast<uintptr_t>(img_grad) & 15) == 0,
@@ -412,17 +469,22 @@ extern "C" int xclip_patchify_scatter(const float* src, int64_t lds, int B, int 
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   const long long* kp = reinterpret_cast<const long long*>(keep);
   if (patch % 4 == 0 && C <= 4) {
-    switch (C) {
-      case 1: patchify_scatter_kernel<1><<<grid, 256, 0, s>>>(src, lds, B, C, H, W, patch, kp, k, n_patches, ppc, img_grad); break;
-      case 2: patchify_scatter_kernel<2><<<grid, 256, 0, s>>>(src, lds, B, C, H, W, patch, kp, k, n_patches, ppc, img_grad); break;
-      case 3: patchify_scatter_kernel<3><<<grid, 256, 0, s>>>(src, lds, B, C, H, W, patch, kp, k, n_patches, ppc, img_grad); break;
-      default: patchify_scatter_kernel<4><<<grid, 256, 0, s>>>(src, lds, B, C, H, W, patch, kp, k, n_patches, ppc, img_grad); break;
-    }
+    launch_scatter_vec<4>(C, grid, s, src, lds, B, H, W, patch, kp, k, n_patches, ppc, img_grad);
+  } else if (patch % 2 == 0 && C <= 4) {
+    launch_scatter_vec<2>(C, grid, s, src, lds, B, H, W, patch, kp, k, n_patches, ppc, img_grad);
   } else {
-    patchify_scatter_kernel<0><<<grid, 256, 0, s>>>(src, lds, B, C, H, W, patch, kp, k, n_patches, ppc, img_grad);
+    patchify_scatter_kernel<0, 1><<<grid, 256, 0, s>>>(src, lds, B, C, H, W, patch, kp, k, n_patches, ppc, img_grad);
   }
   XCLIP_LAUNCH_CHECK("patchify_scatter_kernel");
   return XCLIP_OK;
+}
+
+extern "C" int xclip_patchify_scatter(const float* src, int64_t lds, int B, int C, int H, int W, int patch,
+                                      const int64_t* keep, int k, float* img_grad, xclip_stream_t stream) {
+  using namespace xclip;
+  XCLIP_REQUIRE(((long long)patch * patch * C) % 8 == 0,
+                "patchify_scatter: channels*patch^2 must be a multiple of 8");
+  return xclip_patchify_scatter_rows(src, lds, B, C, H, W, patch, keep, k, img_grad, stream);
 }
 
 extern "C" int xclip_scatter_add_rows(const int32_t* idx, int period, const void* src, int64_t lds,

@@ -354,24 +354,56 @@ class LinearFn(torch.autograd.Function):
         return dx, dw, db, dt
 
 
+def patch_rows(img, patch: int, keep):
+    """bf16 patch rows of `img` (the kept patches, K.patchify_gather) in the layout PatchEmbedFn
+    takes: [B*k, K.patch_row_stride(patch_dim)], zero columns after patch_dim."""
+    return K.patchify_gather(img, patch, keep, ld=K.patch_row_stride(patch * patch * img.shape[1]))
+
+
+def patch_weight_bf16(weight: torch.Tensor) -> torch.Tensor:
+    """bf16 patch-embedding weight [dim, K.patch_row_stride(patch_dim)] with zero columns after
+    patch_dim: the operand that meets patch_rows() in a GEMM with K = row stride (the zero columns add
+    exact zeros).  weight_bf16 itself when patch_dim is a multiple of 8; otherwise shared inside a
+    weight_scope() under a key of its own, apart from weight_bf16's unpadded casts."""
+    ld = K.patch_row_stride(weight.shape[1])
+    if ld == weight.shape[1]:
+        return weight_bf16(weight)
+    key = ("patch_rows", id(weight))
+    if _scope_cache is not None:
+        hit = _scope_cache.get(key)
+        if hit is not None and hit[0] is weight:
+            return hit[1]
+    w = K.cast_bf16_rows(weight.detach(), ld)
+    if _scope_cache is not None:
+        _scope_cache[key] = (weight, w)
+    return w
+
+
 def _patch_embed_fwd(ctx, patches, index, weight, bias, table, keep_wb: bool):
-    wb = weight_bf16(weight)
+    wb = patch_weight_bf16(weight)
     tbl16 = K.cast_bf16(table.detach())
     y = K.gemm(patches, wb, bias=bias.detach(), residual=tbl16, res_row_idx=index)
     ctx.save_for_backward(patches, index)
     ctx.wb = wb if keep_wb else None          # the dgrad operand, kept only when d patches is wanted
     ctx.table_rows = table.shape[0]
+    ctx.patch_dim = weight.shape[1]
     return y
 
 
 def _patch_embed_bwd(ctx, dy, need_dp: bool, need_w: bool, need_b: bool, need_t: bool):
-    """(d patches f32, dW, d bias, d pos), each None unless asked for"""
+    """(d patches f32 [M, row stride], dW [dim, patch_dim], d bias, d pos), each None unless asked for"""
     patches, index = ctx.saved_tensors
     dy = dy.contiguous()
     if dy.dtype != BF16:
         dy = dy.to(BF16)
     dp = K.gemm(dy, ctx.wb, b_major=1, out_dtype=F32) if need_dp else None
-    dw = _wgrad(dy, patches) if need_w else None
+    dw = None
+    if need_w:
+        # N = row stride; the columns past patch_dim are dropped into a contiguous [dim, patch_dim]
+        # gradient (GradSync / FusedAdamW flatten .grad, which would copy a strided view every step)
+        dw = _wgrad(dy, patches)
+        if dw.shape[1] != ctx.patch_dim:
+            dw = dw[:, :ctx.patch_dim].contiguous()
     db = K.colsum_rows_(torch.zeros(dy.shape[1], device=dy.device, dtype=F32), dy) if need_b else None
     dt = None
     if need_t:
@@ -385,9 +417,10 @@ class PatchEmbedFn(torch.autograd.Function):
     """tokens = patches @ W^T + bias + pos[index]  (x_clip.py:356-359, :382-383, with the
     PatchDropout selection :134-151 already applied to `patches` and `index`).
 
-    patches bf16 [B*k, patch_dim] come from K.patchify_gather (only the kept patches are read from
-    the image); `index` int32 [B*k] is the patch index of every row = the row of the position table
-    the GEMM epilogue adds.  Backward: d patches = dy @ W (f32 GEMM output; autograd hands it back in
+    patches bf16 [B*k, K.patch_row_stride(patch_dim)] come from patch_rows() (only the kept patches are
+    read from the image; zero columns after patch_dim, so any patch size runs on the GEMM); `index`
+    int32 [B*k] is the patch index of every row = the row of the position table the GEMM epilogue
+    adds.  Backward: d patches = dy @ W (f32 GEMM output; autograd hands it back in
     the dtype of `patches`), dW by the wgrad GEMM, d bias = column sums, d pos = rows of dy
     scatter-added by `index`; each only for inputs that need a gradient.  An image that wants a
     gradient goes through PatchifyFn instead, which keeps d patches in f32 up to the pixels."""
@@ -414,7 +447,7 @@ class PatchifyFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, img, patch: int, keep, index, weight, bias, table):
-        patches = K.patchify_gather(img, patch, keep)
+        patches = patch_rows(img, patch, keep)
         ctx.shape, ctx.patch, ctx.keep = tuple(img.shape), patch, keep
         return _patch_embed_fwd(ctx, patches, index, weight, bias, table, ctx.needs_input_grad[0])
 
@@ -423,7 +456,9 @@ class PatchifyFn(torch.autograd.Function):
     def backward(ctx, dy):
         n = ctx.needs_input_grad
         dp, dw, db, dt = _patch_embed_bwd(ctx, dy, n[0], n[4], n[5], n[6])
-        dimg = K.patchify_scatter(dp, ctx.shape, ctx.patch, ctx.keep) if dp is not None else None
+        dimg = None
+        if dp is not None:
+            dimg = K.patchify_scatter(dp[:, :ctx.patch_dim], ctx.shape, ctx.patch, ctx.keep)
         ctx.keep = None
         return dimg, None, None, None, dw, db, dt
 

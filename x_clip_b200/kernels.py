@@ -255,9 +255,17 @@ def attn_bwd(qkv, key_mask, o, d_o, lse, B, n, heads, scale, causal=False, dropo
     return dqkv
 
 
-def patchify_gather(img, patch, keep=None):
+def patch_row_stride(patch_dim: int) -> int:
+    """Row stride of the patch rows the patch-embedding GEMM reads: patch_dim rounded up to a multiple
+    of 8 (16-byte bf16 rows for TMA).  Equal to patch_dim for every patch of 8 * m values."""
+    return -(-int(patch_dim) // 8) * 8
+
+
+def patchify_gather(img, patch, keep=None, ld=None):
     """img f32 [B,C,H,W] -> bf16 [B*k, patch*patch*C] (reference (p1 p2 c) order) for the patches
-    keep[b, j] (int64 [B,k]) or all patches in order."""
+    keep[b, j] (int64 [B,k]) or all patches in order.  With `ld` (a multiple of 8, >= patch*patch*C)
+    the rows are [B*k, ld] with zero columns after patch*patch*C (xclip_patchify_gather_rows), for any
+    patch*patch*C; without it patch*patch*C must be a multiple of 8 (xclip_patchify_gather)."""
     _need(img, F32, "image")
     img = img.contiguous()
     B, C, H, W = img.shape
@@ -267,16 +275,32 @@ def patchify_gather(img, patch, keep=None):
         if keep.dtype != torch.int64 or keep.shape[0] != B or keep.device != img.device:
             raise _lib.XClipB200Error("patchify: keep must be int64 [B, k] on the image's device")
         keep = keep.contiguous()
-    out = torch.empty((B * k, patch * patch * C), device=img.device, dtype=BF16)
-    _call(img, "embed", 0.0, B * k * patch * patch * C * 6.0, "xclip_patchify_gather", img.data_ptr(), B, C, H, W,
-          int(patch), _ptr(keep), k, out.data_ptr())
+    pd = patch * patch * C
+    out = torch.empty((B * k, pd if ld is None else int(ld)), device=img.device, dtype=BF16)
+    args = (img.data_ptr(), B, C, H, W, int(patch), _ptr(keep), k, out.data_ptr())
+    nbytes = B * k * pd * 4.0 + out.numel() * 2.0
+    if ld is None:
+        _call(img, "embed", 0.0, nbytes, "xclip_patchify_gather", *args)
+    else:
+        _call(img, "embed", 0.0, nbytes, "xclip_patchify_gather_rows", *args, int(ld))
     return out
+
+
+def cast_bf16_rows(src: torch.Tensor, ld: int) -> torch.Tensor:
+    """f32 [rows, cols] -> bf16 [rows, ld] with zero columns after cols (a weight operand whose K is
+    padded to a multiple of 8).  The patch-1 gather of an image of `rows` samples, each one 1 x 1 pixel
+    of `cols` channels, is exactly this copy, so it runs on xclip_patchify_gather_rows."""
+    _need(src, F32, "src"); _rows2d(src, "src")
+    rows, cols = src.shape
+    return patchify_gather(src.reshape(rows, cols, 1, 1), 1, ld=ld)
 
 
 def patchify_scatter(src, image_shape, patch, keep=None):
     """Inverse of patchify_gather (the image gradient): src f32 [B*k, patch*patch*C] rows in the
-    gather's order -> f32 [B,C,H,W]; pixels of patches not in keep[b, :] are 0.  The indices of one
-    sample must be distinct (xclip_patchify_scatter)."""
+    gather's order (any row stride: a view of the first patch*patch*C columns of wider rows reads
+    only those) -> f32 [B,C,H,W]; pixels of patches not in keep[b, :] are 0.  The indices of one
+    sample must be distinct.  xclip_patchify_scatter when patch*patch*C is a multiple of 8,
+    xclip_patchify_scatter_rows otherwise."""
     _need(src, F32, "src"); _rows2d(src, "src")
     B, C, H, W = (int(s) for s in image_shape)
     n = (H // patch) * (W // patch)
@@ -285,11 +309,13 @@ def patchify_scatter(src, image_shape, patch, keep=None):
         if keep.dtype != torch.int64 or keep.shape[0] != B or keep.device != src.device:
             raise _lib.XClipB200Error("patchify_scatter: keep must be int64 [B, k] on src's device")
         keep = keep.contiguous()
-    if src.shape[0] != B * k or src.shape[1] != patch * patch * C:
-        raise _lib.XClipB200Error(f"patchify_scatter: src must be [{B * k}, {patch * patch * C}], "
+    pd = patch * patch * C
+    if src.shape[0] != B * k or src.shape[1] != pd:
+        raise _lib.XClipB200Error(f"patchify_scatter: src must be [{B * k}, {pd}], "
                                   f"got {tuple(src.shape)}")
     out = torch.empty((B, C, H, W), device=src.device, dtype=F32)
-    _call(src, "embed", 0.0, (B * k + B * n) * patch * patch * C * 4.0, "xclip_patchify_scatter",
+    _call(src, "embed", 0.0, (B * k + B * n) * pd * 4.0,
+          "xclip_patchify_scatter" if pd % 8 == 0 else "xclip_patchify_scatter_rows",
           src.data_ptr(), src.stride(0), B, C, H, W, int(patch), _ptr(keep), k, out.data_ptr())
     return out
 
