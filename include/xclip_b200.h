@@ -168,6 +168,26 @@ int xclip_nce_bwd(const void* a, const void* b, int R, int C, int D, const float
                   float w_row, float w_col, float w_diag, const float* gscale, void* g,
                   int64_t ldg, float* dtemp, xclip_stream_t stream);
 
+/* ---- pairwise sigmoid loss (SigLIP, Zhai et al., ICCV 2023) on the operands of xclip_nce_* -------
+ * l[r,c] = *temp_exp * <a_r, b_c> + *logit_bias (both DEVICE scalars), z[r,c] = +1 if c == r +
+ * diag_offset else -1.  a, b, R, C, D, diag_offset and alignment as for xclip_nce_fwd / _bwd.
+ * fwd:  rowloss[r] = sum_c softplus(-z[r,c] l[r,c]) (f32 [R]);
+ *       *loss_accum += loss_scale * sum_r rowloss[r]   (loss_accum may be NULL).
+ *       part_ws: f32 scratch [xclip_nce_num_col_blocks(C) * R], 4-byte aligned; its blocks are summed
+ *       in a fixed order.  softplus is accurate to fp32 rounding for small terms (log1p, not
+ *       log(1 + x)), and a saturated logit gives softplus(x) = max(x, 0) exactly.
+ * bwd:  g[r,c] = *gscale * (sigmoid(l[r,c]) - [c == r + diag_offset]) (gscale: DEVICE scalar,
+ *       upstream grad / B_global), written as bf16 temp_exp*g [R, ldg >= roundup8(C)], ldg % 8 == 0,
+ *       zero in the columns [C, ldg); the latent gradient is then dA = (that) @ b via xclip_gemm_bf16.
+ *       *dtemp += sum g * (l - *logit_bias) (d loss / d temperature) and *dbias += sum g
+ *       (d loss / d logit_bias), each when non-NULL. */
+int xclip_sigmoid_fwd(const void* a, const void* b, int R, int C, int D, const float* temp_exp,
+                      const float* logit_bias, int diag_offset, float* part_ws, float* rowloss,
+                      float* loss_accum, float loss_scale, xclip_stream_t stream);
+int xclip_sigmoid_bwd(const void* a, const void* b, int R, int C, int D, const float* temp_exp,
+                      const float* logit_bias, int diag_offset, const float* gscale, void* g,
+                      int64_t ldg, float* dtemp, float* dbias, xclip_stream_t stream);
+
 /* ---- vocabulary cross-entropy of the MLM head (x_clip/mlm.py:96-107) on the same kernels ----------
  * l[r,v] = <x_r, w_v> + bias[v] for x bf16 [R,D] (the selected token encodings), w bf16 [V,D] (the
  * bf16 cast of to_logits.weight), bias f32 [V] or NULL; labels int64 [R] hold each row's target in

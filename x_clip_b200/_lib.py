@@ -69,6 +69,10 @@ SIGNATURES = {
     "xclip_nce_bwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int,
                               c_void_p, c_void_p, c_float, c_float, c_float, c_void_p, c_void_p,
                               c_int64, c_void_p, c_void_p]),
+    "xclip_sigmoid_fwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int,
+                                  c_void_p, c_void_p, c_void_p, c_float, c_void_p]),
+    "xclip_sigmoid_bwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int,
+                                  c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
     "xclip_vocab_ce_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p,
                                    c_void_p, c_void_p, c_void_p, c_float, c_void_p]),
     "xclip_vocab_ce_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p,

@@ -27,10 +27,15 @@ pair of segment-max passes (filip.FilipLossFn), each text view masked by its own
 (`sim_reg_loss_weight > 0`) runs fused with the contrastive loss (engine.ContrastiveLossFn) where the
 reference itself runs it: with `extra_latent_projection=True`, without FILIP and with a single view;
 the other combinations fail inside the reference (x_clip.py:779) and raise `Unsupported` here.
+`sigmoid_loss=True` (an extension) trains with SigLIP's pairwise sigmoid loss (engine.SigmoidLossFn) in
+place of InfoNCE: a new scalar parameter `logit_bias` (initial -10) and `temperature` initialised to
+log 10.  It runs in the single pass, with augmented views, MLM / SimSiam / SimCLR and in the micro-batched
+step; FILIP, DCL and the extra latent projection (and so the similarity regularisation) raise `Unsupported`.
 """
 from __future__ import annotations
 
 import copy
+import math
 from typing import Optional
 
 import torch
@@ -354,11 +359,21 @@ class CLIP(nn.Module):
         **kwargs,     # unknown keywords are swallowed, like the reference (:455)
     ):
         super().__init__()
+        # (extension) sigmoid_loss=False: SigLIP's pairwise sigmoid loss in place of InfoNCE.  Taken from
+        # **kwargs, so that the explicit signature stays the reference's plus the micro-batch options
+        sigmoid_loss = bool(kwargs.pop("sigmoid_loss", False))
         assert use_all_token_embeds or (visual_has_cls_token or text_has_cls_token), \
             'CLS token must be included on both vision and text transformers if you are not using fine-grained contrastive learning loss'
         assert not (text_causal_mask and text_eos_id is None), \
             'text EOS token id must be given if using causal mask in text transformer'
         _require(not downsample_image_embeds, "downsample_image_embeds is not implemented")
+        if sigmoid_loss:
+            _require(not use_all_token_embeds, "sigmoid_loss with use_all_token_embeds (no FILIP variant of the sigmoid loss)")
+            _require(not decoupled_contrastive_learning,
+                     "sigmoid_loss with decoupled_contrastive_learning (DCL changes a softmax denominator the sigmoid loss does not have)")
+            _require(not extra_latent_projection and sim_reg_loss_weight <= 0.,
+                     "sigmoid_loss with extra_latent_projection or sim_reg_loss_weight > 0 (the sigmoid loss is "
+                     "symmetric: it has no image-to-text direction for a second projection)")
         if sim_reg_loss_weight > 0.:
             # without the extra projection the reference's einsum at x_clip.py:779 gets the 2-D
             # un-rearranged text_latents_extra and fails; with FILIP its [1, B, B] mask cannot index
@@ -425,7 +440,11 @@ class CLIP(nn.Module):
 
         self.to_text_latent = nn.Linear(dim_text, dim_latent, bias=False)
         self.to_visual_latent = nn.Linear(dim_image, dim_latent, bias=False)
-        self.temperature = nn.Parameter(torch.tensor(1.))
+        # SigLIP's initial logit scale 10 and bias -10 (Zhai et al. 2023; open_clip's SigLIP models)
+        self.sigmoid_loss = sigmoid_loss
+        self.temperature = nn.Parameter(torch.tensor(math.log(10.) if sigmoid_loss else 1.))
+        if sigmoid_loss:
+            self.logit_bias = nn.Parameter(torch.tensor(-10.))
 
         self.use_all_token_embeds = use_all_token_embeds
         self.decoupled_contrastive_learning = decoupled_contrastive_learning
@@ -547,7 +566,8 @@ class CLIP(nn.Module):
             assert self.training, 'loss cannot be used if not training'
             aux = self._aux_inputs(text, image) if (self.use_mlm or self.use_visual_ssl) else None
             return E.ChunkedClipLossFn.apply(self, text, image, text_mask, int(self.microbatch),
-                                             self.temperature, self.microbatch_retain, aux)
+                                             self.temperature, self.microbatch_retain, aux,
+                                             *((self.logit_bias,) if self.sigmoid_loss else ()))
 
         # auxiliary losses on the un-augmented batch (reference :616-621)
         text_ssl_loss = image_ssl_loss = 0
@@ -608,6 +628,8 @@ class CLIP(nn.Module):
             return zt, zi
 
         if not return_loss:
+            # exp(temperature) * similarity, as the reference returns; with sigmoid_loss the logit_bias
+            # is not added (add clip.logit_bias for the logits the sigmoid loss sees)
             temp = self.temperature.exp()
             a, b = (zt_x, zi_x) if (self.extra_latent_projection and not text_to_image) else (zt, zi)
             if self.use_all_token_embeds:
@@ -636,6 +658,9 @@ class CLIP(nn.Module):
             """contrastive loss of text view rows `tsl` against image view rows `isl`; sim_reg =
             (weight, contrastive weight) adds the similarity regularisation (ContrastiveLossFn)"""
             o = [(ops[0][0][tsl], ops[0][1][tsl]), (ops[1][0][isl], ops[1][1][isl])]
+            if self.sigmoid_loss:
+                return E.SigmoidLossFn.apply(zt[tsl], zi[isl], self.temperature, self.logit_bias, tuple(o),
+                                             self.requires_all_gather)
             if self.extra_latent_projection:
                 o += [(ops[2][0][tsl], ops[2][1][tsl]), (ops[3][0][isl], ops[3][1][isl])]
             return E.ContrastiveLossFn.apply(

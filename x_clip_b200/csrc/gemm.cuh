@@ -90,6 +90,10 @@ struct GemmParams {
   bf16* ff_out2;           // DOWN: bf16(acc) [M, d]
   long long ff_ld2;
   const float* ff_ab;      // BWD: [M,2] per-row (mean_k(gdh), mean_k(gdh * hn)) from xclip_ff_bwd_prep
+  // ---- sigmoid (SigLIP) epilogues (EPI_SIG_*): logit = alpha * acc + *logit_bias; alpha_dev,
+  // gscale_dev, diag_offset, nce_part, c / ldc and dtemp as for the InfoNCE epilogues
+  const float* logit_bias; // device scalar (no host sync)
+  float* dbias;            // BWD: scalar accumulator of sum(g) or null
 };
 
 constexpr int EPI_STORE = 0;    // C = alpha*acc (+bias) (+residual)
@@ -134,6 +138,13 @@ constexpr int EPI_SIMREG_BWD = 8;
 //   EPI_VCE_BWD  C = bf16(*gscale_dev * (exp(l - lse_row[row]) - [c == labels[row]])), zero in [N, ldc)
 constexpr int EPI_VCE_FWD = 9;
 constexpr int EPI_VCE_BWD = 10;
+// Pairwise sigmoid loss (SigLIP, nce.cu): logit l = alpha * acc + *logit_bias, label z = +1 on the
+// positive column r + diag_offset and -1 elsewhere; columns >= N take no part.
+//   EPI_SIG_FWD  nce_part[n_blk * M + row] = sum over the tile's columns of softplus(-z l)
+//   EPI_SIG_BWD  C = bf16(alpha * g), g = *gscale_dev * (sigmoid(l) - [positive]), zero in [N, ldc);
+//                *dtemp += sum g * alpha * acc and *dbias += sum g (each when non-null)
+constexpr int EPI_SIG_FWD = 11;
+constexpr int EPI_SIG_BWD = 12;
 
 constexpr int kGemmBlockM = 128;
 constexpr int kGemmBlockK = 64;
@@ -175,6 +186,38 @@ __device__ __forceinline__ float nce_ex2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
+}
+
+// ---- EPI_SIG_*: the pairwise sigmoid loss from u = exp(-|l|) of a logit l, without a division or
+// a log call.  u underflows to exactly 0 once |l| passes ~87 (ex2 flushes to zero), so a saturated
+// logit gives sigmoid 0 or 1 and softplus(l) = max(l, 0) exactly.
+__device__ __forceinline__ float sig_rcp(float x) {
+  float y;
+  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
+}
+__device__ __forceinline__ float sig_u(float l) { return nce_ex2(-fabsf(l) * 1.4426950408889634f); }
+// log1p(u) for u in [0, 1] as 2 atanh(s) = 2 (s + s^3/3 + ... + s^13/13), s = u / (2 + u) <= 1/3:
+// relative truncation error below 2e-8 at every u.  log2(1 + u) in fp32 would lose every u below
+// 2^-24 and most digits of u = 4.5e-5, the negative pairs' term at SigLIP's initial logit bias of -10.
+__device__ __forceinline__ float sig_log1p(float u) {
+  const float s = u * sig_rcp(2.f + u);
+  const float s2 = s * s;
+  float q = fmaf(s2, 1.f / 13.f, 1.f / 11.f);
+  q = fmaf(s2, q, 1.f / 9.f);
+  q = fmaf(s2, q, 1.f / 7.f);
+  q = fmaf(s2, q, 1.f / 5.f);
+  q = fmaf(s2, q, 1.f / 3.f);
+  const float ts = s + s;
+  return fmaf(ts * s2, q, ts);
+}
+// softplus(x) = max(x, 0) + log1p(exp(-|x|))
+__device__ __forceinline__ float sig_softplus(float x) { return fmaxf(x, 0.f) + sig_log1p(sig_u(x)); }
+// sigmoid(l) = 1 / (1 + u) for l >= 0, u / (1 + u) otherwise
+__device__ __forceinline__ float sig_sigmoid(float l) {
+  const float u = sig_u(l);
+  const float r = sig_rcp(1.f + u);
+  return l >= 0.f ? r : u * r;
 }
 
 // Staging tile: 128 rows of 128 fp32, unpadded.  The 16-byte chunk q of row r is stored at chunk
@@ -903,6 +946,82 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         for (int i = 0; i < 32; ++i) s4[i & 3] = fmaf(v[i], v[i], s4[i & 3]);
       }
       if (row_ok) p.nce_part[(long long)n_blk * p.M + row] = (s4[0] + s4[1]) + (s4[2] + s4[3]);
+    } else if constexpr (EPI == EPI_SIG_FWD) {
+      const float alpha = __ldg(p.alpha_dev);
+      const float lb = __ldg(p.logit_bias);
+      const int diag_col = row + p.diag_offset;
+      float s4[4] = {0.f, 0.f, 0.f, 0.f};          // four chains, as EPI_SIMREG_FWD
+#pragma unroll 1
+      for (int c = 0; c < BLOCK_N / 32; ++c) {
+        need(c * 32);
+        const int col0 = n_blk * BLOCK_N + c * 32;
+        if (col0 >= p.N) continue;
+        float v[32];
+        acc_ld32(acc_row, acc_sw, c * 32, v);
+        if (col0 + 32 <= p.N && (diag_col < col0 || diag_col >= col0 + 32)) {
+#pragma unroll
+          for (int i = 0; i < 32; ++i) s4[i & 3] += sig_softplus(fmaf(v[i], alpha, lb));   // z = -1
+        } else {
+#pragma unroll
+          for (int i = 0; i < 32; ++i) {
+            const int col = col0 + i;
+            const float l = fmaf(v[i], alpha, lb);
+            const float sp = sig_softplus(col == diag_col ? -l : l);
+            if (col < p.N) s4[i & 3] += sp;
+          }
+        }
+      }
+      if (row_ok) p.nce_part[(long long)n_blk * p.M + row] = (s4[0] + s4[1]) + (s4[2] + s4[3]);
+    } else if constexpr (EPI == EPI_SIG_BWD) {
+      const float alpha = __ldg(p.alpha_dev);
+      const float lb = __ldg(p.logit_bias);
+      const float gs = __ldg(p.gscale_dev);
+      const int diag_col = row + p.diag_offset;
+      float tsum = 0.f, bsum = 0.f;                // sum g * acc, sum g
+#pragma unroll 1
+      for (int c = 0; c < BLOCK_N / 32; ++c) {
+        need(c * 32);
+        const int col0 = n_blk * BLOCK_N + c * 32;
+        if (!row_ok || col0 >= (int)p.ldc) continue;   // pad columns [N, ldc) get zeros
+        float v[32];
+        acc_ld32(acc_row, acc_sw, c * 32, v);
+        if (col0 + 32 <= p.N && (diag_col < col0 || diag_col >= col0 + 32)) {
+#pragma unroll
+          for (int i = 0; i < 32; ++i) {
+            const float g = gs * sig_sigmoid(fmaf(v[i], alpha, lb));
+            tsum = fmaf(g, v[i], tsum);
+            bsum += g;
+            v[i] = g * alpha;
+          }
+        } else {
+#pragma unroll
+          for (int i = 0; i < 32; ++i) {
+            const int col = col0 + i;
+            // g = -z gs sigmoid(-z l): on the positive, sigmoid(l) - 1 = -sigmoid(-l) without the
+            // cancellation that leaves 0 for every l above ~17
+            const float l = fmaf(v[i], alpha, lb);
+            const bool is_pos = col == diag_col;
+            float g = gs * sig_sigmoid(is_pos ? -l : l);
+            if (is_pos) g = -g;
+            if (col >= p.N) g = 0.f;
+            tsum = fmaf(g, v[i], tsum);
+            bsum += g;
+            v[i] = g * alpha;   // the logit scale folded in: d rows = (alpha g) @ cols
+          }
+        }
+        bf16* grow = reinterpret_cast<bf16*>(p.c) + (long long)row * p.ldc + col0;
+#pragma unroll
+        for (int i = 0; i < 32; i += 8)
+          if (col0 + i < (int)p.ldc) st_bf16x8(grow + i, v + i);
+      }
+      if (p.dtemp != nullptr) {
+        tsum = warp_sum(tsum * alpha);
+        if (lane == 0) atomicAdd(p.dtemp, tsum);
+      }
+      if (p.dbias != nullptr) {
+        bsum = warp_sum(bsum);
+        if (lane == 0) atomicAdd(p.dbias, bsum);
+      }
     } else if constexpr (EPI == EPI_VCE_FWD) {
       // EPI_NCE_FWD's online (max, sum) per 32-column chunk, on l = acc + bias
       constexpr float kLog2e = 1.4426950408889634f;

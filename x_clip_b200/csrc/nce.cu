@@ -14,8 +14,9 @@
 // data parallelism each rank evaluates only its B_g/W row block (SURVEY.md 8e) instead of the
 // reference's redundant full matrix.
 //
-// The MLM head's cross-entropy over the vocabulary (xclip_vocab_ce_*, end of file) is the same
-// softmax with a bias, a label column as the positive and no temperature.
+// The pairwise sigmoid loss (xclip_sigmoid_*) runs on the same operands and row blocks with
+// epilogues of its own.  The MLM head's cross-entropy over the vocabulary (xclip_vocab_ce_*, end of
+// file) is the same softmax with a bias, a label column as the positive and no temperature.
 #include "gemm.cuh"
 #include "host.h"
 
@@ -148,6 +149,91 @@ extern "C" int xclip_nce_bwd(const void* a, const void* b, int R, int C, int D,
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   return block_n == 256 ? launch_nce<256, EPI_NCE_BWD>(tmA, tmB, p, grid, s)
                         : launch_nce<128, EPI_NCE_BWD>(tmA, tmB, p, grid, s);
+}
+
+// ---- pairwise sigmoid loss (SigLIP, Zhai et al. 2023) on the same operands, mainloop and row blocks:
+// logit l = exp(temperature) * <a_r, b_c> + logit_bias, label +1 on column r + diag_offset, -1 elsewhere.
+// No softmax over the batch: the forward sums softplus(-z l) per row, the backward recomputes the tiles
+// into g = gscale * (sigmoid(l) - [positive]).  Nothing R x C is written except the bf16 g.
+
+namespace xclip {
+
+// rowloss[r] = sum of the column-block partials of row r in a fixed order; *loss_accum += scale * sum
+__global__ void __launch_bounds__(1024)
+sigmoid_finalize_kernel(const float* __restrict__ part, int nblk, int rows, float* __restrict__ rowloss,
+                        float* __restrict__ loss_accum, float scale) {
+  __shared__ float red[32];
+  float local = 0.f;
+  for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < rows; r += gridDim.x * blockDim.x) {
+    float s = 0.f;
+    for (int k = 0; k < nblk; ++k) s += part[(long long)k * rows + r];
+    rowloss[r] = s;
+    local += s;
+  }
+  local = warp_sum(local);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = local;
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    float v = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : 0.f;
+    v = warp_sum(v);
+    if (threadIdx.x == 0 && loss_accum != nullptr) atomicAdd(loss_accum, v * scale);
+  }
+}
+
+static int sigmoid_check(int R, int C, const float* temp_exp, const float* logit_bias, int diag_offset,
+                         const char* what) {
+  XCLIP_REQUIRE(temp_exp && logit_bias, "%s: temp_exp / logit_bias device scalars required", what);
+  XCLIP_REQUIRE(diag_offset >= 0 && (long long)diag_offset + R <= C,
+                "%s: positives outside the columns (diag_offset=%d R=%d C=%d)", what, diag_offset, R, C);
+  return XCLIP_OK;
+}
+
+}  // namespace xclip
+
+extern "C" int xclip_sigmoid_fwd(const void* a, const void* b, int R, int C, int D, const float* temp_exp,
+                                 const float* logit_bias, int diag_offset, float* part_ws, float* rowloss,
+                                 float* loss_accum, float loss_scale, xclip_stream_t stream) {
+  GemmParams p;
+  CUtensorMap tmA, tmB;
+  int block_n = 0, grid = 0;
+  int rc = nce_common(a, b, R, C, D, &p, &tmA, &tmB, &block_n, &grid);
+  if (rc) return rc;
+  rc = sigmoid_check(R, C, temp_exp, logit_bias, diag_offset, "sigmoid_fwd");
+  if (rc) return rc;
+  XCLIP_REQUIRE(part_ws && rowloss, "sigmoid_fwd: null workspace/output");
+  XCLIP_REQUIRE((reinterpret_cast<uintptr_t>(part_ws) & 3) == 0, "sigmoid_fwd: misaligned part_ws");
+  p.alpha_dev = temp_exp; p.logit_bias = logit_bias; p.diag_offset = diag_offset;
+  p.nce_part = part_ws;
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  rc = block_n == 256 ? launch_nce<256, EPI_SIG_FWD>(tmA, tmB, p, grid, s)
+                      : launch_nce<128, EPI_SIG_FWD>(tmA, tmB, p, grid, s);
+  if (rc) return rc;
+  const int nblk = xclip_nce_num_col_blocks(C);
+  int fgrid = (R + 1023) / 1024;
+  if (fgrid > num_sms()) fgrid = num_sms();
+  sigmoid_finalize_kernel<<<fgrid, 1024, 0, s>>>(part_ws, nblk, R, rowloss, loss_accum, loss_scale);
+  XCLIP_LAUNCH_CHECK("sigmoid_finalize_kernel");
+  return XCLIP_OK;
+}
+
+extern "C" int xclip_sigmoid_bwd(const void* a, const void* b, int R, int C, int D, const float* temp_exp,
+                                 const float* logit_bias, int diag_offset, const float* gscale, void* g,
+                                 int64_t ldg, float* dtemp, float* dbias, xclip_stream_t stream) {
+  GemmParams p;
+  CUtensorMap tmA, tmB;
+  int block_n = 0, grid = 0;
+  int rc = nce_common(a, b, R, C, D, &p, &tmA, &tmB, &block_n, &grid);
+  if (rc) return rc;
+  rc = sigmoid_check(R, C, temp_exp, logit_bias, diag_offset, "sigmoid_bwd");
+  if (rc) return rc;
+  XCLIP_REQUIRE(g && ldg % 8 == 0 && ldg >= (C + 7) / 8 * 8, "sigmoid_bwd: g needs ld >= roundup8(C)");
+  XCLIP_REQUIRE((reinterpret_cast<uintptr_t>(g) & 15) == 0, "sigmoid_bwd: misaligned g");
+  XCLIP_REQUIRE(gscale, "sigmoid_bwd: gscale device scalar required");
+  p.alpha_dev = temp_exp; p.logit_bias = logit_bias; p.gscale_dev = gscale; p.diag_offset = diag_offset;
+  p.c = g; p.ldc = ldg; p.dtemp = dtemp; p.dbias = dbias;
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  return block_n == 256 ? launch_nce<256, EPI_SIG_BWD>(tmA, tmB, p, grid, s)
+                        : launch_nce<128, EPI_SIG_BWD>(tmA, tmB, p, grid, s);
 }
 
 // ---- vocabulary cross-entropy: the MLM head's F.cross_entropy(x W^T + b, labels) on the same

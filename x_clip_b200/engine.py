@@ -8,7 +8,8 @@ cast to bf16 once per step.
 
 Reference call sites: Transformer.forward x_clip/x_clip.py:274-291 (TransformerFn),
 nn.Linear :358,:368 (LinearFn), :713-724 (ProjectL2NormFn), :759-769 + :797-847
-(ContrastiveLossFn, with x_clip/distributed.py:41-56 for the gather contract).
+(ContrastiveLossFn, with x_clip/distributed.py:41-56 for the gather contract).  SigmoidLossFn is
+SigLIP's pairwise sigmoid loss (not in the reference) on the same operands and gather contract.
 """
 from __future__ import annotations
 
@@ -598,6 +599,62 @@ class ContrastiveLossFn(torch.autograd.Function):
         return grads + (None,) * (len(ctx.needs_input_grad) - len(grads))
 
 
+class SigmoidLossFn(torch.autograd.Function):
+    """The pairwise sigmoid loss of SigLIP (Zhai et al., ICCV 2023) over all pairs of the GLOBAL batch:
+
+        l_ij = exp(temperature) <t_i, v_j> + logit_bias,   z_ij = +1 if i == j else -1
+        L = (1/B) sum_ij softplus(-z_ij l_ij)
+
+    Inputs as ContrastiveLossFn without the extra pair: local unit latents zt, zi [b, D] (fp32, carry the
+    graph), the temperature and logit_bias parameters (scalars) and `ops`, the (zrow, zcol) split-bf16
+    operands of texts and images.  The forward runs one row block, the local texts against all
+    (gathered) images at diag_offset = rank * b; the per-row losses ride in one statistics gather, so every
+    rank returns the same global loss.  Backward: the texts x images block gives d zt and the images x
+    texts block d zi, each through the plain dgrad GEMM; d temperature and d logit_bias come from the
+    first block and are all-reduced, so every rank holds their full-batch gradients (the contract of
+    d temperature in ContrastiveLossFn)."""
+
+    @staticmethod
+    def forward(ctx, zt, zi, temperature, logit_bias, ops, use_gather: bool):
+        rank, world = D_.world() if use_gather else (0, 1)
+        b = ops[0][0].shape[0]
+        D = ops[0][0].shape[1] // 3
+        temp_exp = temperature.detach().float().exp().reshape(1)
+        bias = logit_bias.detach().float().reshape(1).contiguous()
+        rows = [o[0] for o in ops]
+        cols = D_.gather_rows([o[1] for o in ops]) if world > 1 else [o[1] for o in ops]
+        Bg = world * b
+        off = rank * b
+        rowloss = K.sigmoid_fwd(rows[0], cols[1], temp_exp, bias, off)
+        stats = D_.gather_stats(rowloss[None]) if world > 1 else rowloss[None]
+        ctx.cfg = (world, D, Bg, off)
+        ctx.scalars = (temp_exp, bias)
+        ctx.rows, ctx.cols = rows, cols
+        return stats.sum() / Bg
+
+    @staticmethod
+    def backward(ctx, gloss):
+        world, D, Bg, off = ctx.cfg
+        temp_exp, bias = ctx.scalars
+        rows, cols = ctx.rows, ctx.cols
+        gscale = (gloss.detach().float() / Bg).reshape(1)
+        dscalars = torch.zeros(2, device=gloss.device, dtype=F32)     # d temperature, d logit_bias
+
+        def latent_grad(r, c, want_scalars):
+            g = K.sigmoid_bwd(rows[r], cols[c], temp_exp, bias, off, gscale,
+                              dscalars[0:1] if want_scalars else None, dscalars[1:2] if want_scalars else None)
+            # d rows = (temp * g) @ cols_hi ; g is zero-padded to a multiple of 8 columns
+            return K.gemm(g, _pad_rows(cols[c][:, :D], g.shape[1]), b_major=1, out_dtype=F32)
+
+        dzt = latent_grad(0, 1, True)
+        dzi = latent_grad(1, 0, False)
+        if world > 1:
+            D_.all_reduce_sum_(dscalars)
+        ctx.rows = ctx.cols = None
+        # two tensors of their own: .grad buffers must not share storage
+        return dzt, dzi, dscalars[0].clone(), dscalars[1].clone(), None, None
+
+
 # bytes of one backward window of the vocabulary cross-entropy's g [rows, roundup8(V)] bf16: at the
 # CLIP BPE vocabulary (V = 49408) that is 10752 rows, against 2.4 G logits for 49 k selected rows
 VOCAB_CE_WINDOW_BYTES = 1 << 30
@@ -781,7 +838,9 @@ class ChunkedClipLossFn(torch.autograd.Function):
       1. encode every chunk -> latents of the whole local batch
       2. one contrastive loss over ALL latents (with the usual cross-rank all-gather); with
          `use_all_token_embeds` the FILIP loss (filip.FilipLossFn) over all token latents, which
-         works in row chunks of its own and is left `filip.step_reserve_bytes` of HBM by the plan
+         works in row chunks of its own and is left `filip.step_reserve_bytes` of HBM by the plan;
+         with `logit_bias` given (CLIP(sigmoid_loss=True)) the sigmoid loss, SigmoidLossFn, with
+         logit_bias as one more leaf beside the temperature
       3. in backward: d loss / d latents, then back-propagate the matching slice of the latent
          gradient through every chunk's encoders.
     Memory plan: a chunk's saved activations are KEPT from step 1 for as many chunks as
@@ -803,7 +862,7 @@ class ChunkedClipLossFn(torch.autograd.Function):
     re-encodes a chunk with all of its gradient passes."""
 
     @staticmethod
-    def forward(ctx, clip, text, image, text_mask, chunk, temperature, retain="auto", aux=None):
+    def forward(ctx, clip, text, image, text_mask, chunk, temperature, retain="auto", aux=None, logit_bias=None):
         B = text.shape[0]
         dev = text.device
         bounds = [(s, min(s + chunk, B)) for s in range(0, B, chunk)]
@@ -901,6 +960,7 @@ class ChunkedClipLossFn(torch.autograd.Function):
                         for j in range(nsets))
         del zs, opss
         temp_leaf = temperature.detach().requires_grad_(True)
+        bias_leaf = None if logit_bias is None else logit_bias.detach().requires_grad_(True)
         cl_w = 1.0
         if aux is not None:
             cl_w = 1 - (clip.text_ssl_loss_weight + clip.image_ssl_loss_weight)
@@ -912,6 +972,9 @@ class ChunkedClipLossFn(torch.autograd.Function):
                     leaves[0], leaves[1], leaves[2] if nsets == 4 else None,
                     leaves[3] if nsets == 4 else None, temp_leaf, ops_all, text_mask.contiguous(),
                     clip.decoupled_contrastive_learning, clip.requires_all_gather, filip_stats)
+            elif bias_leaf is not None:
+                loss = SigmoidLossFn.apply(leaves[0], leaves[1], temp_leaf, bias_leaf, ops_all,
+                                           clip.requires_all_gather)
             else:
                 loss = ContrastiveLossFn.apply(
                     leaves[0], leaves[1], leaves[2] if nsets == 4 else None,
@@ -931,7 +994,7 @@ class ChunkedClipLossFn(torch.autograd.Function):
         ctx.bounds, ctx.rng_states, ctx.kept = bounds, rng_states, kept
         ctx.aux, ctx.row_bounds = aux, row_bounds
         ctx.img_leaves = img_leaves if want_dimage else None
-        ctx.graph = (loss, leaves, temp_leaf)
+        ctx.graph = (loss, leaves, temp_leaf, bias_leaf)
         ctx.weight_casts = wscope.cache
         n_kept = sum(z is not None for z in kept)
         if planned or (oom_fallbacks and plan_key in plans):
@@ -951,7 +1014,7 @@ class ChunkedClipLossFn(torch.autograd.Function):
     def backward(ctx, g):
         clip = ctx.clip
         text, image, text_mask = ctx.inputs
-        loss, leaves, temp_leaf = ctx.graph
+        loss, leaves, temp_leaf, bias_leaf = ctx.graph
         with torch.enable_grad():
             torch.autograd.backward(loss, g)
         dz = [l.grad for l in leaves]
@@ -994,4 +1057,6 @@ class ChunkedClipLossFn(torch.autograd.Function):
                         del img_k
         torch.cuda.set_rng_state(keep_state, dev)
         ctx.graph = ctx.inputs = ctx.kept = ctx.weight_casts = ctx.img_leaves = ctx.aux = None
-        return None, None, dimage, None, None, temp_leaf.grad, None, None
+        grads = (None, None, dimage, None, None, temp_leaf.grad, None, None,
+                 None if bias_leaf is None else bias_leaf.grad)
+        return grads[:len(ctx.needs_input_grad)]

@@ -477,6 +477,35 @@ def nce_bwd(a, b, temp_exp, diag_offset, dcl, lse_row, lse_col, w_row, w_col, w_
     return g
 
 
+def sigmoid_fwd(a, b, temp_exp, logit_bias, diag_offset, loss_accum=None, loss_scale=0.0):
+    """Row-block sigmoid-loss forward: rowloss [R] = sum_c softplus(-z l) for rows a vs all columns b.
+    temp_exp, logit_bias: fp32 DEVICE scalar tensors (exp(temperature) and the bias)."""
+    _need(a, BF16, "a"); _need(b, BF16, "b"); _need(temp_exp, F32, "temp_exp"); _need(logit_bias, F32, "logit_bias")
+    R, D = a.shape
+    C = b.shape[0]
+    nblk = _lib.load().xclip_nce_num_col_blocks(C)
+    part = torch.empty((nblk, R), device=a.device, dtype=F32)
+    rowloss = torch.empty((R,), device=a.device, dtype=F32)
+    _call(a, "sigmoid_fwd", 2.0 * R * C * D, 2.0 * (R + C) * D + 4.0 * R, "xclip_sigmoid_fwd", a.data_ptr(),
+          b.data_ptr(), R, C, D, temp_exp.data_ptr(), logit_bias.data_ptr(), int(diag_offset), part.data_ptr(),
+          rowloss.data_ptr(), _ptr(loss_accum), float(loss_scale))
+    return rowloss
+
+
+def sigmoid_bwd(a, b, temp_exp, logit_bias, diag_offset, gscale, dtemp=None, dbias=None):
+    """bf16 temp*g [R, roundup8(C)] (columns >= C are zero); see xclip_sigmoid_bwd."""
+    _need(a, BF16, "a"); _need(b, BF16, "b"); _need(temp_exp, F32, "temp_exp"); _need(logit_bias, F32, "logit_bias")
+    _need(gscale, F32, "gscale")
+    R, D = a.shape
+    C = b.shape[0]
+    ldg = (C + 7) // 8 * 8
+    g = torch.empty((R, ldg), device=a.device, dtype=BF16)
+    _call(a, "sigmoid_bwd", 2.0 * R * C * D, 2.0 * (R + C) * D + 2.0 * R * C, "xclip_sigmoid_bwd", a.data_ptr(),
+          b.data_ptr(), R, C, D, temp_exp.data_ptr(), logit_bias.data_ptr(), int(diag_offset), gscale.data_ptr(),
+          g.data_ptr(), ldg, _ptr(dtemp), _ptr(dbias))
+    return g
+
+
 def _vocab_ce_args(x, w, bias, labels):
     _need(x, BF16, "x"); _need(w, BF16, "w"); _rows2d(x, "x")
     if not w.is_contiguous() or w.dim() != 2 or w.shape[1] != x.shape[1]:
