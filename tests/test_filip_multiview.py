@@ -1,7 +1,7 @@
 """FILIP with augmented views on the CPU: the fp64 restatement (tests/filip_multiview_oracle.py) against
 the reference's goldens (tests/golden/filip_mv_*.json, make_golden_filip_multiview.py), the view-block
 layout and positive columns in both column orders, the block weights, the multiview chunk plan and
-saved-argmax arithmetic, and CLIP.forward's routing of a FILIP call with views."""
+saved-argmax arithmetic.  CLIP.forward's routing of a FILIP call with views is in test_loss_head.py."""
 import json
 from pathlib import Path
 
@@ -143,52 +143,11 @@ def test_multiview_passes_plan_like_the_single_view_ones(monkeypatch, m, n):
     assert pa2.plan(0) == 0 and pa2.saved is None
 
 
-# --------------------------------------------------------------------------- routing
+# --------------------------------------------------------------------------- refusals
 
 TINY = dict(dim_text=256, dim_image=256, dim_latent=256, num_text_tokens=128, text_enc_depth=1,
             text_seq_len=16, text_heads=4, visual_enc_depth=1, visual_heads=4, visual_image_size=64,
             visual_patch_size=16, visual_patch_dropout=0.0, use_all_token_embeds=True)
-
-
-class _Enc(torch.nn.Module):
-    """A pluggable tower: [b, ...] -> [b, 1 + tokens, dim] that depends on the input."""
-
-    def __init__(self, tokens, dim):
-        super().__init__()
-        self.tokens, self.dim = tokens, dim
-
-    def forward(self, x, mask=None):
-        seed = x.reshape(x.shape[0], -1).float().sum(dim=1)
-        return seed[:, None, None] + torch.zeros(x.shape[0], 1 + self.tokens, self.dim)
-
-
-@pytest.mark.parametrize("m,n", [(1, 2), (2, 1), (3, 2)])
-def test_filip_with_views_takes_the_multiview_loss(monkeypatch, m, n):
-    """No refusal any more: the m text views and n image views reach the FILIP loss stacked along the
-    batch with per-view text masks, and the weights of x_clip.py:855-868."""
-    import x_clip_b200.clip as C
-    real = C._require
-    monkeypatch.setattr(C, "_require", lambda cond, msg: None if "CUDA" in msg else real(cond, msg))
-    monkeypatch.setattr(C.CLIP, "_project", lambda self, e, lin: (e.float(), (None, None)))
-    seen = {}
-
-    def fake_loss(clip, zt, zi, zt_x, zi_x, ops, text_mask, views=(1, 1), weights=None, **kw):
-        seen.update(zt=zt, zi=zi, mask=text_mask, views=views, weights=weights)
-        return torch.zeros(())
-
-    monkeypatch.setattr(F, "filip_loss", fake_loss)
-    clip = x_clip_b200.CLIP(**TINY, text_encoder=_Enc(16, 256), image_encoder=_Enc(16, 256))
-    clip.train()
-    b = 3
-    text = torch.randint(1, 128, (b, 16))
-    image = torch.randn(b, 3, 64, 64)
-    aug_t = [text.clone().masked_fill(torch.rand(b, 16) < 0.5, 0) for _ in range(m - 1)]
-    aug_i = [torch.randn(b, 3, 64, 64) for _ in range(n - 1)]
-    clip(text, image, return_loss=True, aug_text=tuple(aug_t) or None, aug_image=tuple(aug_i) or None)
-    assert seen["views"] == (m, n)
-    assert seen["weights"] == pytest.approx((0.9, 0.1))
-    assert seen["zt"].shape[0] == m * b and seen["zi"].shape[0] == n * b
-    assert torch.equal(seen["mask"], torch.cat([text] + aug_t) != 0)
 
 
 def test_filip_simreg_with_views_still_raises():

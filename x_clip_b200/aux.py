@@ -79,12 +79,16 @@ class MLM(nn.Module):
     def loss_from(self, masked_seq: torch.Tensor, labels: torch.Tensor, **kwargs) -> torch.Tensor:
         enc = self.transformer(masked_seq, **kwargs)[:, 1:]                  # drop CLS (mlm.py:98-99)
         sel = labels != self.pad_token_id                                     # ignore_index rows
-        rows = enc[sel]                                                       # [n_sel, dim] bf16
+        return self.loss_from_rows(enc[sel], labels[sel])
+
+    def loss_from_rows(self, rows: torch.Tensor, labels: torch.Tensor) -> torch.Tensor:
+        """The head on the encodings of the selected positions, rows [n_sel, dim], against their tokens:
+        the mean over the selected positions == F.cross_entropy(..., ignore_index=pad) of the reference,
+        fused into the vocabulary GEMM for any vocabulary size (no [n_sel, V] logits are written).  No
+        selected position gives 0, still connected to the encoder."""
         if rows.shape[0] == 0:
-            return enc.sum() * 0.
-        # mean over the selected positions == F.cross_entropy(..., ignore_index=pad) of the reference,
-        # fused into the vocabulary GEMM for any vocabulary size: no [n_sel, V] logits are written
-        return E.VocabCrossEntropyFn.apply(rows, self.to_logits.weight, self.to_logits.bias, labels[sel])
+            return rows.sum() * 0.
+        return E.VocabCrossEntropyFn.apply(rows, self.to_logits.weight, self.to_logits.bias, labels)
 
     def forward(self, seq: torch.Tensor, **kwargs) -> torch.Tensor:
         masked, labels = self.corrupt(seq)

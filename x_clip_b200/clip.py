@@ -43,6 +43,7 @@ import torch.distributed as dist
 from torch import nn
 
 from . import engine as E
+from .filip import FilipLossFn
 
 BF16 = torch.bfloat16
 
@@ -478,15 +479,20 @@ class CLIP(nn.Module):
         order = torch.cat((first, rest), dim=1)
         return torch.gather(enc_text, 1, order[:, :, None].expand(-1, -1, d))
 
-    def _encode_to_latents(self, text, image, text_mask):
-        """encoders -> CLS select (FILIP: every token but the CLS) -> projections.
-        Returns ([zt, zi(, zt_x, zi_x)], ops): latents [b, D], or [b, tokens, D] in FILIP mode."""
+    def _encodings(self, text, image, text_mask, freeze_text=False, freeze_image=False):
+        """(text encodings, image encodings) of both towers, a frozen tower without gradient."""
         text_args = (text,) if self.text_encode_without_mask else (text, text_mask)
-        enc_text = self.text_transformer(*text_args)
+        enc_text = _encode(self.text_transformer, text_args, freeze_text)
         if self.text_causal_mask:
             enc_text = self._eos_to_front(enc_text, text)
-        enc_image = self.visual_transformer(image)
+        return enc_text, _encode(self.visual_transformer, (image,), freeze_image)
+
+    def _latents(self, enc_text, enc_image):
+        """CLS select (FILIP: every token but the CLS) -> projections.
+        Returns ([zt, zi(, zt_x, zi_x)], ops): latents [b, D], or [b, tokens, D] in FILIP mode."""
         if self.use_all_token_embeds:
+            assert enc_text.ndim == 3, 'encoded text must have 3 dimensions (batch, seq, features)'
+            assert enc_image.ndim == 3, 'encoded image must have 3 dimensions (batch, seq [height x width], features)'
             te = enc_text[:, 1:] if self.text_has_cls_token else enc_text
             ie = enc_image[:, 1:] if self.visual_has_cls_token else enc_image
         else:
@@ -501,6 +507,10 @@ class CLIP(nn.Module):
             zs += [zt_x, zi_x]
             ops += [ops_tx, ops_ix]
         return zs, ops
+
+    def _encode_to_latents(self, text, image, text_mask):
+        """encoders -> latents (_latents)."""
+        return self._latents(*self._encodings(text, image, text_mask))
 
     def _chunkable_ssl(self) -> bool:
         """visual SSL the micro-batched step can split into encoder passes and a head"""
@@ -534,6 +544,64 @@ class CLIP(nn.Module):
             e = e.to(BF16)
         z, zrow, zcol = E.ProjectL2NormFn.apply(e, linear.weight)
         return z.view(*lead, -1), (zrow, zcol)
+
+    def _loss(self, zs, ops, text_mask, temperature, logit_bias=None, views=(1, 1), mlm=None, ssl=None,
+              filip_stats=None):
+        """The training loss of the single pass and of the micro-batched step (engine.ChunkedClipLossFn).
+
+        zs / ops: _latents' outputs for m text views and n image views (views = (m, n)) of the same b pairs,
+        stacked along the batch; text_mask [m b, n_text].  The FILIP, sigmoid or InfoNCE / DCL loss (with
+        the similarity regularisation), weighted as the reference does (x_clip.py:851-873):
+        cl_w * L[0, 0] + w_text * mlm + w_image * ssl + w_multiview * mean(the other view pairs), where
+        cl_w = 1 - (w_text + w_image + w_multiview).  Without any auxiliary term the loss is returned
+        unweighted.  `mlm` / `ssl`: the auxiliary losses, or None when off; `filip_stats` receives
+        FilipLossFn's plan."""
+        m, n = views
+        multiview = m * n > 1
+        has_aux = multiview or self.use_mlm or self.use_visual_ssl
+        mv_w = self.multiview_loss_weight if multiview else 0
+        cl_w = 1 - (self.text_ssl_loss_weight + self.image_ssl_loss_weight + mv_w)
+        extra = self.extra_latent_projection
+        dcl, gather = self.decoupled_contrastive_learning, self.requires_all_gather
+        others = ()
+        if self.use_all_token_embeds:
+            # every (text view, image view) pair in one pair of segment-max passes, the view pairs
+            # weighted inside the loss
+            loss = FilipLossFn.apply(zs[0], zs[1], *(zs[2:] if extra else (None, None)), temperature,
+                                     tuple(ops), text_mask.contiguous(), dcl, gather, filip_stats, views,
+                                     (cl_w, mv_w))
+            weighted = multiview
+        else:
+            b = zs[0].shape[0] // m
+
+            def pick(k, t, i, j):
+                """text view i (zs / ops 0 and 2) or image view j (1 and 3) of t: t itself for one view"""
+                v, count = (i, m) if k % 2 == 0 else (j, n)
+                return t if count == 1 else t[v * b:(v + 1) * b]
+
+            def pair(i, j):
+                """the loss of text view i against image view j"""
+                z = [pick(k, t, i, j) for k, t in enumerate(zs)]
+                o = tuple((pick(k, r, i, j), pick(k, c, i, j)) for k, (r, c) in enumerate(ops))
+                if self.sigmoid_loss:
+                    return E.SigmoidLossFn.apply(z[0], z[1], temperature, logit_bias, o, gather)
+                # the similarity regularisation (single view: refused with views) weighs the
+                # contrastive term itself: cl_w * contrastive + w * L_sim
+                sim_reg = (self.sim_reg_loss_weight, cl_w if has_aux else 1.0) if self.has_sim_reg_loss else ()
+                return E.ContrastiveLossFn.apply(z[0], z[1], *(z[2:] if extra else (None, None)), temperature,
+                                                 o, dcl, gather, *sim_reg)
+
+            loss, *others = [pair(i, j) for i in range(m) for j in range(n)]
+            weighted = self.has_sim_reg_loss
+        if has_aux and not weighted:
+            loss = loss * cl_w
+        if mlm is not None:
+            loss = loss + mlm * self.text_ssl_loss_weight
+        if ssl is not None:
+            loss = loss + ssl * self.image_ssl_loss_weight
+        if others:
+            loss = loss + torch.stack(others).mean() * mv_w
+        return loss
 
     def forward(
         self,
@@ -570,10 +638,10 @@ class CLIP(nn.Module):
                                              *((self.logit_bias,) if self.sigmoid_loss else ()))
 
         # auxiliary losses on the un-augmented batch (reference :616-621)
-        text_ssl_loss = image_ssl_loss = 0
+        mlm = ssl = None
         if return_loss:
-            text_ssl_loss = self.mlm(text, mask=text_mask) if self.use_mlm else 0
-            image_ssl_loss = self.visual_ssl(image) if self.use_visual_ssl else 0
+            mlm = self.mlm(text, mask=text_mask) if self.use_mlm else None
+            ssl = self.visual_ssl(image) if self.use_visual_ssl else None
 
         # multiview: augmented texts / images are further "views" of the same pairs (:625-650)
         num_batch_texts = num_batch_images = 1
@@ -594,103 +662,22 @@ class CLIP(nn.Module):
         assert not (self.multiview_loss_weight == 0 and is_multiview), \
             'multiview loss weight cannot be 0 if augmented text or images passed in'
 
-        has_aux = is_multiview or self.use_mlm or self.use_visual_ssl
-        text_args = (text,) if self.text_encode_without_mask else (text, text_mask)
-        enc_text = _encode(self.text_transformer, text_args, freeze_text_encoder)
-        if self.text_causal_mask:
-            enc_text = self._eos_to_front(enc_text, text)
-        enc_image = _encode(self.visual_transformer, (image,), freeze_image_encoder)
-
+        enc_text, enc_image = self._encodings(text, image, text_mask, freeze_text_encoder, freeze_image_encoder)
         if return_encodings:
             return enc_text.float(), enc_image.float()
 
-        if self.use_all_token_embeds:
-            assert enc_text.ndim == 3, 'encoded text must have 3 dimensions (batch, seq, features)'
-            assert enc_image.ndim == 3, 'encoded image must have 3 dimensions (batch, seq [height x width], features)'
-            text_embeds = enc_text[:, 1:] if self.text_has_cls_token else enc_text
-            image_embeds = enc_image[:, 1:] if self.visual_has_cls_token else enc_image
-        else:
-            text_embeds = enc_text[:, 0] if enc_text.ndim == 3 else enc_text
-            image_embeds = enc_image[:, 0] if enc_image.ndim == 3 else enc_image
-
-        zt, ops_t = self._project(text_embeds, self.to_text_latent)
-        zi, ops_i = self._project(image_embeds, self.to_visual_latent)
-        zt_x, zi_x = zt, zi
-        ops = [ops_t, ops_i]
-        if self.extra_latent_projection:
-            zt_x, ops_tx = self._project(text_embeds, self.to_text_latent_extra)
-            zi_x, ops_ix = self._project(image_embeds, self.to_visual_latent_extra)
-            ops += [ops_tx, ops_ix]
-
+        zs, ops = self._latents(enc_text, enc_image)
         if return_latents:
-            if self.extra_latent_projection:
-                return zt, zi, zt_x, zi_x
-            return zt, zi
+            return tuple(zs)
 
         if not return_loss:
             # exp(temperature) * similarity, as the reference returns; with sigmoid_loss the logit_bias
             # is not added (add clip.logit_bias for the logits the sigmoid loss sees)
             temp = self.temperature.exp()
-            a, b = (zt_x, zi_x) if (self.extra_latent_projection and not text_to_image) else (zt, zi)
+            a, b = zs[2:] if (self.extra_latent_projection and not text_to_image) else zs[:2]
             if self.use_all_token_embeds:
                 return torch.einsum('btd,bid->bti', a, b) * temp      # per-pair token sims (:740-742)
             return (a * b).sum(dim=-1) * temp                          # per-pair similarity (:744-746)
 
-        if self.use_all_token_embeds:
-            from .filip import filip_loss
-            if is_multiview:
-                # every (text view, image view) pair in one pair of segment-max passes, each pair's
-                # InfoNCE weighted inside the loss: cl_w * L[0, 0] + mv_w * mean(the others) (:851-868)
-                cl_w = 1 - (self.text_ssl_loss_weight + self.image_ssl_loss_weight + self.multiview_loss_weight)
-                loss = filip_loss(self, zt, zi, zt_x, zi_x, ops, text_mask, views=(num_batch_texts, num_batch_images),
-                                  weights=(cl_w, self.multiview_loss_weight))
-                return loss + text_ssl_loss * self.text_ssl_loss_weight \
-                    + image_ssl_loss * self.image_ssl_loss_weight
-            loss = filip_loss(self, zt, zi, zt_x, zi_x, ops, text_mask)
-            if not has_aux:
-                return loss
-            # weighted with the auxiliary terms as the reference does (:851-865)
-            cl_w = 1 - (self.text_ssl_loss_weight + self.image_ssl_loss_weight)
-            return loss * cl_w + text_ssl_loss * self.text_ssl_loss_weight \
-                + image_ssl_loss * self.image_ssl_loss_weight
-
-        def cl(tsl, isl, *sim_reg):
-            """contrastive loss of text view rows `tsl` against image view rows `isl`; sim_reg =
-            (weight, contrastive weight) adds the similarity regularisation (ContrastiveLossFn)"""
-            o = [(ops[0][0][tsl], ops[0][1][tsl]), (ops[1][0][isl], ops[1][1][isl])]
-            if self.sigmoid_loss:
-                return E.SigmoidLossFn.apply(zt[tsl], zi[isl], self.temperature, self.logit_bias, tuple(o),
-                                             self.requires_all_gather)
-            if self.extra_latent_projection:
-                o += [(ops[2][0][tsl], ops[2][1][tsl]), (ops[3][0][isl], ops[3][1][isl])]
-            return E.ContrastiveLossFn.apply(
-                zt[tsl], zi[isl], zt_x[tsl] if self.extra_latent_projection else None,
-                zi_x[isl] if self.extra_latent_projection else None, self.temperature,
-                tuple(o), self.decoupled_contrastive_learning, self.requires_all_gather, *sim_reg)
-
-        if not has_aux:
-            if self.has_sim_reg_loss:
-                return cl(slice(None), slice(None), self.sim_reg_loss_weight, 1.0)
-            return cl(slice(None), slice(None))
-
-        if self.has_sim_reg_loss:
-            # single view (multiview was refused above): cl_w * contrastive + w * L_sim in one call,
-            # the auxiliary terms added as in the reference (:860-873)
-            cl_w = 1 - (self.text_ssl_loss_weight + self.image_ssl_loss_weight)
-            loss = cl(slice(None), slice(None), self.sim_reg_loss_weight, cl_w)
-            return loss + text_ssl_loss * self.text_ssl_loss_weight \
-                + image_ssl_loss * self.image_ssl_loss_weight
-
-        # every (text view m, image view n) pair is its own InfoNCE problem; [0] is the main loss,
-        # the others are averaged into the multiview term (reference :750-755, :851-868)
-        b = text.shape[0] // num_batch_texts
-        losses = [cl(slice(m * b, (m + 1) * b), slice(n * b, (n + 1) * b))
-                  for m in range(num_batch_texts) for n in range(num_batch_images)]
-        cl_loss = losses[0]
-        multiview_w = self.multiview_loss_weight if is_multiview else 0
-        cl_w = 1 - (self.text_ssl_loss_weight + self.image_ssl_loss_weight + multiview_w)
-        loss = cl_loss * cl_w + text_ssl_loss * self.text_ssl_loss_weight \
-            + image_ssl_loss * self.image_ssl_loss_weight
-        if is_multiview:
-            loss = loss + torch.stack(losses[1:]).mean() * multiview_w
-        return loss
+        return self._loss(zs, ops, text_mask, self.temperature, self.logit_bias if self.sigmoid_loss else None,
+                          views=(num_batch_texts, num_batch_images), mlm=mlm, ssl=ssl)

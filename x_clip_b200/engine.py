@@ -487,6 +487,28 @@ class ProjectL2NormFn(torch.autograd.Function):
         return de, dw
 
 
+def _cls_loss_operands(ops, temperature, use_gather: bool):
+    """What both CLS loss Functions start from: (rows, cols, temp_exp, world, Bg, off).  rows: the local
+    row operands of every latent set, [b, 3D] [hi|lo|hi]; cols: the column operands of every rank, one
+    all-gather when use_gather and W > 1; Bg = W b the global batch and off = rank * b this rank's first
+    global row; temp_exp = exp(temperature) as an fp32 [1] tensor."""
+    rank, world = D_.world() if use_gather else (0, 1)
+    b = ops[0][0].shape[0]
+    temp_exp = temperature.detach().float().exp().reshape(1)
+    rows = [o[0] for o in ops]
+    cols = D_.gather_rows([o[1] for o in ops]) if world > 1 else [o[1] for o in ops]
+    return rows, cols, temp_exp, world, world * b, rank * b
+
+
+def _latent_dgrad(g, cols, out=None, alpha: float = 1.0):
+    """d rows = g @ hi(cols) in fp32 for the gradient g [rows, roundup8(C)] of a row block of the logits
+    (zero beyond column C) and the column operand cols [C, 3D]; with `out`, out += alpha * that."""
+    hi = _pad_rows(cols[:, :cols.shape[1] // 3], g.shape[1])
+    if out is None:
+        return K.gemm(g, hi, b_major=1, out_dtype=F32)
+    return K.gemm(g, hi, b_major=1, out=out, alpha=alpha, accumulate=True)
+
+
 class ContrastiveLossFn(torch.autograd.Function):
     """InfoNCE / DCL over all pairs of the GLOBAL batch (x_clip.py:759-769, :813-847).
 
@@ -513,15 +535,7 @@ class ContrastiveLossFn(torch.autograd.Function):
         sim_w = float(sim_reg_weight)
         if sim_w != 0.0 and not extra:
             raise ValueError("the similarity regularisation needs the extra latent pair")
-        rank, world = D_.world() if use_gather else (0, 1)
-        b = ops[0][0].shape[0]
-        D = ops[0][0].shape[1] // 3
-        temp_exp = temperature.detach().float().exp().reshape(1)
-
-        rows = [o[0] for o in ops]                                  # local [b, 3D], [hi|lo|hi]
-        cols = D_.gather_rows([o[1] for o in ops]) if world > 1 else [o[1] for o in ops]
-        Bg = world * b
-        off = rank * b
+        rows, cols, temp_exp, world, Bg, off = _cls_loss_operands(ops, temperature, use_gather)
 
         # forward row blocks: texts vs all images; images vs all texts (extra latents if any)
         T, I, TX, IX = 0, 1, 2, 3
@@ -547,7 +561,7 @@ class ContrastiveLossFn(torch.autograd.Function):
         elif cl_weight != 1.0:
             loss = cl_weight * loss
 
-        ctx.cfg = (dcl, extra, rank, world, b, D, Bg, off)
+        ctx.cfg = (dcl, extra, world, Bg, off)
         ctx.sim = (sim_w, float(cl_weight), sim_ops)
         ctx.temp_exp = temp_exp
         ctx.rows, ctx.cols = rows, cols
@@ -558,7 +572,7 @@ class ContrastiveLossFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, gloss):
-        dcl, extra, rank, world, b, D, Bg, off = ctx.cfg
+        dcl, extra, world, Bg, off = ctx.cfg
         temp_exp = ctx.temp_exp
         rows, cols = ctx.rows, ctx.cols
         lse_t, lse_i, lse_t_all, lse_i_all = ctx.lse
@@ -571,8 +585,7 @@ class ContrastiveLossFn(torch.autograd.Function):
         def latent_grad(r, c, lse_row, lse_col, w_row, w_col, w_diag, want_dtemp):
             g = K.nce_bwd(rows[r], cols[c], temp_exp, off, dcl, lse_row, lse_col, w_row, w_col,
                           w_diag, gscale, dtemp if want_dtemp else None)
-            # d rows = (temp * g) @ cols_hi ; g is zero-padded to a multiple of 8 columns
-            return K.gemm(g, _pad_rows(cols[c][:, :D], g.shape[1]), b_major=1, out_dtype=F32)
+            return _latent_dgrad(g, cols[c])
 
         if not extra:
             dzt = latent_grad(T, I, lse_t, lse_i_all, 1.0, 1.0, 2.0, True)
@@ -588,9 +601,8 @@ class ContrastiveLossFn(torch.autograd.Function):
             sgs = (gloss.detach().float() * (2.0 * sim_w / (Bg * (Bg - 1.0)))).reshape(1)
             for (a, c), t, v, dt_, dv_ in zip(sim_ops, (T, TX), (I, IX), (dzt, dzt_x), (dzi, dzi_x)):
                 g = K.simreg_bwd(a, c, off, sgs)
-                K.gemm(g, _pad_rows(cols[t][:, :D], g.shape[1]), b_major=1, out=dt_, accumulate=True)
-                K.gemm(g, _pad_rows(cols[v][:, :D], g.shape[1]), b_major=1, out=dv_, alpha=-1.0,
-                       accumulate=True)
+                _latent_dgrad(g, cols[t], out=dt_)
+                _latent_dgrad(g, cols[v], out=dv_, alpha=-1.0)
                 del g
         if world > 1:
             D_.all_reduce_sum_(dtemp)       # every rank holds the full-batch d loss / d temperature
@@ -616,25 +628,18 @@ class SigmoidLossFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, zt, zi, temperature, logit_bias, ops, use_gather: bool):
-        rank, world = D_.world() if use_gather else (0, 1)
-        b = ops[0][0].shape[0]
-        D = ops[0][0].shape[1] // 3
-        temp_exp = temperature.detach().float().exp().reshape(1)
+        rows, cols, temp_exp, world, Bg, off = _cls_loss_operands(ops, temperature, use_gather)
         bias = logit_bias.detach().float().reshape(1).contiguous()
-        rows = [o[0] for o in ops]
-        cols = D_.gather_rows([o[1] for o in ops]) if world > 1 else [o[1] for o in ops]
-        Bg = world * b
-        off = rank * b
         rowloss = K.sigmoid_fwd(rows[0], cols[1], temp_exp, bias, off)
         stats = D_.gather_stats(rowloss[None]) if world > 1 else rowloss[None]
-        ctx.cfg = (world, D, Bg, off)
+        ctx.cfg = (world, Bg, off)
         ctx.scalars = (temp_exp, bias)
         ctx.rows, ctx.cols = rows, cols
         return stats.sum() / Bg
 
     @staticmethod
     def backward(ctx, gloss):
-        world, D, Bg, off = ctx.cfg
+        world, Bg, off = ctx.cfg
         temp_exp, bias = ctx.scalars
         rows, cols = ctx.rows, ctx.cols
         gscale = (gloss.detach().float() / Bg).reshape(1)
@@ -643,8 +648,7 @@ class SigmoidLossFn(torch.autograd.Function):
         def latent_grad(r, c, want_scalars):
             g = K.sigmoid_bwd(rows[r], cols[c], temp_exp, bias, off, gscale,
                               dscalars[0:1] if want_scalars else None, dscalars[1:2] if want_scalars else None)
-            # d rows = (temp * g) @ cols_hi ; g is zero-padded to a multiple of 8 columns
-            return K.gemm(g, _pad_rows(cols[c][:, :D], g.shape[1]), b_major=1, out_dtype=F32)
+            return _latent_dgrad(g, cols[c])
 
         dzt = latent_grad(0, 1, True)
         dzi = latent_grad(1, 0, False)
@@ -812,12 +816,8 @@ def _aux_losses(clip, aux, leaves, targets):
     mlm = ssl = None
     i = 0
     if aux["mlm"] is not None:
-        rows, labels = leaves[i], aux["mlm"][2]
+        mlm = clip.mlm.loss_from_rows(leaves[i], aux["mlm"][2])
         i += 1
-        head = clip.mlm.to_logits
-        # no selected position: the single pass's enc.sum() * 0
-        mlm = VocabCrossEntropyFn.apply(rows, head.weight, head.bias, labels) if rows.shape[0] else \
-            rows.sum() * 0.
     if aux["ssl"] is not None:
         r1, r2 = leaves[i], leaves[i + 1]
         if aux["ssl_targets"]:
@@ -857,8 +857,8 @@ class ChunkedClipLossFn(torch.autograd.Function):
     passes in one fixed order (_chunk_passes); the MLM encodings of the selected positions and the
     views' CLS representations become full-batch leaves like the latents, and the heads (vocabulary
     cross-entropy, projector / predictor with BatchNorm over the whole batch, NT-Xent) run once on
-    them.  SimSiam's target passes run chunk by chunk without gradient and are never kept.  The step
-    returns cl_w * contrastive + w_t * MLM + w_i * SSL, as the single pass does.  Retention keeps or
+    them.  SimSiam's target passes run chunk by chunk without gradient and are never kept.  The loss
+    and its weighting are the single pass's (CLIP._loss, on the full-batch leaves).  Retention keeps or
     re-encodes a chunk with all of its gradient passes."""
 
     @staticmethod
@@ -869,12 +869,6 @@ class ChunkedClipLossFn(torch.autograd.Function):
         rng_states, zs, opss, kept, targets = [], [], [], [], []
         want_dimage = image.requires_grad
         img_leaves = []                               # per retained chunk: its image leaf (or None)
-
-        def chunk_image(s, e):
-            if not want_dimage:
-                return image[s:e]
-            return image[s:e].detach().requires_grad_(True)
-
         foot = None                                   # bytes of one retained chunk's activations
         reserve = 0                                   # HBM left to the loss (FILIP: filip.step_reserve_bytes)
         filip = clip.use_all_token_embeds
@@ -888,46 +882,41 @@ class ChunkedClipLossFn(torch.autograd.Function):
         if retain == "auto" and not planned:
             keep_mask = plans[plan_key]
         oom_fallbacks = 0
+
+        def keep_chunk(k, s, e):
+            """Whether chunk k keeps its activations: the remembered plan's choice, the first `retain`
+            chunks of an int plan, or ("auto") whether the free HBM holds one more chunk of its size."""
+            if keep_mask is not None:
+                return keep_mask[k]
+            if retain != "auto":
+                return k < int(retain)
+            if foot is None:                          # first chunk: keep it, measure it
+                return True
+            need = foot * ((e - s) / float(chunk)) * (1.0 + RETAIN_TRANSIENT_FRAC) + RETAIN_MARGIN_BYTES + reserve
+            return _avail_bytes(dev) >= need
+
         with torch.no_grad(), weight_scope() as wscope:
             for k, (s, e) in enumerate(bounds):
                 rng_states.append(torch.cuda.get_rng_state(dev))
-                if keep_mask is not None:
-                    keep_it = keep_mask[k]
-                elif retain == "auto":
-                    scale = (e - s) / float(chunk)
-                    if foot is None:                  # first chunk: keep it, measure it
-                        keep_it = True
-                    else:
-                        need = foot * scale * (1.0 + RETAIN_TRANSIENT_FRAC) + RETAIN_MARGIN_BYTES + reserve
-                        keep_it = _avail_bytes(dev) >= need
-                else:
-                    keep_it = k < int(retain)
-                if keep_it:
+                z = live = img_k = None
+                if keep_chunk(k, s, e):
                     before = torch.cuda.memory_allocated(dev)
-                    z = ops = None
-                    img_k = chunk_image(s, e)
+                    img_k = image[s:e].detach().requires_grad_(True) if want_dimage else None
                     try:
                         with torch.enable_grad():
                             z, ops = _chunk_passes(clip, text, image, text_mask, aux, s, e, img_k)
                     except torch.OutOfMemoryError:
                         # the plan was too optimistic (a fragmented cache, memory taken by someone else
                         # since the estimate): this chunk and all later ones are re-encoded in backward
-                        z = ops = None
                         retain, keep_mask = 0, None   # (an int plan: nothing further is kept)
                         oom_fallbacks += 1
-                    if z is None:
+                    if z is None:                     # out of memory: free the cache, replay the chunk's RNG
                         torch.cuda.empty_cache()
                         torch.cuda.set_rng_state(rng_states[-1], dev)
-                        z, ops = _chunk_passes(clip, text, image, text_mask, aux, s, e)
-                        kept.append(None)
-                        img_leaves.append(None)
-                        zs.append(z)
-                        opss.append(ops)
-                        if aux is not None and aux["ssl_targets"]:
-                            targets.append(_chunk_targets(aux, s, e))
-                        continue
-                    kept.append(list(z))
-                    img_leaves.append(img_k if want_dimage else None)
+                if z is None:                         # not kept: encoded without saving anything
+                    z, ops = _chunk_passes(clip, text, image, text_mask, aux, s, e)
+                else:
+                    live = list(z)
                     if foot is None:
                         foot = max(torch.cuda.memory_allocated(dev) - before, 1)
                         if filip:
@@ -937,13 +926,10 @@ class ChunkedClipLossFn(torch.autograd.Function):
                                                          z[0].shape[2], len(z) == 4)
                         if planned and len(bounds) > 1 and _avail_bytes(dev) < \
                                 foot * (1.0 + RETAIN_TRANSIENT_FRAC) + RETAIN_MARGIN_BYTES + reserve:
-                            kept[-1] = None           # not even a second live chunk fits beside it: let it go
-                            img_leaves[-1] = None
+                            live = None               # not even a second live chunk fits beside it: let it go
                     z = [t.detach() for t in z]
-                else:
-                    z, ops = _chunk_passes(clip, text, image, text_mask, aux, s, e)
-                    kept.append(None)
-                    img_leaves.append(None)
+                kept.append(live)
+                img_leaves.append(img_k if live is not None else None)
                 zs.append(z)
                 opss.append(ops)
                 if aux is not None and aux["ssl_targets"]:
@@ -961,34 +947,11 @@ class ChunkedClipLossFn(torch.autograd.Function):
         del zs, opss
         temp_leaf = temperature.detach().requires_grad_(True)
         bias_leaf = None if logit_bias is None else logit_bias.detach().requires_grad_(True)
-        cl_w = 1.0
-        if aux is not None:
-            cl_w = 1 - (clip.text_ssl_loss_weight + clip.image_ssl_loss_weight)
         filip_stats = {} if filip else None
         with torch.enable_grad():
-            if filip:
-                from .filip import FilipLossFn
-                loss = FilipLossFn.apply(
-                    leaves[0], leaves[1], leaves[2] if nsets == 4 else None,
-                    leaves[3] if nsets == 4 else None, temp_leaf, ops_all, text_mask.contiguous(),
-                    clip.decoupled_contrastive_learning, clip.requires_all_gather, filip_stats)
-            elif bias_leaf is not None:
-                loss = SigmoidLossFn.apply(leaves[0], leaves[1], temp_leaf, bias_leaf, ops_all,
-                                           clip.requires_all_gather)
-            else:
-                loss = ContrastiveLossFn.apply(
-                    leaves[0], leaves[1], leaves[2] if nsets == 4 else None,
-                    leaves[3] if nsets == 4 else None, temp_leaf, ops_all,
-                    clip.decoupled_contrastive_learning, clip.requires_all_gather,
-                    *((clip.sim_reg_loss_weight, cl_w) if clip.has_sim_reg_loss else ()))
-            if aux is not None:
-                if not (clip.has_sim_reg_loss and not filip):      # sim-reg weighs its contrastive term itself
-                    loss = loss * cl_w
-                mlm_loss, ssl_loss = _aux_losses(clip, aux, leaves[nsets:], targets)
-                if mlm_loss is not None:
-                    loss = loss + mlm_loss * clip.text_ssl_loss_weight
-                if ssl_loss is not None:
-                    loss = loss + ssl_loss * clip.image_ssl_loss_weight
+            mlm_loss, ssl_loss = _aux_losses(clip, aux, leaves[nsets:], targets) if aux is not None else (None, None)
+            loss = clip._loss(leaves[:nsets], ops_all, text_mask, temp_leaf, bias_leaf, mlm=mlm_loss, ssl=ssl_loss,
+                              filip_stats=filip_stats)
         del targets
         ctx.clip, ctx.inputs = clip, (text, image, text_mask)
         ctx.bounds, ctx.rng_states, ctx.kept = bounds, rng_states, kept

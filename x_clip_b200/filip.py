@@ -291,12 +291,3 @@ def positive_column(i: int, j: int, x: int, rank: int, b: int, n: int, col_run: 
     k = rank * b + x
     return (k // col_run) * n * col_run + j * col_run + k % col_run
 
-
-def filip_loss(clip, zt, zi, zt_x, zi_x, ops, text_mask, temperature=None, stats=None, views=(1, 1),
-               weights=None):
-    """views = (m, n) text / image views stacked along the batch, weights = (cl_w, mv_w): FilipLossFn."""
-    extra = clip.extra_latent_projection
-    return FilipLossFn.apply(zt, zi, zt_x if extra else None, zi_x if extra else None,
-                             clip.temperature if temperature is None else temperature, tuple(ops),
-                             text_mask.contiguous(), clip.decoupled_contrastive_learning,
-                             clip.requires_all_gather, stats, tuple(views), weights)
