@@ -87,6 +87,14 @@ int xclip_layernorm_bwd(const void* dy, int64_t lddy, const void* x, int64_t ldx
                         const float* stats, const float* g, const void* add, int64_t ldadd,
                         void* dx, int64_t lddx, float* dg, int rows, int d,
                         xclip_stream_t stream);
+/* xclip_layernorm_bwd that also writes xn = bf16(LN(x) * g) (if xn != NULL), the forward's output
+ * rebuilt from the saved stats with the forward's fp32 operations (bit for bit xclip_layernorm_fwd's
+ * out without res, or its out2 when x is that call's bf16(out)) in the pass that reads x anyway:
+ * a backward can take its weight-gradient operand from here instead of keeping it from the forward. */
+int xclip_layernorm_bwd_xn(const void* dy, int64_t lddy, const void* x, int64_t ldx,
+                           const float* stats, const float* g, const void* add, int64_t ldadd,
+                           void* dx, int64_t lddx, float* dg, void* xn, int64_t ldxn, int rows,
+                           int d, xclip_stream_t stream);
 /* l2norm = F.normalize(dim=-1, eps=1e-12) (x_clip/x_clip.py:54-55, used at :715,:724).
  * p f32 [rows,d] -> z f32 [rows,d], inv = 1/max(|p|,eps), and the split-bf16 operands of the
  * logits contraction: zrow = [hi|lo|hi], zcol = [hi|hi|lo], bf16 [rows,3d], hi = bf16(z),

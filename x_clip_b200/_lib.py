@@ -49,6 +49,9 @@ SIGNATURES = {
     "xclip_layernorm_bwd": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p,
                                     c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int, c_int,
                                     c_void_p]),
+    "xclip_layernorm_bwd_xn": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p,
+                                       c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p, c_int64,
+                                       c_int, c_int, c_void_p]),
     "xclip_l2norm_fwd": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
                                  c_int, c_void_p]),
     "xclip_l2norm_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p]),

@@ -189,13 +189,16 @@ ln_fwd_kernel(const bf16* __restrict__ x, long long ldx, const float* __restrict
 // ---------------------------------------------------------------------------
 // LayerNorm backward: dx = rstd * (g*dy - mean(g*dy) - xhat * mean(g*dy*xhat)) (+ add)
 //                     dg += sum_rows dy * xhat
+//                     xn  = bf16(xhat * g)   (optional: the forward's output, rebuilt from the saved
+//                                             stats with ln_fwd_kernel's fp32 operations, same bits)
 // ---------------------------------------------------------------------------
 template <int NV, bool HALF = false>
 __global__ void __launch_bounds__(kRowThreads)
 ln_bwd_kernel(const bf16* __restrict__ dy, long long lddy, const bf16* __restrict__ x,
               long long ldx, const float* __restrict__ stats, const float* __restrict__ g,
               const bf16* __restrict__ add, long long ldadd, bf16* __restrict__ dx,
-              long long lddx, float* __restrict__ dg, int rows) {
+              long long lddx, float* __restrict__ dg, bf16* __restrict__ xn, long long ldxn,
+              int rows) {
   constexpr int D = kRowD<NV, HALF>;
   constexpr int NVT = kRowVecs<NV, HALF>;
   __shared__ float red[D];
@@ -288,6 +291,11 @@ ln_bwd_kernel(const bf16* __restrict__ dy, long long lddy, const bf16* __restric
 #pragma unroll
       for (int e = 0; e < 8; ++e) o[e] = rstd * (gd[j][e] - s1 - xh[j][e] * s2) + a8[e];
       store8(dx + row * lddx + col, o);
+      if (xn != nullptr) {
+#pragma unroll
+        for (int e = 0; e < 8; ++e) o[e] = xh[j][e] * gg[j][e];
+        store8(xn + row * ldxn + col, o);
+      }
     }
   }
   if (dg != nullptr) flush_column_partials<NV, HALF>(dgacc, dg, red);
@@ -567,27 +575,36 @@ extern "C" int xclip_layernorm_fwd(const void* x, int64_t ldx, const float* g, c
   return XCLIP_OK;
 }
 
-extern "C" int xclip_layernorm_bwd(const void* dy, int64_t lddy, const void* x, int64_t ldx,
-                                   const float* stats, const float* g, const void* add,
-                                   int64_t ldadd, void* dx, int64_t lddx, float* dg, int rows,
-                                   int d, xclip_stream_t stream) {
+extern "C" int xclip_layernorm_bwd_xn(const void* dy, int64_t lddy, const void* x, int64_t ldx,
+                                      const float* stats, const float* g, const void* add,
+                                      int64_t ldadd, void* dx, int64_t lddx, float* dg, void* xn,
+                                      int64_t ldxn, int rows, int d, xclip_stream_t stream) {
   int rc = xclip_init();
   if (rc) return rc;
   XCLIP_REQUIRE(dy && x && stats && g && dx, "layernorm_bwd: null pointer");
   XCLIP_REQUIRE(rows > 0 && d > 0 && d % 128 == 0 && d <= 1024, "layernorm_bwd: rows=%d d=%d (d = 128*{1..8})",
                 rows, d);
-  XCLIP_REQUIRE(lddy % 8 == 0 && ldx % 8 == 0 && lddx % 8 == 0 && (!add || ldadd % 8 == 0),
+  XCLIP_REQUIRE(lddy % 8 == 0 && ldx % 8 == 0 && lddx % 8 == 0 && (!add || ldadd % 8 == 0) &&
+                    (!xn || ldxn % 8 == 0),
                 "layernorm_bwd: leading dims must be multiples of 8");
   XCLIP_REQUIRE(ALIGNED16(dy) && ALIGNED16(x) && ALIGNED16(dx) && ALIGNED16(g) &&
-                    (!add || ALIGNED16(add)),
+                    (!add || ALIGNED16(add)) && (!xn || ALIGNED16(xn)),
                 "layernorm_bwd: pointers must be 16-byte aligned");
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   const int per_sm = tune(XCLIP_TUNE_LN_BWD_BLOCKS) > 0 ? tune(XCLIP_TUNE_LN_BWD_BLOCKS) : 2;
   const int grid = row_grid(rows) < num_sms() * per_sm ? row_grid(rows) : num_sms() * per_sm;
   DISPATCH_NARROW(ln_bwd_kernel, d, grid, s, (const bf16*)dy, lddy, (const bf16*)x, ldx, stats, g,
-                  (const bf16*)add, ldadd, (bf16*)dx, lddx, dg, rows)
+                  (const bf16*)add, ldadd, (bf16*)dx, lddx, dg, (bf16*)xn, ldxn, rows)
   XCLIP_LAUNCH_CHECK("ln_bwd_kernel");
   return XCLIP_OK;
+}
+
+extern "C" int xclip_layernorm_bwd(const void* dy, int64_t lddy, const void* x, int64_t ldx,
+                                   const float* stats, const float* g, const void* add,
+                                   int64_t ldadd, void* dx, int64_t lddx, float* dg, int rows,
+                                   int d, xclip_stream_t stream) {
+  return xclip_layernorm_bwd_xn(dy, lddy, x, ldx, stats, g, add, ldadd, dx, lddx, dg, nullptr, 0, rows, d,
+                                stream);
 }
 
 extern "C" int xclip_l2norm_fwd(const float* p, int64_t ldp, float* z, void* zrow, void* zcol,

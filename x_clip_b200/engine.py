@@ -111,6 +111,29 @@ def _grad_target(param: torch.Tensor):
     return g
 
 
+# Set by the micro-batched step around the chunks it keeps in compact mode: TransformerFn then saves
+# per layer only what a GEMM or attention made (xcur, qkv, o, y, acc: 7 d per token-layer, plus the row
+# statistics) and its backward rebuilds the feed-forward's inputs (x1, xn2, u, h: 14 d) one layer at a
+# time with the forward's own LayerNorm and up-projection calls - the same bits, so the same gradients.
+_compact_save = False
+
+
+class _CompactSave:
+    def __init__(self, flag: bool):
+        self.flag = flag
+
+    def __enter__(self):
+        global _compact_save
+        self.prev = _compact_save
+        _compact_save = self.flag
+        return self
+
+    def __exit__(self, *exc):
+        global _compact_save
+        _compact_save = self.prev
+        return False
+
+
 class TransformerFn(torch.autograd.Function):
     """x[B,n,d] (bf16) -> norm_out(blocks(norm_in(x))) (bf16); mask: bool [B,n] or None.
 
@@ -118,6 +141,8 @@ class TransformerFn(torch.autograd.Function):
     causal: the reference's causal mask (x_clip.py:233-236); rot_cos / rot_sin: f32 [n, 16] tables of
     the rotary embedding applied to q, k and v (x_clip.py:221-223) or None.
     TransformerDropoutFn is the same encoder with attention dropout.
+    Saved per token and layer: 21 d bf16 (full), or 7 d under _compact_save.  The pre-norm output xn
+    is never saved: the pre-norm's LayerNorm backward emits it for the wqkv weight gradient.
     """
 
     @staticmethod
@@ -146,6 +171,8 @@ class TransformerFn(torch.autograd.Function):
         # need_bwd = torch.is_grad_enabled() at the call site (inside forward() it is always off and
         # needs_input_grad ignores no_grad): in the first sweep of the micro-batched step and in
         # inference nothing is kept for a backward, and the 8d-wide u = [value | gate] is not written
+        # (nor in compact mode, whose backward rebuilds it)
+        compact = need_bwd and _compact_save
         # bf16 MMA operands of this call's weights; backward reuses exactly these (ctx.wb)
         wb = [tuple(weight_bf16(w) for w in (l[1], l[2], l[5])) for l in layers]
         # norm_in fused with the first pre-norm
@@ -162,13 +189,14 @@ class TransformerFn(torch.autograd.Function):
             # fused feed-forward (csrc/ff.cu): GEGLU in the up-projection's epilogue, LayerNorm(4d)
             # folded into the down-projection.  h is hp = value*gelu(gate) BEFORE the LayerNorm.
             w1p, w2g, colvec = ff_weights(w1, w2, g4)
-            u, h, rowsum = K.ff_up(xn2, w1p, need_u=need_bwd)
+            u, h, rowsum = K.ff_up(xn2, w1p, need_u=need_bwd and not compact)
             x2, acc, st_v = K.ff_down(h, w2g, colvec, rowsum, x1, LN_EPS)
             # forward-only sweeps keep NOTHING alive beyond the layer (the list below would otherwise hold
-            # every layer's activations until the call returns: ~14 of the 22 d per token-layer)
+            # every layer's activations until the call returns: ~14 of the 21 d per token-layer)
             if need_bwd:
-                saved.append((xcur, st1, xn, qkv, o, lse, y, st_y, x1, st_x1, xn2, u, st_v, h,
-                              w2g, colvec, acc))
+                ff_in = None if compact else (x1, st_x1, xn2, u, h)
+                saved.append((xcur, st1, qkv, o, lse, y, st_y, st_v, w1p if compact else None, w2g, colvec, acc,
+                              ff_in))
             del qkv, o, lse, y, x1, xn2, u, h
             xcur = x2
             if L + 1 < depth:
@@ -231,9 +259,14 @@ class TransformerFn(torch.autograd.Function):
         dx = K.layernorm_bwd(dout, x_last, st_out, g_out, dg=dg_out)
         for L in reversed(range(depth)):
             g1, wqkv, wo, go, g2, w1, g4, w2 = layers[L]
-            (xcur, st1, xn, qkv, o, lse, y, st_y, x1, st_x1, xn2, u, st_v, h,
-             w2g, colvec, acc) = ctx.saved[L]
+            xcur, st1, qkv, o, lse, y, st_y, st_v, w1p, w2g, colvec, acc, ff_in = ctx.saved[L]
             ctx.saved[L] = None
+            if ff_in is None:     # compact: the forward's own calls, so the same bits
+                x1, _, xn2, st_x1 = K.layernorm_fwd(y, go, res=xcur, g2=g2, eps=LN_EPS)
+                u, h, _ = K.ff_up(xn2, w1p)
+            else:
+                x1, st_x1, xn2, u, h = ff_in
+            del ff_in
             bqkv, bo, b1 = ctx.wb[L]
             base = 2 + 8 * L
             # feed-forward: x2 = LN(hp) g4 @ w2^T + x1, h the pre-norm hp.  Row means of the LayerNorm
@@ -252,11 +285,13 @@ class TransformerFn(torch.autograd.Function):
                 if tgt is not None or not wneed[base + 7]:
                     dw2 = None
             grads[base + 7] = dw2
+            del u, h
             dxn2 = K.gemm(du, b1, b_major=1)
             grads[base + 5] = weight_grad(base + 5, du, xn2)
-            del du
+            del du, xn2
             dg2, grads[base + 4] = gain_grad(base + 4)
             dx1 = K.layernorm_bwd(dxn2, x1, st_x1, g2, add=dx, dg=dg2)
+            del x1
             # attention: x1 = LN(o @ wo^T) * go + x
             dgo, grads[base + 3] = gain_grad(base + 3)
             dy = K.layernorm_bwd(dx1, y, st_y, go, dg=dgo)
@@ -267,9 +302,13 @@ class TransformerFn(torch.autograd.Function):
             if rot_cos is not None:      # back through the rotation (its transpose)
                 K.rotary_(dqkv, n, 3 * heads, rot_cos, rot_sin, inverse=True)
             dxn = K.gemm(dqkv, bqkv, b_major=1)
-            grads[base + 1] = weight_grad(base + 1, dqkv, xn)
             dg1, grads[base + 0] = gain_grad(base + 0)
-            dx = K.layernorm_bwd(dxn, xcur, st1, g1, add=dx1, dg=dg1)
+            if wneed[base + 1]:
+                dx, xn = K.layernorm_bwd(dxn, xcur, st1, g1, add=dx1, dg=dg1, want_xn=True)
+                grads[base + 1] = weight_grad(base + 1, dqkv, xn)
+                del xn
+            else:
+                dx = K.layernorm_bwd(dxn, xcur, st1, g1, add=dx1, dg=dg1)
         dg_in, grads[0] = gain_grad(0)
         dx_in = K.layernorm_bwd(dx, x_in, st_in, g_in, dg=dg_in)
         ctx.saved = ctx.wb = ctx.drop = None
@@ -762,9 +801,28 @@ def _avail_bytes(dev) -> int:
 # regularisation adds its packed operands, 24 (b + B_g) D bytes for the two latent pairs, and one
 # more transient g[b, B_g] bf16 at a time: 0.72 GB at b = 4096, B_g = 32768, D = 512 - inside the margin.
 RETAIN_MARGIN_BYTES = 10 << 30
-# transient buffers of one chunk's backward (du 8d + a few d-wide rows of one layer) relative to
-# the chunk's saved activations (22 d per token-layer x depth)
-RETAIN_TRANSIENT_FRAC = 0.15
+# transient buffers of one kept chunk's backward relative to its saved activations, per save mode.  Full
+# (21 d per token-layer x depth): du 8d + a few d-wide rows of one layer.  Compact (7 d x depth): those
+# and the layer's rebuilt x1, xn2, u, h, about 24 d of one layer.
+RETAIN_TRANSIENT_FRAC = {"full": 0.15, "compact": 0.3}
+# Save mode of the chunks the micro-batched step keeps (TransformerFn, _compact_save): None lets the
+# "auto" plan choose - full when every chunk fits in full mode, else compact, which keeps three times as
+# many chunks and rebuilds a LayerNorm and the up-projection per layer instead of re-encoding a chunk.
+# "full" / "compact" force one (tests); an int plan keeps full chunks unless forced.
+RETAIN_MODE = None
+
+
+def retain_need_bytes(foot: int, rows: int, chunk: int, mode: str, reserve: int) -> float:
+    """Free HBM the plan asks for before it keeps one more chunk of `rows` pairs in `mode`, for a
+    full-size chunk of `chunk` pairs that holds `foot` bytes in that mode."""
+    return foot * (rows / float(chunk)) * (1.0 + RETAIN_TRANSIENT_FRAC[mode]) + RETAIN_MARGIN_BYTES + reserve
+
+
+def fits_all_full(avail: int, foot: int, rows: List[int], chunk: int, reserve: int) -> bool:
+    """Whether `avail` free bytes, beside the first chunk kept in full mode (`foot` bytes), hold the other
+    chunks of `rows` pairs each in full mode as well, with one backward's transients."""
+    rest = sum(rows[1:]) / float(chunk)
+    return avail >= foot * (rest + RETAIN_TRANSIENT_FRAC["full"]) + RETAIN_MARGIN_BYTES + reserve
 
 
 class _InPlaceGradAccumulation:
@@ -847,7 +905,9 @@ class ChunkedClipLossFn(torch.autograd.Function):
     the GPU's HBM holds (80 GB on an H100) (`retain`: "auto" measures the first chunk's footprint and plans against
     the free memory; an int fixes the count; 0 = none); only the remaining chunks are encoded
     without saving anything and re-encoded in step 3 (RNG replayed for PatchDropout).  Retained
-    chunks cost no extra flops; each re-encoded chunk costs one extra encoder forward.
+    chunks cost no extra flops in full mode; compact ones (a third of the memory, chosen by "auto" when
+    not every chunk fits in full mode, see RETAIN_MODE) rebuild one LayerNorm and the feed-forward's
+    up-projection per layer in backward; each re-encoded chunk costs one extra encoder forward.
     An image that wants a gradient enters every chunk's encoder as a detached per-chunk leaf; backward
     collects the leaves' gradients into d loss / d image, so the outer graph (a generator, an
     augmentation) is only ever entered by autograd itself, after this backward returns.
@@ -866,7 +926,7 @@ class ChunkedClipLossFn(torch.autograd.Function):
         B = text.shape[0]
         dev = text.device
         bounds = [(s, min(s + chunk, B)) for s in range(0, B, chunk)]
-        rng_states, zs, opss, kept, targets = [], [], [], [], []
+        rng_states, zs, opss, kept, lives, targets = [], [], [], [], [], []
         want_dimage = image.requires_grad
         img_leaves = []                               # per retained chunk: its image leaf (or None)
         foot = None                                   # bytes of one retained chunk's activations
@@ -882,53 +942,80 @@ class ChunkedClipLossFn(torch.autograd.Function):
         if retain == "auto" and not planned:
             keep_mask = plans[plan_key]
         oom_fallbacks = 0
+        # save mode of the kept chunks: an int plan keeps full chunks; "auto" measures its first chunk in
+        # full mode and keeps it that way only when every chunk fits so (fits_all_full)
+        mode = RETAIN_MODE or "full"
 
         def keep_chunk(k, s, e):
-            """Whether chunk k keeps its activations: the remembered plan's choice, the first `retain`
-            chunks of an int plan, or ("auto") whether the free HBM holds one more chunk of its size."""
+            """The save mode chunk k keeps its activations in, or None: the remembered plan's choice, the
+            first `retain` chunks of an int plan, or ("auto") whether the free HBM holds one more chunk of
+            its size."""
             if keep_mask is not None:
                 return keep_mask[k]
             if retain != "auto":
-                return k < int(retain)
+                return mode if k < int(retain) else None
             if foot is None:                          # first chunk: keep it, measure it
-                return True
-            need = foot * ((e - s) / float(chunk)) * (1.0 + RETAIN_TRANSIENT_FRAC) + RETAIN_MARGIN_BYTES + reserve
-            return _avail_bytes(dev) >= need
+                return mode
+            return mode if _avail_bytes(dev) >= retain_need_bytes(foot, e - s, chunk, mode, reserve) else None
+
+        def encode_kept(s, e, m):
+            """(latents, ops, image leaf, bytes) of chunk [s, e) encoded with its activations kept in save
+            mode m, or None when it runs out of memory"""
+            before = torch.cuda.memory_allocated(dev)
+            img_k = image[s:e].detach().requires_grad_(True) if want_dimage else None
+            try:
+                with torch.enable_grad(), _CompactSave(m == "compact"):
+                    z, ops = _chunk_passes(clip, text, image, text_mask, aux, s, e, img_k)
+            except torch.OutOfMemoryError:
+                return None
+            return z, ops, img_k, max(torch.cuda.memory_allocated(dev) - before, 1)
 
         with torch.no_grad(), weight_scope() as wscope:
             for k, (s, e) in enumerate(bounds):
                 rng_states.append(torch.cuda.get_rng_state(dev))
                 z = live = img_k = None
-                if keep_chunk(k, s, e):
-                    before = torch.cuda.memory_allocated(dev)
-                    img_k = image[s:e].detach().requires_grad_(True) if want_dimage else None
-                    try:
-                        with torch.enable_grad():
-                            z, ops = _chunk_passes(clip, text, image, text_mask, aux, s, e, img_k)
-                    except torch.OutOfMemoryError:
-                        # the plan was too optimistic (a fragmented cache, memory taken by someone else
-                        # since the estimate): this chunk and all later ones are re-encoded in backward
-                        retain, keep_mask = 0, None   # (an int plan: nothing further is kept)
+                m = keep_chunk(k, s, e)
+                if m is not None:
+                    got = encode_kept(s, e, m)
+                    if got is not None and foot is None:
+                        foot = got[3]
+                        if filip:
+                            from .filip import step_reserve_bytes
+                            world = D_.world()[1] if clip.requires_all_gather else 1
+                            z0 = got[0]
+                            reserve = step_reserve_bytes(B, world * B, z0[0].shape[1], z0[1].shape[1],
+                                                         z0[0].shape[2], len(z0) == 4)
+                            del z0
+                        if planned and RETAIN_MODE is None and len(bounds) > 1 and not fits_all_full(
+                                _avail_bytes(dev), foot, [b - a for a, b in bounds], chunk, reserve):
+                            # not every chunk fits in full mode: measure the first one again in compact mode
+                            got = None
+                            torch.cuda.set_rng_state(rng_states[-1], dev)
+                            mode = m = "compact"
+                            got = encode_kept(s, e, m)
+                            if got is not None:
+                                foot = got[3]
+                    if got is None:
+                        # out of memory - the plan was too optimistic (a fragmented cache, memory taken by
+                        # someone else since the estimate): this chunk and all later ones are re-encoded in
+                        # backward (an int plan: nothing further is kept); free the cache, replay the RNG
+                        retain, keep_mask = 0, None
                         oom_fallbacks += 1
-                    if z is None:                     # out of memory: free the cache, replay the chunk's RNG
                         torch.cuda.empty_cache()
                         torch.cuda.set_rng_state(rng_states[-1], dev)
+                    else:
+                        z, ops, img_k, _ = got
+                        del got
                 if z is None:                         # not kept: encoded without saving anything
                     z, ops = _chunk_passes(clip, text, image, text_mask, aux, s, e)
                 else:
                     live = list(z)
-                    if foot is None:
-                        foot = max(torch.cuda.memory_allocated(dev) - before, 1)
-                        if filip:
-                            from .filip import step_reserve_bytes
-                            world = D_.world()[1] if clip.requires_all_gather else 1
-                            reserve = step_reserve_bytes(B, world * B, z[0].shape[1], z[1].shape[1],
-                                                         z[0].shape[2], len(z) == 4)
-                        if planned and len(bounds) > 1 and _avail_bytes(dev) < \
-                                foot * (1.0 + RETAIN_TRANSIENT_FRAC) + RETAIN_MARGIN_BYTES + reserve:
-                            live = None               # not even a second live chunk fits beside it: let it go
+                    if k == 0 and planned and len(bounds) > 1 and \
+                            _avail_bytes(dev) < retain_need_bytes(foot, chunk, chunk, m, reserve):
+                        live = None                   # not even a second live chunk fits beside it: let it go
                     z = [t.detach() for t in z]
-                kept.append(live)
+                kept.append(m if live is not None else None)
+                lives.append(live)
                 img_leaves.append(img_k if live is not None else None)
                 zs.append(z)
                 opss.append(ops)
@@ -954,20 +1041,21 @@ class ChunkedClipLossFn(torch.autograd.Function):
                               filip_stats=filip_stats)
         del targets
         ctx.clip, ctx.inputs = clip, (text, image, text_mask)
-        ctx.bounds, ctx.rng_states, ctx.kept = bounds, rng_states, kept
+        ctx.bounds, ctx.rng_states, ctx.kept = bounds, rng_states, lives
         ctx.aux, ctx.row_bounds = aux, row_bounds
         ctx.img_leaves = img_leaves if want_dimage else None
         ctx.graph = (loss, leaves, temp_leaf, bias_leaf)
         ctx.weight_casts = wscope.cache
-        n_kept = sum(z is not None for z in kept)
+        n_kept = sum(m is not None for m in kept)
         if planned or (oom_fallbacks and plan_key in plans):
-            plans[plan_key] = [z is not None for z in kept]    # WHICH chunks stay resident
+            plans[plan_key] = kept                    # WHICH chunks stay resident, in which save mode
         passes = ["contrastive"]
         if aux is not None:
             passes += (["mlm"] if aux["mlm"] is not None else []) + (["view1", "view2"] if aux["ssl"] is not None else [])
         clip.last_step_plan = dict(chunks=len(bounds), retained=n_kept, chunk_activation_bytes=foot,
                                    oom_fallbacks=oom_fallbacks, passes=passes,
-                                   retained_chunks=[k for k, z in enumerate(kept) if z is not None])
+                                   retained_chunks=[k for k, m in enumerate(kept) if m is not None],
+                                   compact_chunks=[k for k, m in enumerate(kept) if m == "compact"])
         if filip:
             # rows of both FILIP passes whose argmax was saved / will be recomputed in backward
             clip.last_step_plan.update(filip=filip_stats, loss_reserve_bytes=reserve)

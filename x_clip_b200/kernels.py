@@ -169,18 +169,20 @@ def layernorm_fwd(x, g, *, res=None, g2=None, eps=1e-5, want_stats=True):
     return out, stats, out2, stats2
 
 
-def layernorm_bwd(dy, x, stats, g, *, add=None, dg=None):
-    """dx = dLN(dy) (+add); dg (fp32 [d]) is accumulated into when given."""
+def layernorm_bwd(dy, x, stats, g, *, add=None, dg=None, want_xn=False):
+    """dx = dLN(dy) (+add); dg (fp32 [d]) is accumulated into when given.  want_xn: returns (dx, xn)
+    with xn = LN(x)*g, bit for bit the layernorm_fwd output that `stats` came from."""
     _need(dy, BF16, "dy"); _need(x, BF16, "x"); _rows2d(dy, "dy"); _rows2d(x, "x")
     rows, d = x.shape
     dx = torch.empty((rows, d), device=x.device, dtype=BF16)
+    xn = torch.empty((rows, d), device=x.device, dtype=BF16) if want_xn else None
     if add is not None:
         _need(add, BF16, "add"); _rows2d(add, "add")
-    _call(dy, "layernorm_bwd", 0.0, 2.0 * rows * d * (3 + (1 if add is not None else 0)),
-          "xclip_layernorm_bwd", dy.data_ptr(), dy.stride(0), x.data_ptr(), x.stride(0),
+    _call(dy, "layernorm_bwd", 0.0, 2.0 * rows * d * (3 + (1 if add is not None else 0) + (1 if want_xn else 0)),
+          "xclip_layernorm_bwd_xn", dy.data_ptr(), dy.stride(0), x.data_ptr(), x.stride(0),
               stats.data_ptr(), g.data_ptr(), _ptr(add), add.stride(0) if add is not None else 0,
-              dx.data_ptr(), dx.stride(0), _ptr(dg), rows, d)
-    return dx
+              dx.data_ptr(), dx.stride(0), _ptr(dg), _ptr(xn), xn.stride(0) if want_xn else 0, rows, d)
+    return (dx, xn) if want_xn else dx
 
 
 def l2norm_fwd(p):
