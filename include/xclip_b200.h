@@ -419,6 +419,41 @@ int xclip_rotary_inplace(void* qkv, int64_t ld, int64_t rows, int n, int nslices
                          const float* cos_tab, const float* sin_tab, int inverse,
                          xclip_stream_t stream);
 
+/* ---- SimCLR augmentation of the visual SSL losses (x_clip/visual_ssl.py:24-45) ---------------------
+ * One decision per call for the whole batch, applied to x f32 [B, C, H, W] (contiguous) in this order:
+ *   colour jitter: ops[k] = 0 brightness, 1 contrast, 2 saturation, 3 hue, -1 none, applied for
+ *       k = 0..3 with torchvision's fp32 arithmetic: _blend(img, other, factor[op]) with weights
+ *       factor[op] and one_minus[op] (= fp32(1 - factor[op]), rounded from double as torchvision does)
+ *       and its clamp to [0, 1]; contrast blends with the per-image grayscale mean of the image as it is
+ *       at that point (xclip_augment_mean); hue is _rgb2hsv, (h + factor[3]) % 1, _hsv2rgb;
+ *   grayscale != 0: rgb_to_grayscale (0.2989 / 0.587 / 0.114) into all 3 channels;
+ *   flip != 0: horizontal flip;
+ *   blur != 0: 3x3 cross-correlation with blur_kernel (row-major) and reflect padding at the image
+ *       border, so pixels at the crop's edge see their neighbours outside the crop;
+ *   crop (top, left, height, width), resized to out_h x out_w by ATen's antialiased bilinear
+ *       (align_corners = False); the crop lies inside the image and is no larger than the output;
+ *   normalize != 0: (v - mean[c]) / std[c].
+ * The colour stages and Normalize need C == 3.  Offsets are 64-bit (any B * C * H * W).
+ * mean  : out f32 [B], the grayscale mean per image of the jitter's ops before contrast (C == 3).
+ *         Fixed-order reduction: deterministic.
+ * apply : out f32 [B, C, out_h, out_w]; mean is read only when ops contain contrast (then required).
+ * Both return XCLIP_ERR_INVALID without launching for: a null or misaligned (4-byte) pointer, H or W
+ * < 2, a crop outside the image or larger than the output, colour stages at C != 3. */
+typedef struct xclip_augment_params {
+  int32_t ops[4];
+  float factor[4];
+  float one_minus[4];
+  int32_t grayscale, flip, blur, normalize;
+  float blur_kernel[9];
+  float mean[3], std[3];
+  int32_t top, left, height, width;
+  int32_t out_h, out_w;
+} xclip_augment_params;
+int xclip_augment_mean(const float* x, int B, int C, int H, int W, const xclip_augment_params* params,
+                       float* mean, xclip_stream_t stream);
+int xclip_augment_apply(const float* x, int B, int C, int H, int W, const xclip_augment_params* params,
+                        const float* mean, float* out, xclip_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -2,11 +2,12 @@
 (DCL + extra latent projections + use_visual_ssl, README.md) at 1024 and 4096 pairs per GPU, and cfg3
 with MLM at 4096 pairs per GPU, micro-batch 768.  Prints one JSON line per run with pairs/s, the peak
 allocation, the retention plan, and the card's name and power limit read in the same run.  The SSL
-views are augmented on the whole batch at once; `--augment flip` replaces the reference's pipeline
-(whose Gaussian blur alone allocates 18 GiB at 4096 images of 256 px) by a horizontal flip.
+views are augmented on the whole batch at once by the default augmentation (SimCLRAugmentation, on the
+CUDA kernels); `--augment flip` replaces it by a horizontal flip.  `--lr` > 0 takes a fused AdamW step
+after every step and prints the loss of each timed step (a training run on one fixed batch).
 
     python tools/aux_microbatch_bench.py [--runs readme_simsiam:1024,readme_simsiam:4096,cfg3_mlm:4096]
-                                         [--microbatch 768] [--steps 3] [--warmup 1]
+                                         [--microbatch 768] [--steps 3] [--warmup 1] [--lr 0]
 """
 import argparse
 import json
@@ -32,7 +33,8 @@ def main():
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=1)
     ap.add_argument("--augment", default="default", choices=["default", "flip"],
-                    help="SSL views: the reference's torchvision pipeline, or a horizontal flip only")
+                    help="SSL views: the reference's pipeline, or a horizontal flip only")
+    ap.add_argument("--lr", type=float, default=0.0, help="> 0: an AdamW step after every step")
     a = ap.parse_args()
 
     import torch
@@ -56,11 +58,18 @@ def main():
         if a.augment == "flip" and kw.get("use_visual_ssl"):
             from torchvision import transforms as T
             clip.visual_ssl.augment1 = clip.visual_ssl.augment2 = T.RandomHorizontalFlip()
+        opt = None
+        if a.lr > 0:
+            from x_clip_b200.optim import FusedAdamW
+            opt = FusedAdamW(clip.parameters(), lr=a.lr)
+        losses = []
         text = torch.randint(3, kw["num_text_tokens"], (batch, kw["text_seq_len"]), device=dev)
         image = torch.randn(batch, 3, kw["visual_image_size"], kw["visual_image_size"], device=dev)
         t0 = time.perf_counter()
         for _ in range(a.warmup):
             clip(text, image, return_loss=True).backward()
+            if opt is not None:
+                opt.step()
             clip.zero_grad(set_to_none=True)
         torch.cuda.synchronize()
         torch.cuda.reset_peak_memory_stats(dev)
@@ -69,6 +78,9 @@ def main():
         for _ in range(a.steps):
             loss = clip(text, image, return_loss=True)
             loss.backward()
+            if opt is not None:
+                opt.step()
+                losses.append(loss.detach())
             clip.zero_grad(set_to_none=True)
         e1.record()
         torch.cuda.synchronize()
@@ -78,7 +90,9 @@ def main():
                               step_ms=round(ms, 1), pairs_per_s=round(batch / (ms / 1e3), 1),
                               peak_alloc_gib=round(torch.cuda.max_memory_allocated(dev) / 2 ** 30, 2),
                               chunks=sp["chunks"], retained_chunks=sp["retained_chunks"], passes=sp["passes"],
-                              augment=a.augment, loss=round(loss.item(), 5), wall_s=round(time.perf_counter() - t0, 1), card=gpu)),
+                              augment=a.augment, loss=round(loss.item(), 5),
+                              **(dict(lr=a.lr, losses=[round(v.item(), 5) for v in losses]) if opt else {}),
+                              wall_s=round(time.perf_counter() - t0, 1), card=gpu)),
               flush=True)
         del clip, text, image, loss
         torch.cuda.empty_cache()

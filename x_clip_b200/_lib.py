@@ -118,7 +118,19 @@ SIGNATURES = {
                                            c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "xclip_filip_nce_blocks_bwd": (c_int, [c_void_p, c_int64, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
                                            c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
+    "xclip_augment_mean": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "xclip_augment_apply": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                    c_void_p]),
 }
+
+
+class AugmentParams(ctypes.Structure):
+    """xclip_augment_params of include/xclip_b200.h (passed by host pointer)."""
+    _fields_ = [("ops", c_int * 4), ("factor", c_float * 4), ("one_minus", c_float * 4),
+                ("grayscale", c_int), ("flip", c_int), ("blur", c_int), ("normalize", c_int),
+                ("blur_kernel", c_float * 9), ("mean", c_float * 3), ("std", c_float * 3),
+                ("top", c_int), ("left", c_int), ("height", c_int), ("width", c_int),
+                ("out_h", c_int), ("out_w", c_int)]
 
 
 def load() -> ctypes.CDLL:

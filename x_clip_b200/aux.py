@@ -7,9 +7,11 @@ loss (x_clip/x_clip.py:611-621, :851-868).  Here the same objectives are written
 H100 encoders of this package: the expensive part - every encoder pass - runs on the CUDA kernels
 (engine.TransformerFn), the MLM head's vocabulary projection and its cross entropy run as one
 wgmma GEMM with the softmax in its epilogue over the MASKED positions only
-(engine.VocabCrossEntropyFn: no [n_sel, V] logits, any vocabulary size), and the small heads
-(BatchNorm MLPs, cosine / NT-Xent losses, torchvision augmentations) stay ordinary torch modules,
-exactly as in the reference - they are not on the north-star path.
+(engine.VocabCrossEntropyFn: no [n_sel, V] logits, any vocabulary size), and the SimCLR augmentation
+of the two views runs as two CUDA kernels with torchvision's draws and arithmetic (SimCLRAugmentation:
+the torchvision pipeline's own temporaries do not fit at thousands of images per GPU).  The small
+heads (BatchNorm MLPs, cosine / NT-Xent losses) stay ordinary torch modules, exactly as in the
+reference - they are not on the north-star path.
 
 Parameter names follow the reference (`mlm.to_logits.*`, `visual_ssl.online_encoder.*`) where the
 reference has parameters; masks and augmentations are random in both implementations, so parity is
@@ -18,7 +20,7 @@ checked on the deterministic parts (tests/test_gpu_aux.py: a fixed masking, iden
 from __future__ import annotations
 
 import math
-from typing import Optional, Sequence
+from typing import NamedTuple, Optional, Sequence, Tuple
 
 import torch
 import torch.nn.functional as F
@@ -97,29 +99,116 @@ class MLM(nn.Module):
 
 # ----------------------------------------------------------------------------- visual SSL
 
+class AugmentParams(NamedTuple):
+    """The draws of one call of the SimCLR augmentation (SimCLRAugmentation.draw), for the whole batch.
+    order: the colour-jitter op ids (0 brightness, 1 contrast, 2 saturation, 3 hue) in the drawn order,
+    () when the jitter does not apply; factors: the four jitter factors indexed by op id (None skips an
+    op); sigma: the blur's sigma, None when the blur does not apply; crop: (top, left, height, width)."""
+    order: Tuple[int, ...]
+    factors: Tuple[Optional[float], ...]
+    grayscale: bool
+    flip: bool
+    sigma: Optional[float]
+    crop: Tuple[int, int, int, int]
+
+
+class SimCLRAugmentation(nn.Module):
+    """The SimCLR-style pipeline the reference builds (visual_ssl.py:59-88) from torchvision:
+
+        RandomApply(ColorJitter(0.8, 0.8, 0.8, 0.2), p=0.3)      (RGB only)
+        RandomGrayscale(p=0.2)                                    (RGB only)
+        RandomHorizontalFlip()
+        RandomApply(GaussianBlur((3, 3), (1.0, 2.0)), p=0.2)     (channels > 1)
+        RandomResizedCrop((image_size, image_size))
+        Normalize(ImageNet mean / std)                            (RGB only)
+
+    as one decision per call for the whole batch.  `draw(shape)` takes every parameter from
+    torchvision's own get_params / torch.rand calls in the Sequential's order (CPU generator only, from
+    the shape alone: no host synchronisation); `apply(x, params)` applies them.  A CUDA input that does
+    not take part in autograd runs the CUDA kernels (kernels.augment: one HBM read of the input, one
+    more when contrast needs its per-image mean, one write of the view), which is what lets SimSiam /
+    SimCLR augment thousands of images per GPU at once; an input that requires grad (or a CPU input)
+    takes torchvision's functional ops with the same parameters, so the image still gets a gradient.
+    Registers no parameters or buffers."""
+
+    BLUR_P, JITTER_P, GRAY_P = 0.2, 0.3, 0.2
+    MEAN, STD = (0.485, 0.456, 0.406), (0.229, 0.224, 0.225)
+
+    def __init__(self, image_size: int, channels: int = 3):
+        super().__init__()
+        from torchvision import transforms as T
+        self.image_size, self.channels = int(image_size), int(channels)
+        self.rgb, self.blurs = channels == 3, channels > 1
+        jitter = T.ColorJitter(0.8, 0.8, 0.8, 0.2)
+        self._jitter = (jitter.brightness, jitter.contrast, jitter.saturation, jitter.hue)
+        crop = T.RandomResizedCrop((self.image_size, self.image_size))
+        self._scale, self._ratio = crop.scale, crop.ratio
+        self._blur_sigma = T.GaussianBlur((3, 3), (1.0, 2.0)).sigma
+
+    def draw(self, shape) -> AugmentParams:
+        from torchvision import transforms as T
+        order, factors, gray = (), (None,) * 4, False
+        if self.rgb:
+            if not torch.rand(()) > self.JITTER_P:                # the reference's RandomApply
+                fn_idx, *factors = T.ColorJitter.get_params(*self._jitter)
+                order, factors = tuple(int(i) for i in fn_idx), tuple(factors)
+            gray = bool(torch.rand(1) < self.GRAY_P)
+        flip = bool(torch.rand(1) < 0.5)
+        sigma = None
+        if self.blurs and not torch.rand(()) > self.BLUR_P:
+            sigma = T.GaussianBlur.get_params(*self._blur_sigma)
+        crop = T.RandomResizedCrop.get_params(torch.empty(tuple(shape), device="meta"), self._scale, self._ratio)
+        return AugmentParams(order, factors, gray, flip, sigma, tuple(int(v) for v in crop))
+
+    def apply(self, x: torch.Tensor, params: AugmentParams) -> torch.Tensor:
+        if x.is_cuda and not (x.requires_grad and torch.is_grad_enabled()):
+            return self._apply_kernels(x, params)
+        return self.apply_torchvision(x, params)
+
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        return self.apply(x, self.draw(x.shape))
+
+    def apply_torchvision(self, x: torch.Tensor, params: AugmentParams) -> torch.Tensor:
+        """The same parameters through torchvision's functional ops (any device, dtype and autograd)."""
+        from torchvision.transforms import functional as TF
+        jitter = (TF.adjust_brightness, TF.adjust_contrast, TF.adjust_saturation, TF.adjust_hue)
+        for op in params.order:
+            if params.factors[op] is not None:
+                x = jitter[op](x, params.factors[op])
+        if params.grayscale:
+            x = TF.rgb_to_grayscale(x, num_output_channels=x.shape[-3])
+        if params.flip:
+            x = TF.hflip(x)
+        if params.sigma is not None:
+            x = TF.gaussian_blur(x, [3, 3], [params.sigma, params.sigma])
+        x = TF.resized_crop(x, *params.crop, [self.image_size, self.image_size],
+                            TF.InterpolationMode.BILINEAR, antialias=True)
+        if self.rgb:
+            x = TF.normalize(x, torch.tensor(self.MEAN), torch.tensor(self.STD))
+        return x
+
+    def _apply_kernels(self, x: torch.Tensor, params: AugmentParams) -> torch.Tensor:
+        from . import kernels as K
+        ops = [op for op in params.order if params.factors[op] is not None]
+        factor = [0.0 if f is None else float(f) for f in params.factors]
+        # _blend's (1.0 - ratio) is a double rounded to fp32 when it scales the fp32 image
+        one_minus = [1.0 - f for f in factor]
+        blur = None
+        if params.sigma is not None:
+            from torchvision.transforms._functional_tensor import _get_gaussian_kernel2d
+            blur = _get_gaussian_kernel2d([3, 3], [params.sigma, params.sigma], torch.float32,
+                                          torch.device("cpu")).flatten().tolist()
+        squeeze = x.dim() == 3
+        out = K.augment(x.unsqueeze(0) if squeeze else x, ops=ops, factor=factor, one_minus=one_minus,
+                        grayscale=params.grayscale, flip=params.flip, blur_kernel=blur,
+                        normalize=(self.MEAN, self.STD) if self.rgb else None, crop=params.crop,
+                        out_size=(self.image_size, self.image_size))
+        return out[0] if squeeze else out
+
+
 def default_augmentation(image_size: int, channels: int = 3) -> nn.Module:
-    """The SimCLR-style pipeline the reference builds (visual_ssl.py:59-88) from torchvision."""
-    from torchvision import transforms as T
-
-    class RandomApply(nn.Module):
-        def __init__(self, fn, p):
-            super().__init__()
-            self.fn, self.p = fn, p
-
-        def forward(self, x):
-            return x if torch.rand(()) > self.p else self.fn(x)
-
-    is_rgb = channels == 3
-    is_gt1 = channels > 1
-    return nn.Sequential(
-        RandomApply(T.ColorJitter(0.8, 0.8, 0.8, 0.2), p=0.3) if is_rgb else nn.Identity(),
-        T.RandomGrayscale(p=0.2) if is_rgb else nn.Identity(),
-        T.RandomHorizontalFlip(),
-        RandomApply(T.GaussianBlur((3, 3), (1.0, 2.0)), p=0.2) if is_gt1 else nn.Identity(),
-        T.RandomResizedCrop((image_size, image_size)),
-        T.Normalize(mean=torch.tensor([0.485, 0.456, 0.406]), std=torch.tensor([0.229, 0.224, 0.225]))
-        if is_rgb else nn.Identity(),
-    )
+    """The SimCLR-style pipeline the reference builds (visual_ssl.py:59-88): SimCLRAugmentation."""
+    return SimCLRAugmentation(image_size, channels)
 
 
 def _mlp(dim: int, out: int, hidden: int) -> nn.Sequential:

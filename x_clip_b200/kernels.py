@@ -6,6 +6,7 @@ allocates outputs through torch's caching allocator and forwards to one
 """
 from __future__ import annotations
 
+import ctypes
 from typing import Optional
 
 import torch
@@ -748,3 +749,44 @@ def text_embed_bwd(ids, dx, vocab, pos_rows):
     _call(ids, "embed", 0.0, B * (n + 1) * d * 8.0, "xclip_text_embed_bwd", ids.data_ptr(), dx.data_ptr(),
           dtok.data_ptr(), dpos.data_ptr(), dcls.data_ptr(), B, n, d, vocab)
     return dtok, dpos, dcls
+
+
+def augment(x, *, ops=(), factor=(0.0,) * 4, one_minus=(0.0,) * 4, grayscale=False, flip=False,
+            blur_kernel=None, normalize=None, crop, out_size):
+    """The SimCLR augmentation of one call on x f32 [B, C, H, W] -> f32 [B, C, *out_size]
+    (xclip_augment_mean when ops contain contrast, then xclip_augment_apply).  ops: the jitter op ids
+    in order (0 brightness, 1 contrast, 2 saturation, 3 hue); factor / one_minus indexed by op id;
+    blur_kernel: 9 weights of the 3x3 blur or None; normalize: (mean[3], std[3]) or None; crop:
+    (top, left, height, width) inside the image, no larger than out_size (out_h, out_w)."""
+    _need(x, F32, "image")
+    if x.dim() != 4:
+        raise _lib.XClipB200Error(f"augment: image must be [B, C, H, W], got shape {tuple(x.shape)}")
+    x = x.contiguous()
+    B, C, H, W = x.shape
+    p = _lib.AugmentParams()
+    ops = [int(o) for o in ops]
+    if len(ops) > 4:
+        raise _lib.XClipB200Error(f"augment: at most 4 jitter ops, got {ops}")
+    p.ops[:] = ops + [-1] * (4 - len(ops))
+    p.factor[:] = [float(f) for f in factor]
+    p.one_minus[:] = [float(f) for f in one_minus]
+    p.grayscale, p.flip = int(bool(grayscale)), int(bool(flip))
+    if blur_kernel is not None:
+        p.blur = 1
+        p.blur_kernel[:] = [float(w) for w in blur_kernel]
+    if normalize is not None:
+        p.normalize = 1
+        p.mean[:] = [float(m) for m in normalize[0]]
+        p.std[:] = [float(s) for s in normalize[1]]
+    p.top, p.left, p.height, p.width = (int(v) for v in crop)
+    p.out_h, p.out_w = (int(v) for v in out_size)
+    out = torch.empty((B, C, p.out_h, p.out_w), device=x.device, dtype=F32)
+    mean = None
+    if 1 in ops:
+        mean = torch.empty((B,), device=x.device, dtype=F32)
+        _call(x, "augment", 0.0, x.numel() * 4.0 + B * 4.0, "xclip_augment_mean", x.data_ptr(), B, C, H, W,
+              ctypes.addressof(p), mean.data_ptr())
+    nbytes = B * C * p.height * p.width * 4.0 + out.numel() * 4.0
+    _call(x, "augment", 0.0, nbytes, "xclip_augment_apply", x.data_ptr(), B, C, H, W, ctypes.addressof(p),
+          _ptr(mean), out.data_ptr())
+    return out
