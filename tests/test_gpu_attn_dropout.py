@@ -1,4 +1,4 @@
-"""Attention dropout (xclip_attn_dropout_fwd / _bwd, engine.TransformerDropoutFn) on the GPU.
+"""Attention dropout (xclip_attn_dropout_fwd / _bwd, engine.TransformerFn with `drop`) on the GPU.
 
 - The kernels against attn_oracle's fp64 reference fed dropout_oracle's numpy mask, with attn_oracle's
   per-element gates (the multiplier M / (1 - p) enters wherever P meets V or dP).
@@ -184,7 +184,7 @@ def test_attn_dropout_refuses_bad_arguments(cuda_device):
 
 @pytest.mark.parametrize("name", ["d512_mask_causal", "d768_n197"])
 def test_transformer_dropout_fp64(cuda_device, name):
-    """TransformerDropoutFn (depth 2, p = 0.1) against fp64 autograd of the reference block with the
+    """TransformerFn with dropout (depth 2, p = 0.1) against fp64 autograd of the reference block with the
     numpy masks of layers 0 and 1, under BLOCK_GATES."""
     from x_clip_b200 import engine as E
     case = BO.block_case(name, device=cuda_device)
@@ -194,7 +194,7 @@ def test_transformer_dropout_fp64(cuda_device, name):
     x = case["x"].clone().requires_grad_(True)
     cos, sin = case["rot"] if case["rot"] is not None else (None, None)
     drop = ((0.1, 0.1), _seed(SEED, cuda_device))
-    out = E.TransformerDropoutFn.apply(x, case["mask"], H, BO.BLOCK_DEPTH, case["causal"], cos, sin, True, drop, *ws)
+    out = E.TransformerFn.apply(x, case["mask"], H, BO.BLOCK_DEPTH, case["causal"], cos, sin, True, drop, *ws)
     out.backward(case["dout"])
     torch.cuda.synchronize()
     masks = [DO.attn_drop_mul(SEED, B, H, n, L, 0.1, cuda_device) for L in range(BO.BLOCK_DEPTH)]

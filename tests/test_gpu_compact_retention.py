@@ -36,12 +36,9 @@ def _transformer(case, compact, drop=None):
     ws = [w.clone().requires_grad_(True) for w in case["weights"]]
     x = case["x"].clone().requires_grad_(True)
     cos, sin = case["rot"] if case["rot"] is not None else (None, None)
-    args = (x, case["mask"], case["heads"], BO.BLOCK_DEPTH, case["causal"], cos, sin, True)
-    with E._CompactSave(compact):
-        if drop is None:
-            out = E.TransformerFn.apply(*args, *ws)
-        else:
-            out = E.TransformerDropoutFn.apply(*args, drop, *ws)
+    with E._scoped_global("_compact_save", compact):
+        out = E.TransformerFn.apply(x, case["mask"], case["heads"], BO.BLOCK_DEPTH, case["causal"], cos, sin, True,
+                                    drop, *ws)
     out.backward(case["dout"])
     torch.cuda.synchronize()
     return out.detach(), x.grad, [w.grad for w in ws]

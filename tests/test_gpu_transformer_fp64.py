@@ -25,7 +25,7 @@ def _run(case, prefill=None):
             w.grad = p.clone()
     x = case["x"].clone().requires_grad_(True)
     cos, sin = case["rot"] if case["rot"] is not None else (None, None)
-    out = E.TransformerFn.apply(x, case["mask"], case["heads"], BO.BLOCK_DEPTH, case["causal"], cos, sin, True, *ws)
+    out = E.TransformerFn.apply(x, case["mask"], case["heads"], BO.BLOCK_DEPTH, case["causal"], cos, sin, True, None, *ws)
     out.backward(case["dout"])
     torch.cuda.synchronize()
     return out.detach(), x.grad, [w.grad for w in ws]

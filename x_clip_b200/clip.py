@@ -20,7 +20,7 @@ widths that are not 128 * {1..8}, a causal text tower longer than
 128 tokens, rotary + causal together (broken in the reference itself: n+1 angles for n tokens,
 x_clip.py:328) and conv-downsampled image latents.  Attention dropout (`attn_dropout`, 0 <= p <= 1)
 runs inside the attention kernels, with a counter-based mask that a re-encode regenerates exactly
-(engine.TransformerDropoutFn); `ff_dropout` is accepted and, as in the reference's Transformer
+(engine.TransformerFn); `ff_dropout` is accepted and, as in the reference's Transformer
 (x_clip.py:268), not applied.  MLM, SimSiam / SimCLR and the multiview term run through the fast encoders (aux.py);
 with FILIP, the augmented views (`aug_text` / `aug_image`) run every (text view, image view) pair in one
 pair of segment-max passes (filip.FilipLossFn), each text view masked by its own pad pattern.  The similarity-regularisation term
@@ -115,9 +115,8 @@ class Transformer(nn.Module):
     """norm_in -> depth x (attention, feed-forward) -> norm_out, executed by engine.TransformerFn.
 
     Attention dropout is active, as nn.Dropout is, iff the layer's `dropout` module is in training mode
-    and its p > 0, under no_grad as well; it then runs engine.TransformerDropoutFn with one 64-bit seed
-    per call, drawn from the CUDA generator of the input's device (so torch.manual_seed governs the
-    masks).  `forced_dropout_seed` (an int) pins that seed for tests.  `ff_dropout` is accepted and not
+    and its p > 0, under no_grad as well; engine.TransformerFn then gets one 64-bit seed per call, drawn
+    from the CUDA generator of the input's device (so torch.manual_seed governs the masks).  `forced_dropout_seed` (an int) pins that seed for tests.  `ff_dropout` is accepted and not
     applied: the reference's Transformer never hands it to its FeedForward (x_clip.py:268)."""
 
     def __init__(self, dim: int, *, depth: int, dim_head: int = 64, heads: int = 8,
@@ -161,12 +160,9 @@ class Transformer(nn.Module):
             ang = rotary_pos_emb[:, :16].to(device=x.device, dtype=torch.float32)
             cos, sin = ang.cos().contiguous(), ang.sin().contiguous()
         ps = tuple(float(attn.fn.dropout.p) if attn.fn.dropout.training else 0.0 for attn, _ in self.layers)
-        if any(p > 0.0 for p in ps):
-            return E.TransformerDropoutFn.apply(x, mask, self.heads, self.depth, self.causal, cos, sin,
-                                                torch.is_grad_enabled(), (ps, self.dropout_seed(x.device)),
-                                                *self.flat_weights())
+        drop = (ps, self.dropout_seed(x.device)) if any(p > 0.0 for p in ps) else None
         return E.TransformerFn.apply(x, mask, self.heads, self.depth, self.causal, cos, sin,
-                                     torch.is_grad_enabled(), *self.flat_weights())
+                                     torch.is_grad_enabled(), drop, *self.flat_weights())
 
     def dropout_seed(self, device) -> torch.Tensor:
         """int64 [1] on `device`: the Philox key of this call's attention-dropout masks, drawn from the

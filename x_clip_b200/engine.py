@@ -13,6 +13,7 @@ SigLIP's pairwise sigmoid loss (not in the reference) on the same operands and g
 """
 from __future__ import annotations
 
+import contextlib
 from typing import List, Optional
 
 import torch
@@ -28,18 +29,24 @@ LN_EPS = 1e-5   # the reference's fp32 branch (x_clip.py:118); parameters/output
 _scope_cache = None     # dict while a weight_scope() is active, else None
 
 
+def _scoped_cast(key, anchor: torch.Tensor, make):
+    """make(): a cast of the parameter `anchor`, made once per weight_scope() under `key` and made afresh
+    on every call outside one."""
+    if _scope_cache is None:
+        return make()
+    hit = _scope_cache.get(key)
+    if hit is not None and hit[0] is anchor:
+        return hit[1]
+    out = make()
+    _scope_cache[key] = (anchor, out)     # holds the anchor: ids cannot be recycled inside the scope
+    return out
+
+
 def ff_weights(w1: torch.Tensor, w2: torch.Tensor, g4: torch.Tensor):
     """(w1 permuted bf16, w2*g4 bf16, row sums) for the fused feed-forward; shared inside a
     weight_scope() like weight_bf16."""
-    key = ("ff", id(w1), id(w2), id(g4))
-    if _scope_cache is not None:
-        hit = _scope_cache.get(key)
-        if hit is not None and hit[0] is w1:
-            return hit[1]
-    out = K.ff_weights(w1.detach(), w2.detach(), g4.detach())
-    if _scope_cache is not None:
-        _scope_cache[key] = (w1, out)
-    return out
+    return _scoped_cast(("ff", id(w1), id(w2), id(g4)), w1,
+                        lambda: K.ff_weights(w1.detach(), w2.detach(), g4.detach()))
 
 
 def weight_bf16(p: torch.Tensor) -> torch.Tensor:
@@ -51,38 +58,29 @@ def weight_bf16(p: torch.Tensor) -> torch.Tensor:
     the casts they used in `ctx` for their backward (autograd semantics: backward sees the weights
     of its forward).  Only inside an explicit `weight_scope()` - one micro-batched forward or
     backward sweep, during which no optimizer can run - are casts shared between calls."""
-    if _scope_cache is not None:
-        hit = _scope_cache.get(id(p))
-        if hit is not None and hit[0] is p:
-            return hit[1]
-    w = K.cast_bf16(p.detach())
-    if _scope_cache is not None:
-        _scope_cache[id(p)] = (p, w)     # holds p: ids cannot be recycled inside the scope
-    return w
+    return _scoped_cast(id(p), p, lambda: K.cast_bf16(p.detach()))
 
 
-class weight_scope:
-    """Share bf16 weight casts between the encoder calls of ONE sweep over micro-batches.
-    `cache`: continue with the casts of an earlier scope (the backward sweep of a step reuses the
-    forward sweep's - autograd semantics: backward sees the weights of its forward)."""
+@contextlib.contextmanager
+def _scoped_global(name: str, value):
+    """Set the module global `name` (_scope_cache, _compact_save, _accumulate_into_grad) to `value` for
+    the length of a with block, whose value it is."""
+    prev = globals()[name]
+    globals()[name] = value
+    try:
+        yield value
+    finally:
+        globals()[name] = prev
 
-    def __init__(self, cache=None):
-        self.given = cache
 
-    def __enter__(self):
-        global _scope_cache
-        self.prev = _scope_cache
-        if self.given is not None:
-            _scope_cache = self.given
-        elif _scope_cache is None:
-            _scope_cache = {}
-        self.cache = _scope_cache
-        return self
-
-    def __exit__(self, *exc):
-        global _scope_cache
-        _scope_cache = self.prev
-        return False
+def weight_scope(cache=None):
+    """Share bf16 weight casts between the encoder calls of ONE sweep over micro-batches, inside the
+    with block, whose value is the scope's cache; a scope nested in another shares its casts.  `cache`:
+    continue with the casts of an earlier scope (the backward sweep of a step reuses the forward sweep's
+    - autograd semantics: backward sees the weights of its forward)."""
+    if cache is None:
+        cache = {} if _scope_cache is None else _scope_cache
+    return _scoped_global("_scope_cache", cache)
 
 
 def _wgrad(dy: torch.Tensor, x: torch.Tensor) -> torch.Tensor:
@@ -118,44 +116,25 @@ def _grad_target(param: torch.Tensor):
 _compact_save = False
 
 
-class _CompactSave:
-    def __init__(self, flag: bool):
-        self.flag = flag
-
-    def __enter__(self):
-        global _compact_save
-        self.prev = _compact_save
-        _compact_save = self.flag
-        return self
-
-    def __exit__(self, *exc):
-        global _compact_save
-        _compact_save = self.prev
-        return False
-
-
 class TransformerFn(torch.autograd.Function):
     """x[B,n,d] (bf16) -> norm_out(blocks(norm_in(x))) (bf16); mask: bool [B,n] or None.
 
     flat weights = [norm_in.g, norm_out.g] + depth * [g1, wqkv, wo, go, g2, w1, g4, w2].
     causal: the reference's causal mask (x_clip.py:233-236); rot_cos / rot_sin: f32 [n, 16] tables of
     the rotary embedding applied to q, k and v (x_clip.py:221-223) or None.
-    TransformerDropoutFn is the same encoder with attention dropout.
+    drop: dropout on the attention probabilities (x_clip.py:211, :241-243), or None.  drop = (p per layer,
+    seed): seed is an int64 [1] device tensor, the Philox key of every layer's mask
+    (xclip_attn_dropout_fwd; layer L draws with counter word L).  The backward reuses the seed kept in
+    ctx, so it sees the forward's masks; a second forward with the same seed (the re-encode of a
+    micro-batched step, or a forward-only sweep) draws the same masks as well.  A layer with p = 0 runs
+    the plain kernels.
     Saved per token and layer: 21 d bf16 (full), or 7 d under _compact_save.  The pre-norm output xn
     is never saved: the pre-norm's LayerNorm backward emits it for the wqkv weight gradient.
     """
 
     @staticmethod
-    def forward(ctx, x, mask, heads: int, depth: int, causal: bool, rot_cos, rot_sin, need_bwd: bool,
+    def forward(ctx, x, mask, heads: int, depth: int, causal: bool, rot_cos, rot_sin, need_bwd: bool, drop,
                 *weights):
-        return TransformerFn._forward(ctx, x, mask, heads, depth, causal, rot_cos, rot_sin, need_bwd, None, weights)
-
-    @staticmethod
-    def backward(ctx, dout):
-        return TransformerFn._backward(ctx, dout, 8)
-
-    @staticmethod
-    def _forward(ctx, x, mask, heads, depth, causal, rot_cos, rot_sin, need_bwd, drop, weights):
         B, n, d = x.shape
         M = B * n
         scale = 64 ** -0.5
@@ -214,8 +193,7 @@ class TransformerFn(torch.autograd.Function):
         return out.view(B, n, d)
 
     @staticmethod
-    def _backward(ctx, dout, n_args: int):
-        """-> gradients of the n_args leading arguments (dx and Nones) + the weights' gradients"""
+    def backward(ctx, dout):
         B, n, d, heads, depth, scale, causal = ctx.dims
         rot_cos, rot_sin = ctx.rot
         M = B * n
@@ -233,7 +211,7 @@ class TransformerFn(torch.autograd.Function):
         # parameters with requires_grad=False (a frozen tower: adversarial / guidance use) cost no
         # weight-gradient work: their wgrad GEMMs and gain reductions are skipped and None returned.
         # The data-gradient chain reads none of them, so dx is the same either way.
-        wneed = ctx.needs_input_grad[n_args:]
+        wneed = ctx.needs_input_grad[9:]     # after the 9 leading arguments x ... drop
 
         def gain_grad(idx):
             """fp32 accumulator for the gain gradient of weights[idx]: its .grad (in-place mode) or
@@ -312,7 +290,7 @@ class TransformerFn(torch.autograd.Function):
         dg_in, grads[0] = gain_grad(0)
         dx_in = K.layernorm_bwd(dx, x_in, st_in, g_in, dg=dg_in)
         ctx.saved = ctx.wb = ctx.drop = None
-        return (dx_in.view(B, n, d),) + (None,) * (n_args - 1) + tuple(grads)
+        return (dx_in.view(B, n, d),) + (None,) * 8 + tuple(grads)
 
 
 def _attn_dropout(drop, L: int):
@@ -320,25 +298,6 @@ def _attn_dropout(drop, L: int):
     if drop is None or drop[0][L] == 0.0:
         return None
     return drop[0][L], drop[1], L
-
-
-class TransformerDropoutFn(torch.autograd.Function):
-    """TransformerFn with dropout on the attention probabilities (x_clip.py:211, :241-243).
-
-    drop = (p per layer, seed): seed is an int64 [1] device tensor, the Philox key of every layer's
-    mask (xclip_attn_dropout_fwd; layer L draws with counter word L).  The backward reuses the seed
-    kept in ctx, so it sees the forward's masks; a second forward with the same seed (the re-encode of
-    a micro-batched step, or a forward-only sweep) draws the same masks as well.  A layer with p = 0
-    runs the plain kernels."""
-
-    @staticmethod
-    def forward(ctx, x, mask, heads: int, depth: int, causal: bool, rot_cos, rot_sin, need_bwd: bool, drop,
-                *weights):
-        return TransformerFn._forward(ctx, x, mask, heads, depth, causal, rot_cos, rot_sin, need_bwd, drop, weights)
-
-    @staticmethod
-    def backward(ctx, dout):
-        return TransformerFn._backward(ctx, dout, 9)
 
 
 class TextEmbedFn(torch.autograd.Function):
@@ -408,15 +367,7 @@ def patch_weight_bf16(weight: torch.Tensor) -> torch.Tensor:
     ld = K.patch_row_stride(weight.shape[1])
     if ld == weight.shape[1]:
         return weight_bf16(weight)
-    key = ("patch_rows", id(weight))
-    if _scope_cache is not None:
-        hit = _scope_cache.get(key)
-        if hit is not None and hit[0] is weight:
-            return hit[1]
-    w = K.cast_bf16_rows(weight.detach(), ld)
-    if _scope_cache is not None:
-        _scope_cache[key] = (weight, w)
-    return w
+    return _scoped_cast(("patch_rows", id(weight)), weight, lambda: K.cast_bf16_rows(weight.detach(), ld))
 
 
 def _patch_embed_fwd(ctx, patches, index, weight, bias, table, keep_wb: bool):
@@ -825,20 +776,119 @@ def fits_all_full(avail: int, foot: int, rows: List[int], chunk: int, reserve: i
     return avail >= foot * (rest + RETAIN_TRANSIENT_FRAC["full"]) + RETAIN_MARGIN_BYTES + reserve
 
 
-class _InPlaceGradAccumulation:
-    def __init__(self, flag: bool):
-        self.flag = flag
+class RetainPlan:
+    """Which chunks of one micro-batched step keep their activations for backward: `modes[k]` is the save
+    mode of chunk k, "full" / "compact", or None (encoded without saving anything, re-encoded in backward).
 
-    def __enter__(self):
-        global _accumulate_into_grad
-        self.prev = _accumulate_into_grad
-        _accumulate_into_grad = self.flag
-        return self
+    retain: "auto" or an int (the first `retain` chunks); remembered: the modes remembered for this batch
+    and chunk size, or None; mode: RETAIN_MODE; rows: the pairs of every chunk.  "auto" repeats a
+    remembered plan, else it plans: keep the first chunk and measure it, in compact mode when not every
+    chunk fits in full mode, let it go when not even a second chunk fits beside it, and keep each later
+    chunk while the free HBM holds it.  An out-of-memory ends the keeping.  The plan holds no tensors and
+    measures nothing: the step passes it the free HBM (_avail_bytes) exactly where `weighs`,
+    `weighs_compact` and `weighs_release` ask, so every step measures and allocates in the same order."""
 
-    def __exit__(self, *exc):
-        global _accumulate_into_grad
-        _accumulate_into_grad = self.prev
-        return False
+    def __init__(self, retain, remembered, mode, rows: List[int], chunk: int):
+        self.retain, self.remembered, self.forced = retain, remembered, mode
+        self.rows, self.chunk = list(rows), chunk
+        self.planning = retain == "auto" and remembered is None
+        self.mode = mode or "full"      # save mode of the chunks kept from here on
+        self.foot = None                # bytes one full-size chunk holds in that mode, once measured
+        self.reserve = 0                # HBM left to the loss (FILIP: filip.step_reserve_bytes)
+        self.oom_fallbacks = 0
+        self.modes = []
+
+    @property
+    def weighs(self) -> bool:
+        """Whether mode_for weighs the free HBM: after the first chunk of a planning step, until an OOM."""
+        return self.planning and not self.oom_fallbacks and self.foot is not None
+
+    def mode_for(self, k: int, avail=None):
+        """The save mode chunk k is encoded in (None: not kept); `avail` when `weighs`."""
+        if self.weighs:
+            keep = avail >= retain_need_bytes(self.foot, self.rows[k], self.chunk, self.mode, self.reserve)
+            m = self.mode if keep else None
+        elif self.oom_fallbacks:
+            m = None
+        elif self.retain == "auto" and self.remembered is not None:
+            m = self.remembered[k]
+        elif self.retain != "auto":
+            m = self.mode if k < int(self.retain) else None
+        else:                            # the first chunk of a planning step: kept and measured
+            m = self.mode
+        self.modes.append(m)
+        return m
+
+    def measured(self, nbytes: int, reserve: int):
+        """The footprint of the first chunk kept (again, after `compact`), and the loss's reserve."""
+        self.foot, self.reserve = nbytes, reserve
+
+    @property
+    def weighs_compact(self) -> bool:
+        """Whether `compact` weighs the free HBM: on a planning step of several chunks, no mode forced."""
+        return self.planning and self.forced is None and len(self.rows) > 1
+
+    def compact(self, avail: int) -> bool:
+        """Whether the first chunk is encoded again in compact mode: not every chunk fits in full mode."""
+        if fits_all_full(avail, self.foot, self.rows, self.chunk, self.reserve):
+            return False
+        self.mode = self.modes[-1] = "compact"
+        return True
+
+    def out_of_memory(self):
+        """The latest chunk's kept encode ran out of memory: it and every later chunk are re-encoded."""
+        self.modes[-1] = None
+        self.oom_fallbacks += 1
+
+    def weighs_release(self, k: int) -> bool:
+        """Whether `release` weighs the free HBM after chunk k: the kept first of several planned chunks."""
+        return k == 0 and self.planning and len(self.rows) > 1 and self.modes[0] is not None
+
+    def release(self, avail: int) -> bool:
+        """Whether the first chunk is let go: not even a second full-size chunk fits beside it."""
+        if avail >= retain_need_bytes(self.foot, self.chunk, self.chunk, self.mode, self.reserve):
+            return False
+        self.modes[0] = None
+        return True
+
+    @property
+    def remembers(self) -> bool:
+        """Whether `modes` is remembered: a planning step's, or a remembered plan cut by an out-of-memory."""
+        return self.planning or (self.oom_fallbacks > 0 and self.remembered is not None)
+
+
+class _Chunk:
+    """One chunk [s, e) of the micro-batched step: the RNG state its encode starts from, its save mode
+    (None: re-encoded in backward), its kept outputs (`live`) and image leaf, and `rows`, its rows
+    [start, end) in each full-batch leaf (the MLM leaf has n_sel rows)."""
+
+    def __init__(self, s: int, e: int, rng):
+        self.s, self.e, self.rng = s, e, rng
+        self.mode = self.live = self.img = self.rows = None
+
+
+def _encode_kept(clip, text, image, text_mask, aux, s: int, e: int, mode: str):
+    """(outputs, ops, image leaf, bytes) of chunk [s, e) encoded with its activations kept in save mode
+    `mode`, or None when it runs out of memory."""
+    dev = text.device
+    before = torch.cuda.memory_allocated(dev)
+    img_k = image[s:e].detach().requires_grad_(True) if image.requires_grad else None
+    try:
+        with torch.enable_grad(), _scoped_global("_compact_save", mode == "compact"):
+            z, ops = _chunk_passes(clip, text, image, text_mask, aux, s, e, img_k)
+    except torch.OutOfMemoryError:
+        return None
+    return z, ops, img_k, max(torch.cuda.memory_allocated(dev) - before, 1)
+
+
+def _loss_reserve(clip, B: int, z) -> int:
+    """HBM the plan leaves to the loss, from the outputs z of the first chunk kept: with FILIP
+    filip.step_reserve_bytes for its token latents, else 0."""
+    if not clip.use_all_token_embeds:
+        return 0
+    from .filip import step_reserve_bytes
+    world = D_.world()[1] if clip.requires_all_gather else 1
+    return step_reserve_bytes(B, world * B, z[0].shape[1], z[1].shape[1], z[0].shape[2], len(z) == 4)
 
 
 def _chunk_passes(clip, text, image, text_mask, aux, s: int, e: int, img_k=None):
@@ -901,13 +951,12 @@ class ChunkedClipLossFn(torch.autograd.Function):
          logit_bias as one more leaf beside the temperature
       3. in backward: d loss / d latents, then back-propagate the matching slice of the latent
          gradient through every chunk's encoders.
-    Memory plan: a chunk's saved activations are KEPT from step 1 for as many chunks as
-    the GPU's HBM holds (80 GB on an H100) (`retain`: "auto" measures the first chunk's footprint and plans against
-    the free memory; an int fixes the count; 0 = none); only the remaining chunks are encoded
-    without saving anything and re-encoded in step 3 (RNG replayed for PatchDropout).  Retained
-    chunks cost no extra flops in full mode; compact ones (a third of the memory, chosen by "auto" when
-    not every chunk fits in full mode, see RETAIN_MODE) rebuild one LayerNorm and the feed-forward's
-    up-projection per layer in backward; each re-encoded chunk costs one extra encoder forward.
+    Memory plan (RetainPlan, from `retain`): a chunk's saved activations are KEPT from step 1 for as
+    many chunks as the GPU's HBM holds (80 GB on an H100); only the remaining chunks are encoded without
+    saving anything and re-encoded in step 3 (RNG replayed for PatchDropout).  Retained chunks cost no
+    extra flops in full mode; compact ones (a third of the memory) rebuild one LayerNorm and the
+    feed-forward's up-projection per layer in backward; each re-encoded chunk costs one extra encoder
+    forward.
     An image that wants a gradient enters every chunk's encoder as a detached per-chunk leaf; backward
     collects the leaves' gradients into d loss / d image, so the outer graph (a generator, an
     augmentation) is only ever entered by autograd itself, after this backward returns.
@@ -926,106 +975,52 @@ class ChunkedClipLossFn(torch.autograd.Function):
         B = text.shape[0]
         dev = text.device
         bounds = [(s, min(s + chunk, B)) for s in range(0, B, chunk)]
-        rng_states, zs, opss, kept, lives, targets = [], [], [], [], [], []
-        want_dimage = image.requires_grad
-        img_leaves = []                               # per retained chunk: its image leaf (or None)
-        foot = None                                   # bytes of one retained chunk's activations
-        reserve = 0                                   # HBM left to the loss (FILIP: filip.step_reserve_bytes)
-        filip = clip.use_all_token_embeds
         # "auto" plans ONCE per (batch, chunk size): the first step measures and decides, later steps
         # repeat its decision - the same tensors are then allocated in the same order every step, which
         # is what keeps torch's caching allocator free of fragmentation this close to the HBM limit
         plans = clip.__dict__.setdefault("_retain_plans", {})
         plan_key = (B, chunk, str(dev))
-        planned = retain == "auto" and plan_key not in plans
-        keep_mask = None                              # a remembered plan: which chunks stay resident
-        if retain == "auto" and not planned:
-            keep_mask = plans[plan_key]
-        oom_fallbacks = 0
-        # save mode of the kept chunks: an int plan keeps full chunks; "auto" measures its first chunk in
-        # full mode and keeps it that way only when every chunk fits so (fits_all_full)
-        mode = RETAIN_MODE or "full"
-
-        def keep_chunk(k, s, e):
-            """The save mode chunk k keeps its activations in, or None: the remembered plan's choice, the
-            first `retain` chunks of an int plan, or ("auto") whether the free HBM holds one more chunk of
-            its size."""
-            if keep_mask is not None:
-                return keep_mask[k]
-            if retain != "auto":
-                return mode if k < int(retain) else None
-            if foot is None:                          # first chunk: keep it, measure it
-                return mode
-            return mode if _avail_bytes(dev) >= retain_need_bytes(foot, e - s, chunk, mode, reserve) else None
-
-        def encode_kept(s, e, m):
-            """(latents, ops, image leaf, bytes) of chunk [s, e) encoded with its activations kept in save
-            mode m, or None when it runs out of memory"""
-            before = torch.cuda.memory_allocated(dev)
-            img_k = image[s:e].detach().requires_grad_(True) if want_dimage else None
-            try:
-                with torch.enable_grad(), _CompactSave(m == "compact"):
-                    z, ops = _chunk_passes(clip, text, image, text_mask, aux, s, e, img_k)
-            except torch.OutOfMemoryError:
-                return None
-            return z, ops, img_k, max(torch.cuda.memory_allocated(dev) - before, 1)
-
-        with torch.no_grad(), weight_scope() as wscope:
+        plan = RetainPlan(retain, plans.get(plan_key), RETAIN_MODE, [e - s for s, e in bounds], chunk)
+        chunks, zs, opss, targets = [], [], [], []
+        with torch.no_grad(), weight_scope() as weight_casts:
             for k, (s, e) in enumerate(bounds):
-                rng_states.append(torch.cuda.get_rng_state(dev))
-                z = live = img_k = None
-                m = keep_chunk(k, s, e)
-                if m is not None:
-                    got = encode_kept(s, e, m)
-                    if got is not None and foot is None:
-                        foot = got[3]
-                        if filip:
-                            from .filip import step_reserve_bytes
-                            world = D_.world()[1] if clip.requires_all_gather else 1
-                            z0 = got[0]
-                            reserve = step_reserve_bytes(B, world * B, z0[0].shape[1], z0[1].shape[1],
-                                                         z0[0].shape[2], len(z0) == 4)
-                            del z0
-                        if planned and RETAIN_MODE is None and len(bounds) > 1 and not fits_all_full(
-                                _avail_bytes(dev), foot, [b - a for a, b in bounds], chunk, reserve):
-                            # not every chunk fits in full mode: measure the first one again in compact mode
-                            got = None
-                            torch.cuda.set_rng_state(rng_states[-1], dev)
-                            mode = m = "compact"
-                            got = encode_kept(s, e, m)
-                            if got is not None:
-                                foot = got[3]
-                    if got is None:
-                        # out of memory - the plan was too optimistic (a fragmented cache, memory taken by
-                        # someone else since the estimate): this chunk and all later ones are re-encoded in
-                        # backward (an int plan: nothing further is kept); free the cache, replay the RNG
-                        retain, keep_mask = 0, None
-                        oom_fallbacks += 1
-                        torch.cuda.empty_cache()
-                        torch.cuda.set_rng_state(rng_states[-1], dev)
-                    else:
-                        z, ops, img_k, _ = got
-                        del got
-                if z is None:                         # not kept: encoded without saving anything
+                c = _Chunk(s, e, torch.cuda.get_rng_state(dev))
+                chunks.append(c)
+                mode = plan.mode_for(k, _avail_bytes(dev) if plan.weighs else None)
+                got = None if mode is None else _encode_kept(clip, text, image, text_mask, aux, s, e, mode)
+                if got is not None and plan.foot is None:
+                    plan.measured(got[3], _loss_reserve(clip, B, got[0]))
+                    if plan.weighs_compact and plan.compact(_avail_bytes(dev)):
+                        got = None                    # frees the full-mode activations first
+                        torch.cuda.set_rng_state(c.rng, dev)
+                        got = _encode_kept(clip, text, image, text_mask, aux, s, e, plan.mode)
+                        if got is not None:
+                            plan.measured(got[3], plan.reserve)
+                if mode is not None and got is None:
+                    # out of memory - the plan was too optimistic (a fragmented cache, memory taken by
+                    # someone else since the estimate): free the cache, replay the RNG
+                    plan.out_of_memory()
+                    torch.cuda.empty_cache()
+                    torch.cuda.set_rng_state(c.rng, dev)
+                if got is None:                       # not kept: encoded without saving anything
                     z, ops = _chunk_passes(clip, text, image, text_mask, aux, s, e)
                 else:
-                    live = list(z)
-                    if k == 0 and planned and len(bounds) > 1 and \
-                            _avail_bytes(dev) < retain_need_bytes(foot, chunk, chunk, m, reserve):
-                        live = None                   # not even a second live chunk fits beside it: let it go
+                    z, ops, c.img, _ = got
+                    del got
+                    if plan.weighs_release(k) and plan.release(_avail_bytes(dev)):
+                        c.img = None
+                    else:
+                        c.live = list(z)
                     z = [t.detach() for t in z]
-                kept.append(m if live is not None else None)
-                lives.append(live)
-                img_leaves.append(img_k if live is not None else None)
+                c.mode = plan.modes[k]
                 zs.append(z)
                 opss.append(ops)
                 if aux is not None and aux["ssl_targets"]:
                     targets.append(_chunk_targets(aux, s, e))
-        # rows [start, end) of every chunk in each full-batch leaf (the MLM leaf has n_sel rows)
-        row_bounds, offs = [], [0] * len(zs[0])
-        for z in zs:
-            row_bounds.append([(offs[j], offs[j] + t.shape[0]) for j, t in enumerate(z)])
-            offs = [b for _, b in row_bounds[-1]]
+        offs = [0] * len(zs[0])
+        for c, z in zip(chunks, zs):
+            c.rows = [(a, a + t.shape[0]) for a, t in zip(offs, z)]
+            offs = [b for _, b in c.rows]
         nleaves = len(zs[0])
         nsets = len(opss[0])
         leaves = [torch.cat([z[j] for z in zs]).detach().requires_grad_(True) for j in range(nleaves)]
@@ -1034,31 +1029,28 @@ class ChunkedClipLossFn(torch.autograd.Function):
         del zs, opss
         temp_leaf = temperature.detach().requires_grad_(True)
         bias_leaf = None if logit_bias is None else logit_bias.detach().requires_grad_(True)
-        filip_stats = {} if filip else None
+        filip_stats = {} if clip.use_all_token_embeds else None
         with torch.enable_grad():
             mlm_loss, ssl_loss = _aux_losses(clip, aux, leaves[nsets:], targets) if aux is not None else (None, None)
             loss = clip._loss(leaves[:nsets], ops_all, text_mask, temp_leaf, bias_leaf, mlm=mlm_loss, ssl=ssl_loss,
                               filip_stats=filip_stats)
         del targets
-        ctx.clip, ctx.inputs = clip, (text, image, text_mask)
-        ctx.bounds, ctx.rng_states, ctx.kept = bounds, rng_states, lives
-        ctx.aux, ctx.row_bounds = aux, row_bounds
-        ctx.img_leaves = img_leaves if want_dimage else None
+        ctx.clip, ctx.inputs, ctx.chunks, ctx.aux = clip, (text, image, text_mask), chunks, aux
         ctx.graph = (loss, leaves, temp_leaf, bias_leaf)
-        ctx.weight_casts = wscope.cache
-        n_kept = sum(m is not None for m in kept)
-        if planned or (oom_fallbacks and plan_key in plans):
-            plans[plan_key] = kept                    # WHICH chunks stay resident, in which save mode
+        ctx.weight_casts = weight_casts
+        if plan.remembers:
+            plans[plan_key] = plan.modes              # WHICH chunks stay resident, in which save mode
         passes = ["contrastive"]
         if aux is not None:
             passes += (["mlm"] if aux["mlm"] is not None else []) + (["view1", "view2"] if aux["ssl"] is not None else [])
-        clip.last_step_plan = dict(chunks=len(bounds), retained=n_kept, chunk_activation_bytes=foot,
-                                   oom_fallbacks=oom_fallbacks, passes=passes,
-                                   retained_chunks=[k for k, m in enumerate(kept) if m is not None],
-                                   compact_chunks=[k for k, m in enumerate(kept) if m == "compact"])
-        if filip:
+        clip.last_step_plan = dict(chunks=len(bounds), retained=sum(m is not None for m in plan.modes),
+                                   chunk_activation_bytes=plan.foot, oom_fallbacks=plan.oom_fallbacks,
+                                   passes=passes,
+                                   retained_chunks=[k for k, m in enumerate(plan.modes) if m is not None],
+                                   compact_chunks=[k for k, m in enumerate(plan.modes) if m == "compact"])
+        if filip_stats is not None:
             # rows of both FILIP passes whose argmax was saved / will be recomputed in backward
-            clip.last_step_plan.update(filip=filip_stats, loss_reserve_bytes=reserve)
+            clip.last_step_plan.update(filip=filip_stats, loss_reserve_bytes=plan.reserve)
         return loss.detach()
 
     @staticmethod
@@ -1071,43 +1063,37 @@ class ChunkedClipLossFn(torch.autograd.Function):
         dz = [l.grad for l in leaves]
         dev = text.device
         keep_state = torch.cuda.get_rng_state(dev)
-        kept = ctx.kept
-        dimage = torch.empty_like(image) if ctx.img_leaves is not None else None
+        dimage = torch.empty_like(image) if image.requires_grad else None
         # retained chunks first: their backward releases HBM before any chunk is re-encoded
-        order = [k for k in range(len(ctx.bounds)) if kept[k] is not None] + \
-                [k for k in range(len(ctx.bounds)) if kept[k] is None]
+        order = [c for c in ctx.chunks if c.mode is not None] + [c for c in ctx.chunks if c.mode is None]
         with weight_scope(ctx.weight_casts):
-            for pos, k in enumerate(order):
-                s, e = ctx.bounds[k]
+            for pos, c in enumerate(order):
+                last = pos == len(order) - 1
                 # parameter gradients accumulate over the chunks; gradient-sync hooks (GradSync)
                 # must see a parameter ONCE per step, with its complete gradient: every chunk but
                 # the last one processed runs with the hooks deferred (the DDP no_sync convention)
-                with torch.enable_grad(), D_.defer_grad_sync(pos != len(order) - 1), \
-                        _InPlaceGradAccumulation(INPLACE_GRAD_ACCUMULATION and pos != len(order) - 1):
-                    img_k = None
-                    if kept[k] is not None:
-                        z, kept[k] = kept[k], None
-                        if dimage is not None:
-                            img_k, ctx.img_leaves[k] = ctx.img_leaves[k], None
+                with torch.enable_grad(), D_.defer_grad_sync(not last), \
+                        _scoped_global("_accumulate_into_grad", INPLACE_GRAD_ACCUMULATION and not last):
+                    if c.mode is not None:
+                        z, img_k, c.live, c.img = c.live, c.img, None, None
                     else:
-                        torch.cuda.set_rng_state(ctx.rng_states[k], dev)
-                        if dimage is not None:
-                            img_k = image[s:e].detach().requires_grad_(True)
-                        z, _ = _chunk_passes(clip, text, image, text_mask, ctx.aux, s, e, img_k)
+                        torch.cuda.set_rng_state(c.rng, dev)
+                        img_k = image[c.s:c.e].detach().requires_grad_(True) if dimage is not None else None
+                        z, _ = _chunk_passes(clip, text, image, text_mask, ctx.aux, c.s, c.e, img_k)
                     # accumulates into .grad; an output with no gradient or no rows in this chunk is skipped
-                    pairs = [(t, dz[j][a:b]) for j, (t, (a, b)) in enumerate(zip(z, ctx.row_bounds[k]))
+                    pairs = [(t, dz[j][a:b]) for j, (t, (a, b)) in enumerate(zip(z, c.rows))
                              if dz[j] is not None and b > a and t.requires_grad]
                     if pairs:
                         torch.autograd.backward([t for t, _ in pairs], [d for _, d in pairs])
                     del z, pairs
                     if img_k is not None:
                         if img_k.grad is None:
-                            dimage[s:e].zero_()
+                            dimage[c.s:c.e].zero_()
                         else:
-                            dimage[s:e].copy_(img_k.grad)
+                            dimage[c.s:c.e].copy_(img_k.grad)
                         del img_k
         torch.cuda.set_rng_state(keep_state, dev)
-        ctx.graph = ctx.inputs = ctx.kept = ctx.weight_casts = ctx.img_leaves = ctx.aux = None
+        ctx.graph = ctx.inputs = ctx.chunks = ctx.weight_casts = ctx.aux = None
         grads = (None, None, dimage, None, None, temp_leaf.grad, None, None,
                  None if bias_leaf is None else bias_leaf.grad)
         return grads[:len(ctx.needs_input_grad)]
