@@ -115,6 +115,13 @@ def ff_permute(w1: torch.Tensor) -> torch.Tensor:
     return torch.cat([v, g], dim=1).reshape(8 * d, d)
 
 
+def ff_unpermute(w1p: torch.Tensor) -> torch.Tensor:
+    """Inverse of ff_permute: [value rows | gate rows] from the tile order of xclip_ff_permute_cast."""
+    d = w1p.shape[1]
+    t = w1p.view(-1, 128, d)
+    return torch.cat([t[:, :64].reshape(4 * d, d), t[:, 64:].reshape(4 * d, d)])
+
+
 def ff_forward64(x, w1b, w2, g4, eps=LN_EPS):
     """fp64 restatement of x_clip.py:180-199 (value first, gate second): -> (u, hp, y = LN(hp) g4 W2^T)."""
     u = x.double() @ w1b.double().t()

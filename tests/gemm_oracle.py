@@ -17,6 +17,14 @@ at most 0.42 (the fp32 additions), and bf16 outputs 0.996, which is the bf16 rou
 (a value just above a power of two).  GAMMA keeps that headroom; every bite of
 test_gemm_edges_gates.py holds with it.
 
+GAMMA does not hold for long k-block chains: the tensor cores do not round the fp32 accumulation to
+nearest, so its error grows with the MMAs of a chain.  At the training step's shapes a latent gradient
+(128 k-blocks, one large term early in many rows) erred by 4.1 x GAMMA S, a weight gradient of 1568
+k-blocks by 1.8 x.  gemm_gate therefore takes, where given, the larger of GAMMA S and chain_bound: two
+ulp per MMA of the running partial sum of the element's own chain (chain_sums64).  That bound follows
+the data: with products of both signs the running sum grows like the square root of the chain, and a
+missing or doubled k-block still spans many gates (test_gemm_edges_gates.py).
+
 Operands have rows of A and rows of B (the output's columns) scaled over three orders of magnitude,
 so output tiles of small values exist and their gates are small with them.
 """
@@ -153,9 +161,52 @@ def abs_sum64(a, b, a_major=0, b_major=0):
     return logical(a, a_major).abs() @ logical(b, b_major).abs().t()
 
 
+# One wgmma (k = 16 for bf16) adds its 16 products into the fp32 accumulator without rounding to
+# nearest: at most two ulp, 2^-22 relative, of the larger of the running sum and the products' magnitude.
+MMA_ULP = 2.0 ** -22
+
+
+def _kslice(t, major: int, k0: int, k1: int):
+    return t[:, k0:k1] if major == 0 else t[k0:k1]
+
+
+def chain_sums64(a, b, a_major=0, b_major=0, ranges=None, k_chunk=8192):
+    """fp64 (A B^T, S = |A| |B|^T, P) of the stored operands, P the sum over every 64-wide k-block b of
+    |P_b|, the running partial sum of its split's chain after block b (ranges: the k-block ranges of
+    the splits, split_ranges; None: one chain).  Converted to fp64 k_chunk columns of K at a time."""
+    K = a.shape[1] if a_major == 0 else a.shape[0]
+    starts = {0} if ranges is None else {r[0] for r in ranges}
+    acc = S = P = run = None
+    for k0 in range(0, K, k_chunk):
+        k1 = min(K, k0 + k_chunk)
+        A, B = logical(_kslice(a, a_major, k0, k1), a_major), logical(_kslice(b, b_major, k0, k1), b_major)
+        Aa, Ba = A.abs(), B.abs()
+        for j0 in range(0, k1 - k0, BLOCK_K):
+            j1 = min(k1 - k0, j0 + BLOCK_K)
+            p = A[:, j0:j1] @ B[:, j0:j1].t()
+            s = Aa[:, j0:j1] @ Ba[:, j0:j1].t()
+            if acc is None:
+                acc, S, P = p.clone(), s, torch.zeros_like(p)
+            else:
+                acc += p
+                S += s
+            run = p if (k0 + j0) // BLOCK_K in starts else run + p
+            P += run.abs()
+    return acc, S, P
+
+
+def chain_bound(S, P):
+    """Per-element bound on the accumulation error of the k-block chains: MMA_ULP (4 P + 5 S).  Within
+    k-block b the four MMAs see running sums of at most |P_b| + s_b (s_b its share of S), so the chain
+    adds at most MMA_ULP (4 sum_b (|P_b| + s_b) + S).  The running sum, not S, carries the bound: with products
+    of both signs it grows like the square root of the chain and one k-block stays visible."""
+    return MMA_ULP * (4.0 * P + 5.0 * S)
+
+
 def gemm_gate(a, b, a_major=0, b_major=0, alpha=1.0, bias=None, residual=None, res_rows=None, prefill=None,
-              bf16_out=False, splits=1, ref=None, S=None):
-    """Per-element gate of the GEMM output (see the module docstring)."""
+              bf16_out=False, splits=1, ref=None, S=None, P=None):
+    """Per-element gate of the GEMM output (see the module docstring).  With P (chain_sums64) the
+    accumulation term is the larger of GAMMA S and chain_bound(S, P)."""
     if S is None:
         S = abs_sum64(a, b, a_major, b_major)
     terms = abs(alpha) * S
@@ -165,7 +216,8 @@ def gemm_gate(a, b, a_major=0, b_major=0, alpha=1.0, bias=None, residual=None, r
         terms = terms + residual.double().abs()[res_rows]
     if prefill is not None:
         terms = terms + prefill.double().abs()
-    gate = GAMMA * abs(alpha) * S + ADD_ULP * (splits + 2) * terms
+    acc = GAMMA * S if P is None else torch.maximum(GAMMA * S, chain_bound(S, P))
+    gate = abs(alpha) * acc + ADD_ULP * (splits + 2) * terms
     if bf16_out:
         if ref is None:
             ref = gemm64(a, b, a_major, b_major, alpha, bias, residual, res_rows, prefill)
@@ -243,6 +295,14 @@ def patch_embed_case(B: int, n: int, k: int, patch_dim: int, d: int, seed: int =
     table = torch.randn(n, d, generator=gen)
     dy = (torch.randn(B * k, d, generator=gen) * _scales(B * k, gen)).bfloat16()
     return dict(keep=keep, patches=patches, w=w, bias=bias, table=table, dy=dy)
+
+
+def patchify64(img, p):
+    """[B, C, H, W] -> [B, (H/p)(W/p), p p C] patch rows in the reference's (p1 p2 c) order, in the
+    dtype of img (exact: a permutation)."""
+    b, c, H, W = img.shape
+    x = img.view(b, c, H // p, p, W // p, p).permute(0, 2, 4, 3, 5, 1)
+    return x.reshape(b, (H // p) * (W // p), p * p * c)
 
 
 # --------------------------------------------------------------------------- AdamW

@@ -149,19 +149,13 @@ def test_scatter_colsum_strided(cuda_device, rows, d):
     BO.check(f"colsum_rows{rows}_d{d}", col, col0.double() + s.sum(0), GO.red_gate(col0.double().abs() + s.abs().sum(0)))
 
 
-def _ref_patchify(img, p):
-    b, c, H, W = img.shape
-    x = img.view(b, c, H // p, p, W // p, p).permute(0, 2, 4, 3, 5, 1)
-    return x.reshape(b, (H // p) * (W // p), p * p * c)
-
-
 @pytest.mark.parametrize("B,C,S,p", [(2, 1, 64, 8), (3, 1, 48, 16), (2, 3, 64, 8), (2, 3, 224, 16)])
 def test_patchify_gather_exact(cuda_device, B, C, S, p):
     from x_clip_b200 import kernels as K
     g = torch.Generator().manual_seed(B * S + C + p)
     img = torch.randn(B, C, S, S, generator=g)
     n = (S // p) ** 2
-    ref = _ref_patchify(img, p)
+    ref = GO.patchify64(img, p)
     out = K.patchify_gather(img.to(cuda_device), p)
     keep = torch.stack([torch.randperm(n, generator=g)[: max(1, n // 2)] for _ in range(B)])
     outk = K.patchify_gather(img.to(cuda_device), p, keep.to(cuda_device))

@@ -11,7 +11,7 @@ Error budget, with temp = exp(temperature) as the kernels receive it (fp32):
     against the bf16 operands themselves only the fp32 accumulation remains);
   - lse / pos inherit it, plus the fp32 rounding and the approximate exp2 / log2 of the log-sum-exp;
   - g = bf16(temp * gscale * (...)): each exp term carries the logit error as a relative error, plus
-    the exp2 argument's fp32 rounding and ex2.approx (_exp_rel), then one bf16 rounding (at most 2^-8
+    the exp2 argument's fp32 rounding and ex2.approx (nce_oracle.exp_rel), then one bf16 rounding (at most 2^-8
     relative; gated at BF16_REL = 2^-7);
   - d temperature = sum g * s is gated against the magnitudes of its terms, not against |d temperature|:
     the terms cancel.
@@ -22,14 +22,16 @@ import math
 import pytest
 import torch
 
+from nce_oracle import LOGIT_GATE
+from nce_oracle import check_bwd_rows as _check_bwd_rows
+from nce_oracle import dtemp_gate as _dtemp_gate
+from nce_oracle import lse_gate as _lse_gate
+from nce_oracle import ref_rows as _ref_rows
 from test_gpu_filip import _report_peak, _start_peak
 
 pytestmark = pytest.mark.gpu
 
 BF16, F32, F64 = torch.bfloat16, torch.float32, torch.float64
-LN_1E20 = math.log(1e-20)
-LOGIT_GATE = 2.0 ** -16
-BF16_REL = 2.0 ** -7                    # bf16 keeps 8 significant bits: one rounding <= 2^-8 relative
 BLOCK_ELEMS = 1 << 24                   # fp64 elements per [rows, C] reference chunk (128 MiB)
 
 
@@ -93,30 +95,6 @@ def _ops(n, D, dev, seed):
     return zrow, zcol
 
 
-def _ref_rows(s, first_pos, dcl):
-    """fp64 (lse, pos) of logit rows s [r, C] whose row i has its positive at column first_pos + i.
-    An empty DCL denominator (C == 1) gives the reference's ln(1e-20)."""
-    r = s.shape[0]
-    rows = torch.arange(r, device=s.device)
-    pos = s[rows, rows + first_pos]
-    if dcl:
-        s = s.clone()
-        s[rows, rows + first_pos] = -math.inf
-    lse = torch.logsumexp(s, dim=1)
-    return torch.where(torch.isinf(lse), LN_1E20, lse), pos
-
-
-def _lse_gate(temp, ref_lse):
-    # logit error, plus fp32 rounding and exp2 / log2 approximations of the log-sum-exp
-    return temp * LOGIT_GATE + 2.0 ** -20 * (1.0 + ref_lse.abs())
-
-
-def _exp_rel(temp):
-    """Relative error of one exp term of g: the logit error temp * 2^-16 as a relative error of
-    exp, with 2x headroom, plus the exp2 argument's fp32 rounding and ex2.approx (2^-18)."""
-    return temp * 2.0 * LOGIT_GATE + 2.0 ** -18
-
-
 COLS = [1, 7, 31, 32, 33, 127, 128, 129, 255, 256, 257, 1000, 4095, 4096]
 DIMS = [256, 512, 768, 1024, 72]
 TEMPS = [0.1, 1.0, math.e, 1 / 0.07, 100.0]
@@ -175,48 +153,6 @@ def test_nce_fwd_matches_fp64(cuda_device, C, D, dcl):
         del s_unit
     print(f"nce_fwd C={C} D={D} dcl={dcl}: error/gate lse {worst['lse']:.3f} pos {worst['pos']:.3f} "
           f"loss {worst['loss']:.3f}")
-
-
-def _check_bwd_rows(g, s, first_pos, dcl, lse_row, lse_col, w, gs, temp):
-    """g [r, >= C] (bf16 temp * g from xclip_nce_bwd) against fp64 for logit rows s [r, C] (temp
-    included) with the kernel's own lse_row [r] / lse_col [C].  Returns (max error / gate, sum g s,
-    sum |g| |s|, sum |g|) of this block, |g| the magnitude of an element's terms.  The pad columns must be exactly zero; under DCL each positive
-    must be exactly bf16(fp32(-w_diag * gs) * temp)."""
-    w_row, w_col, w_diag = w
-    r, C = s.shape
-    rows = torch.arange(r, device=s.device)
-    ex = torch.zeros_like(s)
-    if w_row:
-        ex += w_row * torch.exp(s - lse_row.double()[:, None])
-    if w_col:
-        ex += w_col * torch.exp(s - lse_col.double()[None, :])
-    if dcl:
-        ex[rows, rows + first_pos] = 0.0
-    g64 = gs * ex
-    g64[rows, rows + first_pos] -= gs * w_diag
-    ref = temp * g64
-    gate = BF16_REL * ref.abs() + temp * gs * ex * _exp_rel(temp) + temp * gs * 2.0 ** -120
-    got = g[:, :C].double()
-    err = ((got - ref).abs() / gate).max().item()
-    assert bool((g[:, C:] == 0).all()), "pad columns of g are not zero"
-    if dcl:
-        want = ((torch.tensor([-w_diag], dtype=F32) * torch.tensor([gs], dtype=F32))
-                * torch.tensor([temp], dtype=F32)).to(BF16).to(s.device)
-        assert bool((g[rows, rows + first_pos] == want).all()), "DCL positives are not exactly -w_diag"
-    # magnitude of each element's terms (its exp terms and the positive's -w_diag cancel at the diagonal)
-    mag = gs * ex.abs()
-    mag[rows, rows + first_pos] += gs * abs(w_diag)
-    return err, (g64 * s).sum().item(), (mag * s.abs()).sum().item(), mag.sum().item()
-
-
-def _dtemp_gate(temp, abs_gs, abs_g, R, C):
-    """d temperature = sum g s, gated against the magnitudes of its terms (sum |g| |s| and sum |g| with
-    |g| the sum of an element's term magnitudes): the logit error through sum |g|, the exp error through
-    sum |g| |s|, and the fp32 summation - 256 sequential terms per thread, a 32-lane tree, one atomic per
-    warp and column block."""
-    nblk = (C + 255) // 256 if C >= 256 else (C + 127) // 128
-    n_add = 256 + 5 + -(-R // 32) * nblk
-    return abs_g * temp * LOGIT_GATE + abs_gs * (_exp_rel(temp) + n_add * 2.0 ** -24)
 
 
 WEIGHTS = [(1.0, 1.0, 2.0), (1.0, 0.0, 1.0), (0.0, 1.0, 1.0)]
