@@ -7,12 +7,15 @@ of every other argument: majors, accumulate, bias / residual mode, causal, mask,
 need_u, ...) runs the real call, is checked against an fp64 reference computed on the GPU in row
 chunks, and prints `GATE <wrapper>[<signature>]<output> <ratio>`; later calls of the signature run
 unchecked.  Buffers a call writes in place or accumulates into are cloned before it runs, so the
-reference starts from what the kernel started from.  Wrappers with no entry in CHECKS are counted in
-`unchecked`; NOT_REACHED lists, with a reason, the wrappers no bench workload calls.
+reference starts from what the kernel started from.  Every wrapper that launches a kernel has an entry
+in CHECKS and every variant of it is checked; a call of a wrapper with no entry is counted in
+`unchecked`.
 
 The references are the existing oracles: gemm_oracle (gemm64, gemm_gate, text_embed_bwd64,
 patchify64, adamw64), block_oracle (LayerNorm and feed-forward stages, rotate64), attn_oracle
-(attn_ref64) and nce_oracle.  The per-element gates are theirs.  Sums over the rows of a call - the
+(attn_ref64) with dropout_oracle's masks (drawn on the device), nce_oracle, sigmoid_oracle,
+simreg_oracle and augment_oracle (augment64).  The per-element gates are theirs; the vocabulary
+cross-entropy's are derived below from what its kernels compute.  Sums over the rows of a call - the
 LayerNorm gain gradient dg, the feed-forward's vsum and dg4, the column sums (d bias, dpos, dcls) and
 the scatter-adds (dtok, d pos table) - are gated at `n_add * 2^-24 * sum |terms|`, n_add the longest
 chain of fp32 additions any term goes through in the kernel's launch: the sequential rows of one
@@ -29,9 +32,13 @@ from collections import Counter
 import torch
 
 import attn_oracle as AO
+import augment_oracle as AU
 import block_oracle as BO
+import dropout_oracle as DO
 import gemm_oracle as GO
 import nce_oracle as NO
+import sigmoid_oracle as SG
+import simreg_oracle as SR
 
 U24 = 2.0 ** -24          # one fp32 addition, relative to the sum of |terms| it adds
 ROWS = 4096               # rows per fp64 reference chunk
@@ -44,22 +51,6 @@ EXACT_FAIL = math.inf     # the ratio of a bit-exact output that differs
 HOST_HELPERS = {
     "patch_row_stride": "row stride arithmetic, no launch",
     "check_arg16_seg_len": "argument check, no launch",
-}
-
-# wrappers none of the bench workloads (cfg3 nce / dcl_extra, cfg2, cfg4 FILIP, the AdamW step) calls
-NOT_REACHED = {
-    "cast_bf16_rows": "patch rows of 16 x 16 x 3 and 32 x 32 x 3 values are multiples of 8: no padded cast",
-    "patchify_scatter": "bench images take no gradient",
-    "sigmoid_fwd": "bench trains InfoNCE / DCL / FILIP, not the sigmoid loss",
-    "sigmoid_bwd": "bench trains InfoNCE / DCL / FILIP, not the sigmoid loss",
-    "vocab_ce_fwd": "no MLM loss in bench",
-    "vocab_ce_bwd": "no MLM loss in bench",
-    "simreg_pack": "bench runs without the similarity regularisation",
-    "simreg_fwd": "bench runs without the similarity regularisation",
-    "simreg_bwd": "bench runs without the similarity regularisation",
-    "augment": "no SimSiam / SimCLR views in bench",
-    "filip_nce_blocks_fwd": "multiview FILIP only (aug_text / aug_image); bench's FILIP has one view",
-    "filip_nce_blocks_bwd": "multiview FILIP only (aug_text / aug_image); bench's FILIP has one view",
 }
 
 
@@ -343,25 +334,32 @@ def _attn_slices(A):
         yield b0, b1, slice(b0 * n, b1 * n), mk
 
 
+def _attn_ref(A, b0, b1, rows, mk, bwd):
+    """attn_oracle's fp64 reference of batch items [b0, b1), or with dropout dropout_oracle's, fed the
+    mask of the call's seed and layer drawn on the device (dropout_oracle.attn_drop_mul_torch)."""
+    qkv, n, H = A["qkv"][rows], A["n"], A["heads"]
+    o, d_o = (A["o"][rows], A["d_o"][rows]) if bwd else (None, None)
+    if A["dropout"] is None:
+        return AO.attn_ref64(qkv, mk, b1 - b0, n, H, A["scale"], A["causal"], o=o, d_o=d_o)
+    p, seed, layer = A["dropout"]
+    drop = DO.attn_drop_mul_torch(int(seed.item()), b0, b1, H, n, layer, p, qkv.device)
+    return DO._attn_chunk64(qkv, mk, b1 - b0, n, H, A["scale"], A["causal"], o, d_o, drop)
+
+
 def check_attn_fwd(A, before, res):
-    if A["dropout"] is not None:
-        return None                       # dropout masks: test_gpu_attn_dropout.py
     o, lse = res
     w = Worst()
     for b0, b1, rows, mk in _attn_slices(A):
-        r = AO.attn_ref64(A["qkv"][rows], mk, b1 - b0, A["n"], A["heads"], A["scale"], A["causal"])
+        r = _attn_ref(A, b0, b1, rows, mk, False)
         w.add("o", BO.gate_ratio(o[rows], r["o"], r["g_o"]))
         w.add("lse", BO.gate_ratio(lse[b0:b1], r["lse"], r["g_lse"]))
     return w
 
 
 def check_attn_bwd(A, before, dqkv):
-    if A["dropout"] is not None:
-        return None
     w = Worst()
     for b0, b1, rows, mk in _attn_slices(A):
-        r = AO.attn_ref64(A["qkv"][rows], mk, b1 - b0, A["n"], A["heads"], A["scale"], A["causal"],
-                          o=A["o"][rows], d_o=A["d_o"][rows])
+        r = _attn_ref(A, b0, b1, rows, mk, True)
         w.add("dqkv", BO.gate_ratio(dqkv[rows], r["dqkv"], r["g_dqkv"]))
     return w
 
@@ -426,17 +424,29 @@ def _logits(a, b, temp, r0, r1):
 NCE_ROWS = 2048
 
 
+def _loss_sum_ratio(loss, before, scale, terms_sum, terms_abs, term_gates, n_add):
+    """A fused loss sum loss_accum += scale * sum(terms): the terms' own gates scaled, plus n_add fp32
+    additions of the sum of |terms| and of the prefill."""
+    l0 = before["loss_accum"].double().item()
+    gate = abs(scale) * term_gates + n_add * U24 * (abs(l0) + abs(scale) * terms_abs)
+    return abs(loss.double().item() - (l0 + scale * terms_sum)) / gate
+
+
 def check_nce_fwd(A, before, res):
-    if A["loss_accum"] is not None:
-        return None                       # the fused loss sum: test_gpu_nce.py
     lse, pos = res
     a, b, off, dcl = A["a"], A["b"], A["diag_offset"], A["dcl"]
     temp = A["temp_exp"].double().item()
     w = Worst()
+    t_sum = t_abs = t_gate = 0.0
     for r0, r1 in _chunks(a.shape[0], NCE_ROWS):
         ref_lse, ref_pos = NO.ref_rows(_logits(a, b, temp, r0, r1), off + r0, dcl)
-        w.add("lse", BO.gate_ratio(lse[r0:r1], ref_lse, NO.lse_gate(temp, ref_lse)))
-        w.add("pos", BO.gate_ratio(pos[r0:r1], ref_pos, torch.full_like(ref_pos, temp * NO.LOGIT_GATE)))
+        g_lse, g_pos = NO.lse_gate(temp, ref_lse), torch.full_like(ref_pos, temp * NO.LOGIT_GATE)
+        w.add("lse", BO.gate_ratio(lse[r0:r1], ref_lse, g_lse))
+        w.add("pos", BO.gate_ratio(pos[r0:r1], ref_pos, g_pos))
+        t = ref_lse - ref_pos
+        t_sum, t_abs, t_gate = t_sum + t.sum().item(), t_abs + t.abs().sum().item(), t_gate + (g_lse + g_pos).sum().item()
+    if A["loss_accum"] is not None:
+        w.add("loss", _loss_sum_ratio(A["loss_accum"], before, A["loss_scale"], t_sum, t_abs, t_gate, a.shape[0]))
     return w
 
 
@@ -636,12 +646,309 @@ def check_filip_expand16(A, before, g):
     return {"g": exact(g, want)}
 
 
+def block_columns(n, b, B, col_run, j, device=None):
+    """Columns of image view j's global samples k = 0 .. B-1 in a view-block matrix [m b, n B]:
+    view-major (col_run = B) is n runs of all B samples; rank-major (col_run = b) is, per rank of b
+    samples, that rank's n views in turn."""
+    idx = torch.arange(n * B, device=device)
+    if col_run == B:
+        return idx.view(n, B)[j]
+    assert col_run == b and B % b == 0, (col_run, b, B)
+    return idx.view(B // b, n, b)[:, j, :].reshape(-1)
+
+
+def _blocks_ref(A):
+    """fp64 per (row, block): the lse over the block's columns (the positive left out under DCL, an
+    empty DCL denominator ln(1e-20)), the positive's similarity, the block weight of the row, and
+    p = exp(s - lse) over the block's columns.  -> (lse [R, n], pos [R, n], bw [R, n], [(cols, p)])."""
+    s, m, n, col_run, off, dcl = A["s"], A["m"], A["n"], A["col_run"], A["diag_off"], A["dcl"]
+    R, Ctot = s.shape
+    b, B = R // m, Ctot // n
+    rows = torch.arange(R, device=s.device)
+    x = rows % b
+    bw_all = A["block_w"].double().view(m, n)[rows // b]
+    lse, pos, parts = [], [], []
+    for j in range(n):
+        cols = block_columns(n, b, B, col_run, j, s.device)
+        sj = s[:, cols].double()
+        pos.append(sj[rows, x + off])
+        if dcl:
+            sj[rows, x + off] = -math.inf
+        lj = torch.logsumexp(sj, dim=1)
+        if dcl:
+            lj = torch.where(torch.isinf(lj) & (lj < 0), NO.LN_1E20, lj)
+        lse.append(lj)
+        parts.append((cols, torch.exp(sj - lj[:, None])))
+    return torch.stack(lse, 1), torch.stack(pos, 1), bw_all, parts
+
+
+def _row_valid_of(A, R, dev):
+    rv = A["row_valid"]
+    return torch.ones(R, dtype=torch.bool, device=dev) if rv is None else rv
+
+
+def check_filip_nce_blocks_fwd(A, before, lse):
+    s, loss = A["s"], A["loss_accum"]
+    valid = _row_valid_of(A, s.shape[0], s.device)
+    ref, pos, bw, _ = _blocks_ref(A)
+    gate = 1e-6 * ref.abs() + 4e-6
+    w = Worst()
+    w.add("lse", ((lse.double() - ref).abs() / gate)[valid].max().item() if bool(valid.any()) else 0.0)
+    if not bool(valid.all()):                 # rows without a valid token: lse 0 exactly
+        w.add("lse_invalid", exact(lse[~valid], torch.zeros_like(lse[~valid])))
+    if loss is not None:
+        terms = (bw * (ref - pos))[valid]
+        w.add("loss", _loss_sum_ratio(loss, before, 1.0, terms.sum().item(), terms.abs().sum().item(),
+                                      (bw * gate)[valid].sum().item(), terms.numel()))
+    return w
+
+
+def check_filip_nce_blocks_bwd(A, before, g):
+    s, off = A["s"], A["diag_off"]
+    R = s.shape[0]
+    b = R // A["m"]
+    gs = A["gscale"].double().item()
+    valid = _row_valid_of(A, R, s.device)
+    _, _, bw, parts = _blocks_ref(A)
+    rows = torch.arange(R, device=s.device)
+    w = Worst()
+    for j, (cols, p) in enumerate(parts):
+        scale = gs * bw[:, j:j + 1]
+        ref = scale * p
+        ref[rows, rows % b + off] -= scale[:, 0]
+        gate = scale.abs() * (2e-5 * p + 2e-6)
+        err = ((g[:, cols].double() - ref).abs() / gate)[valid]
+        w.add("g", err.max().item() if err.numel() else 0.0)
+    if not bool(valid.all()):                 # rows without a valid token: g 0 exactly
+        w.add("g_invalid", exact(g[~valid], torch.zeros_like(g[~valid])))
+    return w
+
+
+# --------------------------------------------------------------------------- sigmoid loss
+# Gates of sigmoid_oracle (test_gpu_sigmoid_loss.py's): row losses ROW_REL relative, g G_REL relative
+# where |l| < G_LIVE and exactly 0 where |l| > G_SATURATED, d temperature / d logit_bias SUM_REL of the
+# sum of their terms' magnitudes.  The logits come from the bf16 operands the call received, so the
+# split hi | lo product is the kernel's.
+
+def _sig_rows(A, r0, r1):
+    temp, bias = A["temp_exp"].double().item(), A["logit_bias"].double().item()
+    l = _logits(A["a"], A["b"], temp, r0, r1) + bias
+    z = SG.labels(r1 - r0, l.shape[1], A["diag_offset"] + r0, like=l)
+    return l, z, temp, bias
+
+
+def check_sigmoid_fwd(A, before, rowloss):
+    w = Worst()
+    total = 0.0
+    for r0, r1 in _chunks(A["a"].shape[0], NCE_ROWS):
+        l, z, _, _ = _sig_rows(A, r0, r1)
+        ref = SG.softplus(-z * l).sum(1)
+        w.add("rows", BO.gate_ratio(rowloss[r0:r1], ref, SG.ROW_REL * ref + 1e-30))
+        total += ref.sum().item()
+    if A["loss_accum"] is not None:
+        l0, sc = before["loss_accum"].double().item(), A["loss_scale"]
+        gate = SG.LOSS_REL * abs(sc) * total + 2.0 ** -23 * abs(l0) + 1e-30
+        w.add("loss", abs(A["loss_accum"].double().item() - (l0 + sc * total)) / gate)
+    return w
+
+
+def check_sigmoid_bwd(A, before, g):
+    gs = A["gscale"].double().item()
+    C = A["b"].shape[0]
+    w = Worst()
+    w.add("pad", exact(g[:, C:], torch.zeros_like(g[:, C:])))
+    dt = dt_abs = db = db_abs = 0.0
+    for r0, r1 in _chunks(A["a"].shape[0], NCE_ROWS):
+        l, z, temp, bias = _sig_rows(A, r0, r1)
+        rg = gs * -z * torch.sigmoid(-z * l)                  # sigmoid(l) - [positive], no cancellation
+        want = temp * rg
+        gk = g[r0:r1, :C].double()
+        live = l.abs() < SG.G_LIVE
+        rel = (gk - want).abs()[live] / want.abs()[live]
+        w.add("g", rel.max().item() / SG.G_REL if rel.numel() else 0.0)
+        w.add("g_saturated", 0.0 if not bool(gk[l.abs() > SG.G_SATURATED].ne(0).any()) else EXACT_FAIL)
+        t = rg * (l - bias)
+        dt, dt_abs = dt + t.sum().item(), dt_abs + t.abs().sum().item()
+        db, db_abs = db + rg.sum().item(), db_abs + rg.abs().sum().item()
+    for name, val, mag in (("dtemp", dt, dt_abs), ("dbias", db, db_abs)):
+        if A[name] is not None:
+            d0 = before[name].double().item()
+            gate = SG.SUM_REL * (mag + abs(d0)) + 1e-30
+            w.add(name, abs(A[name].double().item() - (d0 + val)) / gate)
+    return w
+
+
+# --------------------------------------------------------------------------- vocabulary cross-entropy
+# Per-element gates derived from what the kernels compute.  A logit l = x w^T + bias is an fp32
+# accumulation at K = d: its error is within gemm_oracle.GAMMA of sum |x| |w| (the GEMM gate's
+# accumulation term) plus one rounding of the bias add.  lse inherits the softmax-weighted logit error
+# plus the fp32 log-sum-exp (nce_oracle.lse_gate's 2^-20 (1 + |lse|)); the target logit its own logit
+# error.  g = bf16(gscale (exp(l - lse) - onehot)) with the call's lse: one bf16 rounding, plus
+# gscale p times the logit's error, the fp32 rounding of l - lse and the exp approximation.
+
+VCE_ROWS = 1024
+
+
+def _vce_rows(A, r0, r1):
+    x, wt, bias = A["x"][r0:r1].double(), A["w"].double(), A["bias"]
+    l = x @ wt.t()
+    e_l = GO.GAMMA * (x.abs() @ wt.abs().t())
+    if bias is not None:
+        l += bias.double()
+    e_l += U24 * l.abs()
+    return l, e_l
+
+
+def check_vocab_ce_fwd(A, before, res):
+    lse, pos = res
+    labels = A["labels"]
+    w = Worst()
+    t_sum = t_abs = t_gate = 0.0
+    for r0, r1 in _chunks(A["x"].shape[0], VCE_ROWS):
+        l, e_l = _vce_rows(A, r0, r1)
+        ref = torch.logsumexp(l, dim=1)
+        g_lse = (torch.exp(l - ref[:, None]) * e_l).sum(1) + 2.0 ** -20 * (1.0 + ref.abs())
+        lab = labels[r0:r1, None]
+        ref_pos, g_pos = l.gather(1, lab)[:, 0], e_l.gather(1, lab)[:, 0]
+        w.add("lse", BO.gate_ratio(lse[r0:r1], ref, g_lse))
+        w.add("target", BO.gate_ratio(pos[r0:r1], ref_pos, g_pos))
+        t = ref - ref_pos
+        t_sum, t_abs, t_gate = t_sum + t.sum().item(), t_abs + t.abs().sum().item(), t_gate + (g_lse + g_pos).sum().item()
+    if A["loss_accum"] is not None:
+        w.add("loss", _loss_sum_ratio(A["loss_accum"], before, A["loss_scale"], t_sum, t_abs, t_gate,
+                                      A["x"].shape[0]))
+    return w
+
+
+def check_vocab_ce_bwd(A, before, g):
+    gs = A["gscale"].double().item()
+    V = A["w"].shape[0]
+    labels, lse_k = A["labels"], A["lse"]
+    w = Worst()
+    w.add("pad", exact(g[:, V:], torch.zeros_like(g[:, V:])))
+    for r0, r1 in _chunks(A["x"].shape[0], VCE_ROWS):
+        l, e_l = _vce_rows(A, r0, r1)
+        lk = lse_k[r0:r1].double()[:, None]
+        p = torch.exp(l - lk)
+        ref = gs * p
+        ref.scatter_add_(1, labels[r0:r1, None], torch.full((r1 - r0, 1), -gs, dtype=ref.dtype, device=ref.device))
+        gate = (NO.BF16_REL * ref.abs() + gs * p * (e_l + 2.0 ** -23 * (l.abs() + lk.abs()) + 2.0 ** -22)
+                + gs * 2.0 ** -120)
+        w.add("g", BO.gate_ratio(g[r0:r1, :V], ref, gate))
+    return w
+
+
+# --------------------------------------------------------------------------- similarity regularisation
+# Gates of simreg_oracle (test_gpu_simreg.py's) against E = a b^T of the call's bf16 operands, the
+# diagonal column of each row zeroed.  E's own error, simreg_oracle.E_ABS, was measured on latents of
+# random directions, where the partial sums of E's K = 6 D chain stay near |<t_r, t_c>| ~ D^-1/2.  A
+# training step's latents are far from orthogonal (a freshly initialised tower maps every input near
+# one direction), so the chain's running sums reach |<t_r, t_c>| ~ 1 before the -V V^T half brings
+# them back to E: its accumulation error is then bounded by the GEMM's own per-element chain bound
+# (gemm_oracle.chain_bound of the running sums), and E's error term is the larger of the two.
+
+def _simreg_rows(A, r0, r1):
+    """fp64 E of rows [r0, r1) with the diagonal zeroed, and the bound on the kernel's error of E."""
+    e, S, P = GO.chain_sums64(A["a"][r0:r1], A["b"])
+    e_err = torch.clamp(GO.chain_bound(S, P), min=SR.E_ABS)
+    del S, P
+    r = torch.arange(r1 - r0, device=e.device)
+    e[r, r + r0 + A["diag_offset"]] = 0.0
+    return e, e_err
+
+
+def check_simreg_pack(A, before, out):
+    v = -A["v"] if A["negate_v"] else A["v"]
+    return {"": exact(out, torch.cat([A["t"], v], 1))}
+
+
+def check_simreg_fwd(A, before, rowsum):
+    w = Worst()
+    total = 0.0
+    for r0, r1 in _chunks(A["a"].shape[0], NCE_ROWS):
+        e, e_err = _simreg_rows(A, r0, r1)
+        ref = (e * e).sum(1)
+        w.add("rowsum", BO.gate_ratio(rowsum[r0:r1], ref, SR.ROWSUM_REL * ref + 2 * (e_err * e.abs()).sum(1)))
+        total += ref.sum().item()
+    if A["loss_accum"] is not None:
+        l0, sc = before["loss_accum"].double().item(), A["loss_scale"]
+        gate = SR.LOSS_REL * abs(sc) * total + 2.0 ** -23 * abs(l0) + 1e-30
+        w.add("loss", abs(A["loss_accum"].double().item() - (l0 + sc * total)) / gate)
+    return w
+
+
+def check_simreg_bwd(A, before, g):
+    gs = A["gscale"].double().item()
+    C, off = A["b"].shape[0], A["diag_offset"]
+    R = A["a"].shape[0]
+    r = torch.arange(R, device=g.device)
+    w = Worst()
+    w.add("pad", exact(g[:, C:], torch.zeros_like(g[:, C:])))
+    w.add("diag", exact(g[r, r + off], torch.zeros_like(g[r, r + off])))
+    for r0, r1 in _chunks(R, NCE_ROWS):
+        e, e_err = _simreg_rows(A, r0, r1)
+        ref = gs * e
+        w.add("g", BO.gate_ratio(g[r0:r1, :C], ref, SR.G_REL * ref.abs() + abs(gs) * e_err))
+    return w
+
+
+# --------------------------------------------------------------------------- augmentation
+
+AUG_IMAGES = 256          # images per fp64 augmentation reference chunk
+AUG_ARGS = ("ops", "factor", "one_minus", "grayscale", "flip", "blur_kernel", "normalize", "crop", "out_size")
+
+
+def check_augment(A, before, out):
+    """augment_oracle.augment64 of the call's own arguments, at augment_oracle.GATE of max(1, max |ref|)."""
+    x = A["x"]
+    kw = {k: A[k] for k in AUG_ARGS}
+    err = top = 0.0
+    for b0, b1 in _chunks(x.shape[0], AUG_IMAGES):
+        ref = AU.augment64(x[b0:b1], **kw)
+        err = max(err, (out[b0:b1].double() - ref).abs().max().item())
+        top = max(top, ref.abs().max().item())
+    return {"": err / (AU.GATE * max(1.0, top))}
+
+
+# --------------------------------------------------------------------------- image gradients
+
+def cast_rows_check(A, before, out):
+    src, cols = A["src"], A["src"].shape[1]
+    return {"": exact(out[:, :cols], src.bfloat16()), "pad": exact(out[:, cols:], torch.zeros_like(out[:, cols:]))}
+
+
+def unpatchify64(rows, image_shape, p, keep):
+    """The inverse of gemm_oracle.patchify64 with PatchDropout's keep: rows [B k, p p C] (only their first
+    p p C columns are read) -> fp64 [B, C, H, W], every pixel of a patch not in keep[b] 0."""
+    B, C, H, W = (int(v) for v in image_shape)
+    gh, gw, pd = H // p, W // p, p * p * C
+    r = rows[:, :pd].double().view(B, -1, pd)
+    if keep is not None:
+        r = torch.zeros((B, gh * gw, pd), dtype=r.dtype, device=r.device).scatter_(
+            1, keep[:, :, None].expand(-1, -1, pd), r)
+    img = torch.zeros((B, C, H, W), dtype=r.dtype, device=r.device)
+    img[:, :, :gh * p, :gw * p] = r.view(B, gh, gw, p, p, C).permute(0, 5, 1, 3, 2, 4).reshape(B, C, gh * p, gw * p)
+    return img
+
+
+def check_patchify_scatter(A, before, img):
+    """Each pixel comes from exactly one f32 row element (or is 0): exact."""
+    src, shape, p, keep = A["src"], A["image_shape"], A["patch"], A["keep"]
+    B = int(shape[0])
+    k = src.shape[0] // B
+    w = Worst()
+    for b0, b1 in _chunks(B, 256):
+        ref = unpatchify64(src[b0 * k:b1 * k], (b1 - b0,) + tuple(shape[1:]), p,
+                           None if keep is None else keep[b0:b1])
+        w.add("", exact(img[b0:b1].double(), ref))
+    return w
+
+
 # --------------------------------------------------------------------------- registry
 
 class Check:
-    """check(bound arguments after the call, {name: clone before the call}, result) -> {output: ratio},
-    or None for a variant this registry does not check; inplace(arguments) -> names of the buffers
-    the call writes in place or accumulates into."""
+    """check(bound arguments after the call, {name: clone before the call}, result) -> {output: ratio};
+    inplace(arguments) -> names of the buffers the call writes in place or accumulates into."""
 
     def __init__(self, check, inplace=()):
         self.check = check
@@ -672,7 +979,7 @@ CHECKS = {
     "ff_bwd": Check(check_ff_bwd),
     "ff_w2_grad_post_": Check(check_ff_w2_grad_post, ("raw", "dg")),
     "adamw_step_": Check(check_adamw, ("p", "m", "v")),
-    "nce_fwd": Check(check_nce_fwd),
+    "nce_fwd": Check(check_nce_fwd, ("loss_accum",)),
     "nce_bwd": Check(check_nce_bwd, ("dtemp",)),
     "text_embed_fwd": Check(check_text_embed_fwd),
     "text_embed_bwd": Check(check_text_embed_bwd),
@@ -681,6 +988,18 @@ CHECKS = {
     "filip_nce_fwd": Check(check_filip_nce_fwd, ("loss_accum",)),
     "filip_nce_bwd": Check(check_filip_nce_bwd),
     "filip_expand16": Check(check_filip_expand16),
+    "filip_nce_blocks_fwd": Check(check_filip_nce_blocks_fwd, ("loss_accum",)),
+    "filip_nce_blocks_bwd": Check(check_filip_nce_blocks_bwd),
+    "sigmoid_fwd": Check(check_sigmoid_fwd, ("loss_accum",)),
+    "sigmoid_bwd": Check(check_sigmoid_bwd, ("dtemp", "dbias")),
+    "vocab_ce_fwd": Check(check_vocab_ce_fwd, ("loss_accum",)),
+    "vocab_ce_bwd": Check(check_vocab_ce_bwd),
+    "simreg_pack": Check(check_simreg_pack),
+    "simreg_fwd": Check(check_simreg_fwd, ("loss_accum",)),
+    "simreg_bwd": Check(check_simreg_bwd),
+    "augment": Check(check_augment),
+    "cast_bf16_rows": Check(cast_rows_check),
+    "patchify_scatter": Check(check_patchify_scatter),
 }
 
 
@@ -724,7 +1043,7 @@ class Recorder:
     """Spies on every public wrapper of the kernels module K (see the module docstring).
 
     results: [(label, ratio)] of every checked output; calls: Counter of wrapper calls; unchecked:
-    Counter of calls to wrappers (or variants) with no check; signatures: the checked signatures."""
+    Counter of calls to wrappers with no check; signatures: the checked signatures."""
 
     def __init__(self, K, verbose=True):
         self.K, self.verbose = K, verbose
@@ -758,16 +1077,13 @@ class Recorder:
             torch.cuda.synchronize()
             ratios = check.check(A, before, out)
             del before
-            if ratios is None:
-                self.unchecked[f"{name}[{_sig_text(A)}]"] += 1
-            else:
-                label = f"{name}[{_sig_text(A)}]"
-                self.signatures[key] = label
-                self.arguments[key] = {k: _meta(v) for k, v in A.items()}
-                for k, r in ratios.items():
-                    self.results.append((label + k, r))
-                    if self.verbose:
-                        print(f"GATE {label}{k} {r:.4f}", flush=True)
+            label = f"{name}[{_sig_text(A)}]"
+            self.signatures[key] = label
+            self.arguments[key] = {k: _meta(v) for k, v in A.items()}
+            for k, r in ratios.items():
+                self.results.append((label + k, r))
+                if self.verbose:
+                    print(f"GATE {label}{k} {r:.4f}", flush=True)
             torch.cuda.empty_cache()
             return out
 

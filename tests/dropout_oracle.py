@@ -52,6 +52,56 @@ def attn_keep(seed: int, B: int, H: int, n: int, layer: int, p: float, rows=None
     return words.astype(np.uint64) < np.uint64(keep_threshold(p))
 
 
+# --------------------------------------------------------------------------- the same mask in torch
+# philox4x32_10 / attn_keep restated on int64 tensors, so the mask of a whole training-shape layer can be
+# drawn on the device.  Every 32 x 32-bit product is formed from 16-bit halves, so no intermediate
+# leaves the int64 range.
+
+_M32 = 0xFFFFFFFF
+
+
+def _mulhilo(a: torch.Tensor, m: int):
+    """(hi, lo) 32-bit words of the 64-bit product of a (int64 holding uint32) and the constant m."""
+    al, ah = a & 0xFFFF, a >> 16
+    ml, mh = m & 0xFFFF, m >> 16
+    t0 = al * ml
+    t1 = al * mh + ah * ml + (t0 >> 16)
+    return ah * mh + (t1 >> 16), (t0 & 0xFFFF) | ((t1 & 0xFFFF) << 16)
+
+
+def philox4x32_10_torch(c0, c1, c2, c3, key):
+    """Philox4x32-10 of the counter words (int64 tensors holding uint32) -> 4 int64 tensors of uint32."""
+    k0, k1 = key
+    for r in range(10):
+        if r:
+            k0, k1 = (k0 + W0) & _M32, (k1 + W1) & _M32
+        h0, l0 = _mulhilo(c0, M0)
+        h1, l1 = _mulhilo(c2, M1)
+        c0, c1, c2, c3 = h1 ^ c1 ^ k0, l1, h0 ^ c3 ^ k1, l0
+    return c0, c1, c2, c3
+
+
+def attn_keep_torch(seed: int, b0: int, b1: int, H: int, n: int, layer: int, p: float, device="cpu") -> torch.Tensor:
+    """attn_keep for the batch items [b0, b1) of a layer: bool [b1 - b0, H, n, n], on `device`."""
+    ng = (n + 3) // 4
+    dev = torch.device(device)
+    bh = torch.arange(b0 * H, b1 * H, device=dev, dtype=torch.int64).view(-1, 1, 1)
+    i = torch.arange(n, device=dev, dtype=torch.int64).view(1, -1, 1)
+    g = torch.arange(ng, device=dev, dtype=torch.int64).view(1, 1, -1)
+    shape = (bh.shape[0], n, ng)
+    ctr = [g.expand(shape), i.expand(shape), bh.expand(shape), torch.full(shape, int(layer), device=dev)]
+    words = torch.stack(philox4x32_10_torch(*ctr, seed_key(seed)), -1)
+    words = words.reshape(b1 - b0, H, n, 4 * ng)[..., :n]
+    return words < keep_threshold(p)
+
+
+def attn_drop_mul_torch(seed: int, b0: int, b1: int, H: int, n: int, layer: int, p: float, device="cpu"):
+    """attn_drop_mul for the batch items [b0, b1), drawn with attn_keep_torch."""
+    pf = float(np.float32(p))
+    keep = attn_keep_torch(seed, b0, b1, H, n, layer, p, device)
+    return keep.double() * (0.0 if pf == 1.0 else 1.0 / (1.0 - pf))
+
+
 def attn_drop_mul(seed: int, B: int, H: int, n: int, layer: int, p: float, device="cpu") -> torch.Tensor:
     """fp64 [B, H, n, n] multiplier M / (1 - p) of the probabilities (0 everywhere at p = 1)."""
     keep = torch.from_numpy(attn_keep(seed, B, H, n, layer, p)).to(device)

@@ -20,10 +20,16 @@ test_gemm_edges_gates.py holds with it.
 GAMMA does not hold for long k-block chains: the tensor cores do not round the fp32 accumulation to
 nearest, so its error grows with the MMAs of a chain.  At the training step's shapes a latent gradient
 (128 k-blocks, one large term early in many rows) erred by 4.1 x GAMMA S, a weight gradient of 1568
-k-blocks by 1.8 x.  gemm_gate therefore takes, where given, the larger of GAMMA S and chain_bound: two
-ulp per MMA of the running partial sum of the element's own chain (chain_sums64).  That bound follows
-the data: with products of both signs the running sum grows like the square root of the chain, and a
-missing or doubled k-block still spans many gates (test_gemm_edges_gates.py).
+k-blocks by 1.8 x.  gemm_gate therefore takes, where given, the larger of GAMMA S and chain_bound: four
+ulp per MMA of the running partial sum of the element's own chain (chain_sums64).  Four, not two: one
+wgmma (k = 16) aligns its 16 products to the largest exponent among them and the accumulator and
+truncates each to two bits below that ulp, so it loses up to 16 / 4 = 4 ulp, all in one direction when
+the products share a sign.  Measured on an H100 80GB HBM3 with one MMA of 16 positive products 2^-12 to
+2^-32 of a running sum of 1.0: at most 3.995 ulp, 2.2 on average; with mixed signs 3.3.  A bound of
+2^-22 |x| (two ulp at the top of a binade) is exceeded there, and was, by 1.05 x, on the MLM head's
+weight gradient (168 k-blocks of small same-sign softmax terms).  The bound follows the data: with
+products of both signs the running sum grows like the square root of the chain, and a missing or
+doubled k-block still spans many gates (test_gemm_edges_gates.py).
 
 Operands have rows of A and rows of B (the output's columns) scaled over three orders of magnitude,
 so output tiles of small values exist and their gates are small with them.
@@ -161,19 +167,30 @@ def abs_sum64(a, b, a_major=0, b_major=0):
     return logical(a, a_major).abs() @ logical(b, b_major).abs().t()
 
 
-# One wgmma (k = 16 for bf16) adds its 16 products into the fp32 accumulator without rounding to
-# nearest: at most two ulp, 2^-22 relative, of the larger of the running sum and the products' magnitude.
-MMA_ULP = 2.0 ** -22
+# One wgmma (k = 16 for bf16) aligns its 16 products to the largest exponent among them and the fp32
+# accumulator and truncates each two bits below that ulp: at most 4 ulp of the largest magnitude it
+# adds (measured 3.995).  An ulp of x is 2^-23 floor2(x), floor2(x) = 2^floor(log2 x).
+MMA_ULPS = 4.0
+ULP = 2.0 ** -23
+DRIFT = 1.0 + 2.0 ** -8        # the accumulator the MMA sees may exceed the exact running sum by its error
 
 
 def _kslice(t, major: int, k0: int, k1: int):
     return t[:, k0:k1] if major == 0 else t[k0:k1]
 
 
+def floor2(x: torch.Tensor) -> torch.Tensor:
+    """2^floor(log2 x) for x > 0, 0 for x = 0."""
+    m, e = torch.frexp(x)
+    return torch.where(x > 0, torch.ldexp(torch.full_like(x, 0.5), e), torch.zeros_like(x))
+
+
 def chain_sums64(a, b, a_major=0, b_major=0, ranges=None, k_chunk=8192):
     """fp64 (A B^T, S = |A| |B|^T, P) of the stored operands, P the sum over every 64-wide k-block b of
-    |P_b|, the running partial sum of its split's chain after block b (ranges: the k-block ranges of
-    the splits, split_ranges; None: one chain).  Converted to fp64 k_chunk columns of K at a time."""
+    floor2(DRIFT (|P_b| + s_b)), P_b the running partial sum of its split's chain after block b and s_b
+    the block's share of S: each of the block's four MMAs adds terms no larger than |P_b| + s_b (ranges:
+    the k-block ranges of the splits, split_ranges; None: one chain).  Converted to fp64 k_chunk columns
+    of K at a time."""
     K = a.shape[1] if a_major == 0 else a.shape[0]
     starts = {0} if ranges is None else {r[0] for r in ranges}
     acc = S = P = run = None
@@ -186,21 +203,21 @@ def chain_sums64(a, b, a_major=0, b_major=0, ranges=None, k_chunk=8192):
             p = A[:, j0:j1] @ B[:, j0:j1].t()
             s = Aa[:, j0:j1] @ Ba[:, j0:j1].t()
             if acc is None:
-                acc, S, P = p.clone(), s, torch.zeros_like(p)
+                acc, S, P = p.clone(), s.clone(), torch.zeros_like(p)
             else:
                 acc += p
                 S += s
             run = p if (k0 + j0) // BLOCK_K in starts else run + p
-            P += run.abs()
+            P += floor2(DRIFT * (run.abs() + s))
     return acc, S, P
 
 
 def chain_bound(S, P):
-    """Per-element bound on the accumulation error of the k-block chains: MMA_ULP (4 P + 5 S).  Within
-    k-block b the four MMAs see running sums of at most |P_b| + s_b (s_b its share of S), so the chain
-    adds at most MMA_ULP (4 sum_b (|P_b| + s_b) + S).  The running sum, not S, carries the bound: with products
-    of both signs it grows like the square root of the chain and one k-block stays visible."""
-    return MMA_ULP * (4.0 * P + 5.0 * S)
+    """Per-element bound on the accumulation error of the k-block chains: MMA_ULPS ulp for each of the
+    four MMAs of every k-block, 16 ULP P, plus ULP S for the final conversion.  The running sum, not
+    S, carries the bound: with products of both signs it grows like the square root of the chain and
+    one k-block stays visible."""
+    return 4.0 * MMA_ULPS * ULP * P + ULP * S
 
 
 def gemm_gate(a, b, a_major=0, b_major=0, alpha=1.0, bias=None, residual=None, res_rows=None, prefill=None,

@@ -23,6 +23,21 @@ from oracle import clip_oracle as O
 INIT_TEMPERATURE = math.log(10.0)
 INIT_LOGIT_BIAS = -10.0
 
+# Gates of the kernels xclip_sigmoid_fwd / _bwd (test_gpu_sigmoid_loss.py and the per-call checks of
+# bench_call_oracle.py): about 2x the largest error measured on an H100 80GB HBM3 at a 700 W power limit.
+# Per-row loss 5.2e-5 relative (the summed loss no more, 3.6e-5 for one row), g 4.0e-3 elementwise (one
+# bf16 rounding, 2^-8), d temperature and d logit_bias 2.3e-5 of the sum of their terms' magnitudes.  The
+# row errors peak on rows whose positive is their own latent at a logit near 0: the split-bf16 operands
+# drop the lo * lo product, up to 2^-18 of a similarity, and exactly there softplus' = 1/2.
+ROW_REL = 1e-4          # per-row loss, relative
+LOSS_REL = 1e-4         # sum of the rows (the kernel's loss_accum), relative
+G_REL = 8e-3            # bf16 g, elementwise relative where the logit is not saturated (|l| < G_LIVE)
+# d temperature and d logit_bias are sums of terms of both signs: gated relative to the sum of the
+# terms' magnitudes
+SUM_REL = 5e-5
+G_LIVE = 80.0           # |l| below this: u = e^-|l| is a normal fp32 number, g is checked elementwise
+G_SATURATED = 88.0      # |l| above this: g must be exactly 0
+
 
 def logits(zt, zi, temperature, logit_bias):
     return temperature.exp() * (zt @ zi.t()) + logit_bias

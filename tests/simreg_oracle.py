@@ -15,6 +15,18 @@ import torch
 
 from oracle import clip_oracle as O
 
+# Gates of the kernels xclip_simreg_fwd / _bwd against fp64 E = a b^T of their exact bf16 operands (shared
+# by test_gpu_simreg.py and the per-call checks of bench_call_oracle.py; measured maxima from an H100 80GB
+# HBM3 at a 700 W power limit).  E's own error is the tensor cores' fp32 accumulation over K = 6 D terms
+# whose partial sums reach the size of <t_r, t_c>, not of E: measured at most 6.2e-7 absolute (an aligned
+# case, |E| ~ 1e-4).  A row sum of E^2 may therefore miss 2 |E| E_ABS per entry on top of its relative
+# error (measured 1.6e-5 where E is not small); g = bf16(gscale * E) one bf16 rounding (2^-9) plus
+# gscale * E_ABS.
+E_ABS = 1.5e-6
+ROWSUM_REL = 5e-5
+LOSS_REL = 1e-4        # loss_accum against fp64 (measured at most 4.3e-5); g measured at most 1.45e-6 beyond
+G_REL = 2 ** -8        #   its bf16 rounding (gate 2.55e-6); row sums at most 0.16 of their gate
+
 
 def sim_reg_loss(zt, zi, zt_x, zi_x):
     """(:777-784) F.mse_loss of the off-diagonal similarities, averaged over the two latent pairs."""

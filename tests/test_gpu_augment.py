@@ -16,9 +16,8 @@ from x_clip_b200.aux import AugmentParams, SimCLRAugmentation
 pytestmark = pytest.mark.gpu
 
 FACTORS = (1.37, 0.61, 1.52, 0.13)          # brightness, contrast, saturation, hue
-# max |kernel - fp64| over max(1, max |fp64|); about twice the largest error measured on an H100
-# (8.5e-6, 3 x 130 x 97 -> 224: the resample's fp32 weights, which ATen's fp32 path computes the same way)
-GATE = 2e-5
+# max |kernel - fp64| over max(1, max |fp64|): augment_oracle.GATE, with what was measured against it
+GATE = AO.GATE
 
 
 @pytest.fixture(autouse=True)

@@ -29,11 +29,11 @@ calls (casts, embedding forward, patch gather, expand16) exact.  The ratios near
 the rounding bound.  AdamW p 0.554.  Retention plans: every gradient within 0.0004 of its 2e-3 gate;
 "auto" kept four compact chunks of six.
 
-The GEMM gate's accumulation term is the larger of GAMMA S and gemm_oracle.chain_bound, two ulp per
+The GEMM gate's accumulation term is the larger of GAMMA S and gemm_oracle.chain_bound, four ulp per
 MMA of each element's running partial sum along its split's k-block chain.  With GAMMA alone, the
 latent data gradient g @ hi at K = 8192 (dcl_extra) erred by 4.1 x its gate and a weight gradient of
-1568 k-blocks in one chain by 1.8 x; under the chain bound they use 0.70 and 0.18 of it.  The
-self-test's unsplit weight gradient of 1176 k-blocks uses 0.14 of its gate, and the same call with
+1568 k-blocks in one chain by 1.8 x; under the chain bound the latent gradient uses 0.43 of it.  The
+self-test's unsplit weight gradient of 1176 k-blocks uses 0.095 of its gate, and the same call with
 its first or last k-block dropped 63 and 62 gates.
 """
 import gc

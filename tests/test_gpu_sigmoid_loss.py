@@ -26,17 +26,10 @@ pytestmark = pytest.mark.gpu
 BF16, F32, F64 = torch.bfloat16, torch.float32, torch.float64
 
 # Gates: about 2x the largest error measured on an H100 80GB HBM3 at a 700 W power limit over the cases
-# below.  Kernels: per-row loss 5.2e-5 relative (the summed loss no more, 3.6e-5 for one row), g 4.0e-3
-# elementwise (one bf16 rounding, 2^-8), d temperature and d logit_bias 2.3e-5 of the sum of their terms'
-# magnitudes.  The row errors peak on rows whose positive is their own latent at a logit near 0: the
-# split-bf16 operands drop the lo * lo product, up to 2^-18 of a similarity, and exactly there
-# softplus' = 1/2.  SigmoidLossFn: loss 2.2e-5 (global batch 2), latent gradients 3.4e-3.
-ROW_REL = 1e-4          # per-row loss, relative
-LOSS_REL = 1e-4         # sum of the rows (the kernel's loss_accum), relative
-G_REL = 8e-3            # bf16 g, elementwise relative where the logit is not saturated
-# d temperature and d logit_bias are sums of terms of both signs: the kernel gate is relative to the sum
-# of the terms' magnitudes, SigmoidLossFn's (as test_gpu_nce_loss.py) rel * |ref| + abs
-SUM_REL = 5e-5
+# below.  Kernels: ROW_REL, LOSS_REL, G_REL and SUM_REL of sigmoid_oracle (shared with the per-call
+# checks of bench_call_oracle.py).  SigmoidLossFn: loss 2.2e-5 (global batch 2), latent gradients 3.4e-3;
+# its d temperature and d logit_bias gates are (as test_gpu_nce_loss.py) rel * |ref| + abs.
+ROW_REL, LOSS_REL, G_REL, SUM_REL = SG.ROW_REL, SG.LOSS_REL, SG.G_REL, SG.SUM_REL
 DSCALAR_REL, DSCALAR_ABS = 1e-4, 1e-7
 FN_LOSS_REL = 5e-5      # SigmoidLossFn: loss, relative
 FN_GRAD_REL = 8e-3      # SigmoidLossFn: latent gradients, relative Frobenius (two bf16 roundings)

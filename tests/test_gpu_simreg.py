@@ -28,14 +28,9 @@ pytestmark = pytest.mark.gpu
 BF16, F32, F64 = torch.bfloat16, torch.float32, torch.float64
 GOLD = Path(__file__).parent / "golden"
 
-# E's own error is the tensor cores' fp32 accumulation over K = 6 D terms whose partial sums reach the
-# size of <t_r, t_c>, not of E: measured at most 6.2e-7 absolute (an aligned case, |E| ~ 1e-4).  A row
-# sum of E^2 may therefore miss 2 |E| E_ABS per entry on top of its relative error (measured 1.6e-5
-# where E is not small); g = bf16(gscale * E) one bf16 rounding (2^-9) plus gscale * E_ABS.
-E_ABS = 1.5e-6
-ROWSUM_REL = 5e-5
-LOSS_REL = 1e-4        # loss_accum against fp64 (measured at most 4.3e-5); g measured at most 1.45e-6 beyond
-G_REL = 2 ** -8        #   its bf16 rounding (gate 2.55e-6); row sums at most 0.16 of their gate
+# The kernel gates E_ABS, ROWSUM_REL, LOSS_REL and G_REL live in simreg_oracle (shared with the per-call
+# checks of bench_call_oracle.py), with what was measured against them.
+E_ABS, ROWSUM_REL, LOSS_REL, G_REL = SR.E_ABS, SR.ROWSUM_REL, SR.LOSS_REL, SR.G_REL
 # ContrastiveLossFn with the term (w = 300, B 2..4096) against fp64: loss rel measured at most 6.4e-6,
 # latent gradient rel error norm 3.6e-3 (at B = 2; two bf16 roundings as in test_gpu_nce_loss), d
 # temperature rel 7.7e-5

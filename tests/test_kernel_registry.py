@@ -1,21 +1,30 @@
 """Every public wrapper of x_clip_b200.kernels has an fp64 per-call check in bench_call_oracle.CHECKS, or is
-a host helper that launches nothing, or is listed with the reason no bench workload reaches it.  A new
-wrapper fails here until it is one of the three.  Runs without a GPU."""
+a host helper that launches nothing.  A new wrapper fails here until it is one of the two.  Runs without
+a GPU."""
+import inspect
+
 import bench_call_oracle as BC
 
 
 def test_every_wrapper_is_checked_or_listed():
+    """Listed: a host helper, with the reason it launches nothing."""
     from x_clip_b200 import kernels
     names = set(BC.public_wrappers(kernels))
-    groups = {"checked": set(BC.CHECKS), "host helper": set(BC.HOST_HELPERS), "not reached": set(BC.NOT_REACHED)}
-    for a in groups:
-        for b in groups:
-            assert a == b or not (groups[a] & groups[b]), (a, b, groups[a] & groups[b])
-    listed = set().union(*groups.values())
-    assert not (names - listed), f"kernels wrappers with no fp64 check and no reason: {sorted(names - listed)}"
+    checked, helpers = set(BC.CHECKS), set(BC.HOST_HELPERS)
+    assert not (checked & helpers), checked & helpers
+    listed = checked | helpers
+    assert not (names - listed), f"kernels wrappers with no fp64 check: {sorted(names - listed)}"
     assert not (listed - names), f"listed names that are not kernels wrappers: {sorted(listed - names)}"
-    for name, why in {**BC.HOST_HELPERS, **BC.NOT_REACHED}.items():
+    for name, why in BC.HOST_HELPERS.items():
         assert why.strip() and "\n" not in why, name
+    assert not hasattr(BC, "NOT_REACHED")
+
+
+def test_no_check_skips_a_variant():
+    """A check returns its ratios for every call: none has a path that returns None."""
+    for name, c in BC.CHECKS.items():
+        src = inspect.getsource(c.check)
+        assert "return None" not in src, name
 
 
 def test_reduction_gates_grow_with_the_rows():
